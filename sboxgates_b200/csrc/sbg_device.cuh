@@ -238,6 +238,14 @@ __device__ __forceinline__ int clz_nonzero(uint32_t x) {
   return c;
 }
 
+// Each byte of x replaced by its top bit spread over the whole byte (0x00 or 0xff), in one PRMT:
+// selector nibbles with the high bit set replicate the sign of the selected byte.
+__device__ __forceinline__ uint32_t prmt_sign_bytes(uint32_t x) {
+  uint32_t d;
+  asm("prmt.b32 %0, %1, 0, 0xba98;" : "=r"(d) : "r"(x));
+  return d;
+}
+
 // Shared-memory load from a 32-bit shared-window address (one address instruction in the caller).
 __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) {
   uint32_t v;
@@ -813,13 +821,16 @@ __device__ __forceinline__ void unrank_weighted_warp(uint32_t t, int np,
 // first g (= window base 6 .. n-1), a copy of the rows shifted down to it (31 gates per word, the
 // target bit on top; (n - 6) * m words of shared memory, built once at the start of the kernel); one
 // word per position then covers every candidate of nearly every prefix and the position loop does
-// half the accumulates.  Windows with <= 15 gates use the PACKED form (see the cell loop).
+// half the accumulates.  A chunk's windows start at the smallest candidate g of its live lanes, so
+// they are often much shorter than the prefix's range: windows with <= 15 gates use the PACKED form
+// and windows with <= 7 gates the QUAD form (see the cell loop).
 // CTAs per SM the register allocation aims at: 3 for the shifted-window form (about 80 registers,
 // against 2 CTAs with about 113; the gain measured for 3 was small, and it has not been re-measured
 // on the H100), 2 for the two-word forms of larger n (a cap of 80 spills there).
 #ifndef SBG_FILTER_MIN_CTAS
 #define SBG_FILTER_MIN_CTAS (SH ? 3 : 2)
 #endif
+constexpr int kQuadGates = 7;   // QUAD windows: 7 candidate gates + the target bit per byte
 template <int NW, int W, int P, bool FS, bool SH = false>
 __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(const DevProblem *__restrict__ prob,
     DevCtl *__restrict__ ctl, uint64_t *__restrict__ hits, uint64_t *__restrict__ aux,
@@ -869,9 +880,10 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
   const uint32_t sxt_top = (uint32_t)__cvta_generic_to_shared(sxt + 31);   // row 31 of base 6
   const uint32_t xr_base = (uint32_t)__cvta_generic_to_shared(s_xr);
   const uint32_t neg_row_bytes = 0u - (uint32_t)ngw * 4u;   // one multiply-add per address
-  // 0x7fffffff held in a register: as a literal the compiler re-creates it at every position
-  // (max_warps is never negative; the arithmetic only hides the constant from constant folding)
-  const uint32_t low31 = 0x7fffffffu ^ ((uint32_t)max_warps >> 31);
+  // 0x7fffffff held in a register: as a literal the compiler re-creates it at every position, and
+  // as a warp-uniform value it copies it from a uniform register at every position (max_warps is
+  // never negative; the arithmetic only hides the constant from constant folding and uniformity)
+  const uint32_t low31 = 0x7fffffffu ^ (((uint32_t)max_warps >> 31) & (uint32_t)lane);
 
   if (chain_is_over(ctl) || volatile_load32(&ctl->skip7) != 0) return;
   // position-major rows: 8-byte cp.async chunks, one row per warp at a time (no division); they
@@ -889,15 +901,19 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
   stage_tables(s_tabs, prob, NW, npad);
   if constexpr (SH) {
     // Window `base` = gates base .. base+30 in bits 0..30 and the row's target bit on top -- or, where
-    // at most packed_gates gates remain (PACKED, below), 15 gates + the target bit, twice over.
+    // at most packed_gates gates remain (PACKED, below), 15 gates + the target bit, twice over; or,
+    // where at most kQuadGates remain as well (QUAD), 7 gates + the target bit, four times over.
     for (int base = 6 + warp; base < n; base += kWarpsPerCta) {
       const bool packed_b = n - base <= packed_gates;
+      const bool quad_b = packed_b && n - base <= kQuadGates;
       for (int pp = lane; pp < m; pp += 32) {
         const uint32_t lo = s_xr[pp * ngw], hi = s_xr[pp * ngw + 1];
         const uint32_t tb = (n <= 31 ? lo : hi) & 0x80000000u;   // the row's target bit
         const uint32_t v = base < 32 ? __funnelshift_r(lo, hi, base) : (hi >> (base - 32));
         const uint32_t half = (v & 0x7fffu) | (tb >> 16);
-        sxt[(base - 6) * m + pp] = packed_b ? (half | (half << 16)) : ((v & 0x7fffffffu) | tb);
+        const uint32_t quarter = (v & 0x7fu) | (tb >> 24);
+        sxt[(base - 6) * m + pp] = quad_b ? quarter * 0x01010101u
+            : packed_b ? (half | (half << 16)) : ((v & 0x7fffffffu) | tb);
       }
     }
     __syncthreads();
@@ -1090,6 +1106,7 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
       const int mc = __popc(mixed_ballot);
 #ifdef SBG_COUNT_FILTER
       unsigned long long dbg_chunks = 0, dbg_windows = 0, dbg_cells = 0, dbg_pos = 0, dbg_packed = 0;
+      unsigned long long dbg_quad = 0;
       unsigned long long dbg_mc = (unsigned long long)mc;
 #endif
 
@@ -1128,8 +1145,15 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         // (once per cell and word) instead of living in 2 x NW registers across the whole chunk
         const uint32_t *tab_e = s_tabs + ge, *tab_f = s_tabs + gf;
         // windows of 32*W candidate gates g, from the first that can hold the smallest possible g
-        // (SH: windows of 31 gates starting AT the smallest possible g, wb counts them)
-        const int first_g = last + (K - P);
+        // (SH: windows of 31 gates starting AT the chunk's smallest candidate g, wb counts them)
+        int first_g = last + (K - P);
+        if constexpr (SH) {
+          // a lane needs only g > f: the chunk's windows start at the lowest gf + 1 of its live lanes
+          // (often well above the prefix's last + 3), so that more of them take the packed forms
+          const uint32_t lo = __reduce_min_sync(kFull, lane_ok ? (uint32_t)(gf + 1) : (uint32_t)n);
+          if (lo >= (uint32_t)n) continue;   // no live lane: nothing to test or emit
+          first_g = (int)lo;
+        }
         const int wb0 = SH ? 0 : ((first_g >> 5) & ~(W - 1));
         int nvw = 0;      // words of surviving-g vectors stored for this chunk
         bool chunk_live = false;   // some lane kept a candidate in some window
@@ -1138,7 +1162,9 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
           // PACKED (SH only): a window with at most 15 candidate last gates keeps TWO parts in one
           // accumulator register -- halves of 15 gates + the target bit each, the shifted rows stored
           // twice over -- so a position costs 2 part masks + 4 accumulates instead of 4 + 8.
+          // QUAD: at most 7 candidates, all FOUR parts in one register, a byte each: 2 + 2.
           const bool packed = SH && n - base <= packed_gates;   // 15, or 0 = never
+          const bool quad = packed && n - base <= kQuadGates;
           const uint32_t sx_top = sxt_top + (uint32_t)((base - 6) * m) * 4u;
           uint32_t V[W];
           if constexpr (SH) {
@@ -1165,7 +1191,8 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
           for (int j = 0; j < W; j++) alive |= V[j] != 0;
 #ifdef SBG_COUNT_FILTER
           dbg_windows++;
-          if (packed) dbg_packed++;
+          if (packed && !quad) dbg_packed++;
+          if (quad) dbg_quad++;
 #endif
           bool any_alive = __any_sync(kFull, alive);
           for (int cj = 0; cj < mc && any_alive; cj++) {
@@ -1174,6 +1201,37 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
             for (int w = 0; w < NW; w++) dbg_pos += __popc(cells[cj * NW + w]);
 #endif
             if constexpr (SH) {
+              if (quad) {
+                // part 2e + f in byte 2e + f of (aq, oq): e picks the half, f the byte within it
+                uint32_t aq = 0xffffffffu, oq = 0u;
+#pragma unroll
+                for (int w = 0; w < NW; w++) {
+                  uint32_t bits = cells[cj * NW + w];
+                  const uint32_t tf_w = tab_f[w * npad];
+                  const uint32_t te_w = tab_e[w * npad];
+                  while (bits != 0) {
+                    const int c = clz_nonzero(bits);
+                    bits &= low31 >> c;
+                    const uint32_t fb = (uint32_t)((int32_t)(tf_w << c) >> 31);
+                    const uint32_t eb = (uint32_t)((int32_t)(te_w << c) >> 31);
+                    const uint32_t x = lds_u32(sx_top + (uint32_t)(w * 128) - 4u * (uint32_t)c);
+                    const uint32_t mq = lop3<0x60>(eb ^ 0x0000ffffu, fb, 0x00ff00ffu);   // a & (b ^ c)
+                    aq = lop3<0xd0>(aq, x, mq);
+                    oq = lop3<0xf8>(oq, x, mq);
+                  }
+                }
+                // per byte: admissible g = constant over the part, or the part lacks a target value
+                // (bit 7 of a byte: OR = some target 1 seen, AND = only target 1 seen); the sign
+                // of each byte of z spread over the byte, then the four bytes ANDed into the low one
+                uint32_t t = prmt_sign_bytes(oq & ~aq);
+                t = aq | ~oq | ~t;
+                t &= t >> 16;
+                t &= t >> 8;
+                V[0] &= t;
+                alive = V[0] != 0;
+                any_alive = __any_sync(kFull, alive);
+                continue;
+              }
               if (packed) {
                 // parts 0 | 1 in the low | high half of (and01, or01), parts 2 | 3 of (and23, or23)
                 uint32_t and01 = 0xffffffffu, or01 = 0u, and23 = 0xffffffffu, or23 = 0u;
@@ -1366,6 +1424,7 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         atomicAdd(&ctl->pad1[4], dbg_pos);
         atomicAdd(&ctl->pad1[5], dbg_packed);
         atomicAdd(&ctl->pad1[6], dbg_mc);
+        atomicAdd(&ctl->pad1[7], dbg_quad);
       }
 #endif
     }
@@ -1402,10 +1461,11 @@ __global__ void __launch_bounds__(256) k_offsets(DevCtl *__restrict__ ctl,
         + min(volatile_load(&ctl->hit_count), (unsigned long long)0xffffffffu);
     ctl->list_count = (unsigned int)min(total, (unsigned long long)list_cap);
 #ifdef SBG_COUNT_FILTER
-    printf("F1 prefixes %llu chunks %llu windows %llu cells %llu positions %llu packed %llu mixed %llu hits %llu\n",
+    // windows = single (31 gates) + packed (two parts of 15) + quad (four parts of 7)
+    printf("F1 prefixes %llu chunks %llu windows %llu cells %llu positions %llu packed %llu mixed %llu hits %llu quad %llu\n",
         ctl->pad1[0], ctl->pad1[1], ctl->pad1[2], ctl->pad1[3], ctl->pad1[4], ctl->pad1[5],
-        ctl->pad1[6], ctl->hit_count);
-    for (int i = 0; i < 7; i++) ctl->pad1[i] = 0;
+        ctl->pad1[6], ctl->hit_count, ctl->pad1[7]);
+    for (int i = 0; i < 8; i++) ctl->pad1[i] = 0;
 #endif
   }
   if (first >= handed) return;
