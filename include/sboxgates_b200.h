@@ -197,6 +197,49 @@ int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_o
 int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
     const uint8_t *middle_order, sbg_result *res);
 
+/* ---- enumeration: every match, not only the first -------------------------------------------- */
+/* The matches of search_5lut / search_7lut are the keys (as in sbg_result::key, so ascending key
+   order is the reference's enumeration order) of the candidates that get_lut_function accepts
+   without its random fill (lut.c:79-103), after the inbits rejection (lut.c:177-185) and
+   check_n_lut_possible (lut.c:34-66):
+     5-LUT: rank<<12 | k<<8 | pos over all combinations of C(n,5);
+     7-LUT: idx<<23 | k<<16 | po<<8 | pm over the phase-1 list (the first SBG_LIST_CAP feasible
+            7-combinations in lexicographic order), decided on the TRUE gate tables.  The reference's
+            stale outer cache (lut.c:432-435, sbg_result::stale_outer) is not reproduced; it can only
+            act on a list entry whose first gate is 0, so where inbits excludes gate 0 the smallest
+            7-LUT match is the key sbg_search7 returns.
+   One record per match, decoded on the device; nothing consumes the caller's RNG (the random fill
+   of func_inner's don't-care bits stays with the caller, as for sbg_result).  32 bytes: */
+typedef struct {
+  uint64_t key;            /* offset 0 */
+  uint16_t gates[7];       /* 8: LUT inputs in reference order a..e (5-LUT; then 0) or a..g */
+  uint8_t func_outer;      /* 22: the function at position (key >> 8) & 0xff of the outer order */
+  uint8_t func_middle;     /* 23: 7-LUT: the function at position key & 0xff of the middle order */
+  uint8_t func_inner;      /* 24: solved bits only; don't-care bits are 0 */
+  uint8_t inner_seen;      /* 25: bit c set = inner cell c occurs under the mask */
+  uint8_t width;           /* 26: 5 or 7 */
+  uint8_t pad[5];          /* 27: 0 */
+} sbg_match;
+#define SBG_ENUM_MAX_MATCHES (1u << 24)   /* largest max_matches of one call */
+
+/* Enumerates the matches of the current problem in this part's share of the work (part/nparts as
+   for sbg_search5_part / sbg_decomp7_part: the parts' totals add up to the whole, and merging their
+   first-K lists and cutting at K gives the whole's first K).  Writes the first
+   n = min(max_matches, matches) of them, in ascending key order, to out[0..n-1] and n to *n_out.
+   total != NULL: *total = the exact number of matches of the share.  total == NULL: the sweep may
+   stop as soon as the first max_matches matches are known (max_matches = 1: a first-match search).
+   *feasible (may be NULL): 5-LUT: feasible combinations met (all of the share's when counting);
+   7-LUT: the length of the list.  max_matches may be 0 (counting only), at most
+   SBG_ENUM_MAX_MATCHES.  The match and count buffers are allocated on the first call. */
+int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, uint64_t max_matches,
+    sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible);
+/* The 7-LUT list: the one installed for the current problem (sbg_set_list7 / sbg_set_list7_device /
+   sbg_allgather_merge7, sbg_filter7_part with nparts == 1, or an earlier sbg_search7 of it), else
+   phase 1 runs here over the whole space and its list stays installed. */
+int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
+    const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
+    uint64_t *total, uint64_t *feasible);
+
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense
    states").  width = 7 with prefix_gates = 4 or 5 (search_7lut phase 1), width = 5 with

@@ -9,12 +9,14 @@ does not.
 """
 from .rng import Xorshift1024
 from .lut import LutEngine, SearchResult, NO_GATE, search_5lut, search_7lut, shuffled_order, \
-    shuffled_orders7, ordering_row, solve_inner, lut_table, lut_search, LutSearchResult
-from .native import load_library, NativeLibraryError
+    shuffled_orders7, ordering_row, solve_inner, lut_table, lut_search, LutSearchResult, \
+    Enumeration, enumerate_5lut, enumerate_7lut, match_to_ret, decode_key5, decode_key7
+from .native import load_library, NativeLibraryError, MATCH_DTYPE
 
 __all__ = [
     "Xorshift1024", "LutEngine", "SearchResult", "NO_GATE", "search_5lut", "search_7lut",
     "shuffled_order", "shuffled_orders7", "ordering_row", "solve_inner", "lut_table",
-    "lut_search", "LutSearchResult",
+    "lut_search", "LutSearchResult", "Enumeration", "enumerate_5lut", "enumerate_7lut",
+    "match_to_ret", "decode_key5", "decode_key7", "MATCH_DTYPE",
     "load_library", "NativeLibraryError",
 ]

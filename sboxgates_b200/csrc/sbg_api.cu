@@ -136,6 +136,12 @@ struct sbg_lane {
   float ms[4] = {0, 0, 0, 0};
   uint64_t last_key = SBG_KEY_NONE;   // sbg_decomp7_part's result and the two list entries behind it
   uint64_t last_tuple = 0, last_tuple_prev = 0;
+  // enumeration (sbg_enum5 / sbg_enum7; allocated on the first call)
+  EnumCtl *d_ectl = nullptr;
+  uint32_t *d_ecount = nullptr;             // matches per ticket
+  unsigned long long *d_eoffset = nullptr;  // their exclusive prefix sum
+  DevMatch *d_ematch = nullptr;             // the emitted records
+  uint64_t ecount_cap = 0, ematch_cap = 0;
 };
 
 struct sbg_handle {
@@ -1342,6 +1348,145 @@ int finish7_slot(sbg_handle *h, const sbg_handle::HostProblem &hp, uint64_t key,
   return SBG_OK;
 }
 
+// ---- enumeration (sbg_enum5 / sbg_enum7) -------------------------------------------------------
+
+static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
+    && offsetof(sbg_match, gates) == offsetof(DevMatch, gates)
+    && offsetof(sbg_match, func_outer) == offsetof(DevMatch, func_outer)
+    && offsetof(sbg_match, inner_seen) == offsetof(DevMatch, inner_seen)
+    && offsetof(sbg_match, width) == offsetof(DevMatch, width), "sbg_match and DevMatch agree");
+
+// Count-free windows start at this many tickets and double: a first-match search then costs a few
+// windows of work past the first match, a search without one about twice the counting sweep's
+// launches (log2 of the tickets) and no more work.
+constexpr uint64_t kEnumWindow5 = kNominalWarps;
+constexpr uint64_t kEnumWindow7 = kNominalWarps / 4;
+
+int ensure_enum(sbg_handle *h, sbg_lane &L, uint64_t tickets, uint64_t matches) {
+  if (L.d_ectl == nullptr) SBG_CUDA(h, cudaMalloc(&L.d_ectl, sizeof(EnumCtl)));
+  if (L.ecount_cap < tickets) {
+    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+    cudaFree(L.d_ecount);
+    cudaFree(L.d_eoffset);
+    L.d_ecount = nullptr;
+    L.d_eoffset = nullptr;
+    L.ecount_cap = 0;
+    SBG_CUDA(h, cudaMalloc(&L.d_ecount, tickets * sizeof(uint32_t)));
+    SBG_CUDA(h, cudaMalloc(&L.d_eoffset, tickets * sizeof(unsigned long long)));
+    L.ecount_cap = tickets;
+  }
+  if (L.ematch_cap < matches) {
+    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+    cudaFree(L.d_ematch);
+    L.d_ematch = nullptr;
+    L.ematch_cap = 0;
+    SBG_CUDA(h, cudaMalloc(&L.d_ematch, matches * sizeof(DevMatch)));
+    L.ematch_cap = matches;
+  }
+  return SBG_OK;
+}
+
+// One enumeration pass (count or emit) over tickets [a, b) of the lane's problem.
+template <bool SEVEN, bool EMIT>
+int launch_enum(sbg_handle *h, sbg_lane &L, const EnumOrders &ord, int part, int nparts,
+    uint64_t max_out, uint64_t a, uint64_t b) {
+  const sbg_handle::HostProblem &hp = h->slots[L.slot];
+  const int n = hp.n;
+  cudaError_t e = cudaSuccess;
+  int rc = SBG_OK;
+#define SBG_LAUNCH_ENUM(NWV)                                                                   \
+  {                                                                                            \
+    if (SEVEN) {                                                                               \
+      const size_t smem = decomp_smem<NWV>(n);                                                 \
+      auto kern = k_enum7<NWV, EMIT>;                                                          \
+      if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
+      e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
+          h->d_slots + L.slot, L.d_ectl, ord, (const uint64_t *)L.d_sorted,                    \
+          (unsigned int)L.list_count, L.d_ecount, (const unsigned long long *)L.d_eoffset,     \
+          L.d_ematch, (unsigned long long)max_out, (unsigned long long)a,                      \
+          (unsigned long long)b, part, nparts, (const DevTables *)h->d_tab);                   \
+    } else {                                                                                   \
+      const size_t smem = sweep_smem<NWV>(n);                                                  \
+      auto kern = k_enum5<NWV, EMIT>;                                                          \
+      if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
+      e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
+          h->d_slots + L.slot, L.d_ectl, ord, L.d_ecount,                                      \
+          (const unsigned long long *)L.d_eoffset, L.d_ematch, (unsigned long long)max_out,    \
+          (unsigned long long)a, (unsigned long long)b, part, nparts,                          \
+          (const DevTables *)h->d_tab);                                                        \
+    }                                                                                          \
+  }
+  switch (hp.nw) {
+    case 1: SBG_LAUNCH_ENUM(1) break;
+    case 2: SBG_LAUNCH_ENUM(2) break;
+    case 4: SBG_LAUNCH_ENUM(4) break;
+    default: SBG_LAUNCH_ENUM(8) break;
+  }
+#undef SBG_LAUNCH_ENUM
+  if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "enumeration launch: %s", cudaGetErrorString(e));
+  if (!EMIT) {
+    e = launch(h, k_enum_scan, 1, 1024, 0, L.stream, false, L.d_ectl, (const uint32_t *)L.d_ecount,
+        L.d_eoffset, (unsigned long long)a, (unsigned long long)b);
+    if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_scan: %s", cudaGetErrorString(e));
+  }
+  return SBG_OK;
+}
+
+// Count pass (in windows when only the first max_matches are wanted), offsets, emit pass, copy-out.
+// The lane's problem is prepared on the device.
+template <bool SEVEN>
+int run_enum(sbg_handle *h, sbg_lane &L, const EnumOrders &ord, int part, int nparts,
+    uint64_t tickets, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
+    uint64_t *feasible) {
+  int rc;
+  if ((rc = ensure_enum(h, L, std::max<uint64_t>(tickets, 1), 0)) != SBG_OK) return rc;
+  SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
+  const bool count_all = total != nullptr;
+  uint64_t window = count_all ? tickets : (SEVEN ? kEnumWindow7 : kEnumWindow5);
+  uint64_t done = 0;
+  EnumCtl ec;
+  memset(&ec, 0, sizeof(ec));
+  while (done < tickets) {
+    const uint64_t end = std::min(tickets, done + window);
+    if ((rc = launch_enum<SEVEN, false>(h, L, ord, part, nparts, 0, done, end)) != SBG_OK) return rc;
+    done = end;
+    window *= 2;
+    if (!count_all) {
+      // ordered stop: every later ticket holds larger keys only
+      SBG_CUDA(h, cudaMemcpyAsync(&ec, L.d_ectl, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
+      SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+      if (ec.carry >= max_matches) break;
+    }
+  }
+  SBG_CUDA(h, cudaMemcpyAsync(&ec, L.d_ectl, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  const uint64_t emit = std::min<uint64_t>(max_matches, ec.carry);
+  if (emit > 0) {
+    if ((rc = ensure_enum(h, L, 0, emit)) != SBG_OK) return rc;
+    if ((rc = launch_enum<SEVEN, true>(h, L, ord, part, nparts, emit, 0, done)) != SBG_OK) return rc;
+    SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, emit * sizeof(sbg_match), cudaMemcpyDeviceToHost,
+        L.stream));
+    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+    h->d2h_bytes += emit * sizeof(sbg_match);
+  }
+  *n_out = emit;
+  if (total != nullptr) *total = ec.carry;
+  if (feasible != nullptr) *feasible = SEVEN ? (uint64_t)L.list_count : ec.feasible;
+  return SBG_OK;
+}
+
+int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, sbg_match *out,
+    uint64_t *n_out) {
+  if (n_out == nullptr || (max_matches > 0 && out == nullptr)) return fail(h, SBG_ERR_ARG, "null output");
+  if (max_matches > SBG_ENUM_MAX_MATCHES) {
+    return fail(h, SBG_ERR_ARG, "max_matches %llu above %u", (unsigned long long)max_matches,
+        SBG_ENUM_MAX_MATCHES);
+  }
+  if (nparts < 1 || part < 0 || part >= nparts) return fail(h, SBG_ERR_ARG, "bad part %d/%d", part, nparts);
+  if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
+  return SBG_OK;
+}
+
 // LOP3 issue-rate microbenchmark (sbg_alu_peak): CHAINS independent dependent chains per thread.
 template <int CHAINS>
 __global__ void k_lop3_peak(uint32_t *out, int iters, uint32_t seed) {
@@ -1645,6 +1790,11 @@ int sbg_create(sbg_handle **out, int device) {
     SBG_CUDA(h, cudaMemcpyToSymbol(c_j_first_k, first_k, sizeof(first_k)));
     SBG_CUDA(h, cudaMemcpyToSymbol(c_j_rows, nrows, sizeof(nrows)));
     SBG_CUDA(h, cudaMemcpyToSymbol(c_row_b, row_b, sizeof(row_b)));
+    uint8_t rows5[10][5], rows7[70][7];
+    for (int k = 0; k < 10; k++) for (int i = 0; i < 5; i++) rows5[k][i] = (uint8_t)h_rows5[k][i];
+    for (int k = 0; k < 70; k++) for (int i = 0; i < 7; i++) rows7[k][i] = (uint8_t)h_rows7[k][i];
+    SBG_CUDA(h, cudaMemcpyToSymbol(c_rows5, rows5, sizeof(rows5)));
+    SBG_CUDA(h, cudaMemcpyToSymbol(c_rows7, rows7, sizeof(rows7)));
   }
 
   stamp("constant tables");
@@ -1669,6 +1819,7 @@ void sbg_destroy(sbg_handle *h) {
       cudaFree(L.d_ctl); cudaFree(L.d_par7); cudaFree(L.d_pos5); cudaFree(L.d_order3);
       cudaFree(L.d_hits); cudaFree(L.d_aux); cudaFree(L.d_sorted);
       cudaFree(L.d_tcount); cudaFree(L.d_toffset); cudaFree(L.d_gcount);
+      cudaFree(L.d_ectl); cudaFree(L.d_ecount); cudaFree(L.d_eoffset); cudaFree(L.d_ematch);
       if (L.h_out != nullptr) cudaFreeHost(L.h_out);
       if (L.h_ctl != nullptr) cudaFreeHost(L.h_ctl);
       for (int k = 0; k < 8; k++) if (L.ev[k] != nullptr) cudaEventDestroy(L.ev[k]);
@@ -2155,6 +2306,63 @@ int sbg_search7(sbg_handle *h, const uint8_t *outer_order, const uint8_t *middle
   if (rc != SBG_OK) return rc;
   *res = nr.r7;
   return SBG_OK;
+}
+
+int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, uint64_t max_matches,
+    sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  int rc;
+  if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
+  const sbg_handle::HostProblem &hp = cur(h);
+  if (hp.n < 5) return fail(h, SBG_ERR_ARG, "search_5lut needs n >= 5 (lut.c:119)");
+  if (!valid_order(func_order)) return fail(h, SBG_ERR_ARG, "func_order is not a permutation");
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
+  L.seq++;
+  CallInputs in;
+  in.order5 = func_order;
+  if ((rc = enqueue_begin(h, L, kBeginSearch5, in, 0)) != SBG_OK) return rc;
+  // this part's tickets: its deal blocks of kDeal prefixes (the last one may be cut short)
+  const uint64_t blocks = (h_binom[hp.n - 2][3] + kDeal - 1) / kDeal;
+  const uint64_t mine = blocks > (uint64_t)part ? (blocks - part + nparts - 1) / nparts : 0;
+  EnumOrders ord;
+  memcpy(ord.order[0], func_order, 256);
+  memset(ord.order[1], 0, 256);
+  return run_enum<false>(h, L, ord, part, nparts, mine * kDeal, max_matches, out, n_out, total,
+      feasible);
+}
+
+int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
+    const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
+    uint64_t *total, uint64_t *feasible) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  int rc;
+  if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
+  if (cur(h).n < 7) return fail(h, SBG_ERR_ARG, "search_7lut needs n >= 7 (lut.c:259)");
+  if (!valid_order(outer_order) || !valid_order(middle_order)) {
+    return fail(h, SBG_ERR_ARG, "function order is not a permutation");
+  }
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
+  if (L.list_ready) {
+    // the installed list: only bring the problem block up to date
+    L.seq++;
+    CallInputs none;
+    if ((rc = enqueue_begin(h, L, kBeginKeepCtl, none, 0)) != SBG_OK) return rc;
+  } else {
+    uint32_t count = 0;
+    if ((rc = run_filter7(h, L, 0, 1, &count)) != SBG_OK) return rc;
+    L.list_count = count;
+    L.list_ready = true;
+  }
+  const uint64_t count = L.list_count;
+  const uint64_t mine = count > (uint64_t)part ? (count - part + nparts - 1) / nparts : 0;
+  EnumOrders ord;
+  memcpy(ord.order[0], outer_order, 256);
+  memcpy(ord.order[1], middle_order, 256);
+  return run_enum<true>(h, L, ord, part, nparts, mine, max_matches, out, n_out, total, feasible);
 }
 
 }  // extern "C"

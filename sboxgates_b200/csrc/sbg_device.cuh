@@ -339,10 +339,11 @@ __device__ __forceinline__ void close_stage(DevCtl *ctl, HostOut *out, int stage
 // 1 / a masked 0 of the target).  Returns the first (ordering, position in the shuffled function
 // order) that decomposes, as k<<8 | pos, or 0xffffffff.
 
+// The tuple's 32-cell summary (lane = cell, first gate = most significant bit): bit l of H1 / H0 is
+// set iff cell l holds a masked position with target 1 / 0.
 template <int NW>
-__device__ __forceinline__ uint32_t decomp5_tuple(const uint32_t *s_tabs, int npad, const int *g,
-    const uint32_t *T, const uint32_t *M, int lane, const uint8_t *s_pos,
-    const DevTables *__restrict__ tab) {
+__device__ __forceinline__ void summary5(const uint32_t *s_tabs, int npad, const int *g,
+    const uint32_t *T, const uint32_t *M, int lane, uint32_t &H1, uint32_t &H0) {
   uint32_t ones = 0, zeros = 0;
 #pragma unroll
   for (int w = 0; w < NW; w++) {
@@ -355,30 +356,45 @@ __device__ __forceinline__ uint32_t decomp5_tuple(const uint32_t *s_tabs, int np
     ones |= tt & T[w];
     zeros |= tt & ~T[w];
   }
-  const uint32_t H1 = __ballot_sync(kFull, ones != 0);
-  const uint32_t H0 = __ballot_sync(kFull, zeros != 0);
-  for (int k = 0; k < 10; k++) {
-    const int s = tab->src5[k][lane];
-    const uint32_t b1 = __ballot_sync(kFull, (H1 >> s) & 1u);
-    const uint32_t b0 = __ballot_sync(kFull, (H0 >> s) & 1u);
-    // wv(u): bits 0-3 = inner cells (x, d, e) with a masked 1 contributed by outer pattern u,
-    // bits 4-7 = the same for masked 0.
+  H1 = __ballot_sync(kFull, ones != 0);
+  H0 = __ballot_sync(kFull, zeros != 0);
+}
+
+// Ordering k of a tuple with summary H1 / H0: ok[hi] bit lane and ok[7 - hi] bit 31 - lane both
+// set <=> outer function hi*32+lane decomposes.
+__device__ __forceinline__ void outer_ok5(uint32_t H1, uint32_t H0, int k, int lane,
+    const DevTables *__restrict__ tab, uint32_t *ok) {
+  const int s = tab->src5[k][lane];
+  const uint32_t b1 = __ballot_sync(kFull, (H1 >> s) & 1u);
+  const uint32_t b0 = __ballot_sync(kFull, (H0 >> s) & 1u);
+  // wv(u): bits 0-3 = inner cells (x, d, e) with a masked 1 contributed by outer pattern u,
+  // bits 4-7 = the same for masked 0.
 #define SBG_W5(u) (((b1 >> (4 * (u))) & 0xfu) | (((b0 >> (4 * (u))) & 0xfu) << 4))
-    uint32_t L = 0;
+  uint32_t L = 0;
 #pragma unroll
-    for (int u = 0; u < 5; u++) {
-      if ((lane >> u) & 1) L |= SBG_W5(u);
-    }
-    uint32_t ok[8];
+  for (int u = 0; u < 5; u++) {
+    if ((lane >> u) & 1) L |= SBG_W5(u);
+  }
 #pragma unroll
-    for (int hi = 0; hi < 8; hi++) {
-      uint32_t rr = L;
-      if (hi & 1) rr |= SBG_W5(5);
-      if (hi & 2) rr |= SBG_W5(6);
-      if (hi & 4) rr |= SBG_W5(7);
-      ok[hi] = __ballot_sync(kFull, ((rr & (rr >> 4)) & 0xfu) == 0);
-    }
+  for (int hi = 0; hi < 8; hi++) {
+    uint32_t rr = L;
+    if (hi & 1) rr |= SBG_W5(5);
+    if (hi & 2) rr |= SBG_W5(6);
+    if (hi & 4) rr |= SBG_W5(7);
+    ok[hi] = __ballot_sync(kFull, ((rr & (rr >> 4)) & 0xfu) == 0);
+  }
 #undef SBG_W5
+}
+
+template <int NW>
+__device__ __forceinline__ uint32_t decomp5_tuple(const uint32_t *s_tabs, int npad, const int *g,
+    const uint32_t *T, const uint32_t *M, int lane, const uint8_t *s_pos,
+    const DevTables *__restrict__ tab) {
+  uint32_t H1, H0;
+  summary5<NW>(s_tabs, npad, g, T, M, lane, H1, H0);
+  for (int k = 0; k < 10; k++) {
+    uint32_t ok[8];
+    outer_ok5(H1, H0, k, lane, tab, ok);
     // Outer function fo = hi*32+lane maps pattern u to x = bit u of fo; it works iff neither
     // {u: x=1} nor {u: x=0} merges a masked 1 and a masked 0 into one inner cell.
     uint32_t best_pos = 256;
@@ -2041,6 +2057,78 @@ __device__ __forceinline__ uint32_t triples_with_colourings(const uint32_t *sH, 
   return __ballot_sync(kFull, lane < 25 && (v[0] | v[1] | v[2] | v[3]) != 0);
 }
 
+// Phase 2, stage 1 for outer triple j of a tuple with summary Hs (srcw = DevTables::src7[j][lane]):
+// W[u] = low half: the 16 cells (over the four non-outer gates) in which outer pattern u holds a
+// masked 1, high half: the same for a masked 0; ok[hi] bit lane and ok[7 - hi] bit 31 - lane both
+// set <=> outer function hi*32+lane leaves a conflict-free 5-input remainder.
+__device__ __forceinline__ void outer_ok7(const uint32_t *Hs, uint32_t srcw, int lane, uint32_t *W,
+    uint32_t *ok) {
+  uint32_t P1[4], P0[4];
+#pragma unroll
+  for (int t4 = 0; t4 < 4; t4++) {
+    const uint32_t c = (srcw >> (8 * t4)) & 0x7fu;
+    P1[t4] = __ballot_sync(kFull, (Hs[c >> 5] >> (c & 31u)) & 1u);
+    P0[t4] = __ballot_sync(kFull, (Hs[4 + (c >> 5)] >> (c & 31u)) & 1u);
+  }
+#pragma unroll
+  for (int u = 0; u < 8; u++) {
+    W[u] = ((P1[u >> 1] >> (16 * (u & 1))) & 0xffffu)
+        | (((P0[u >> 1] >> (16 * (u & 1))) & 0xffffu) << 16);
+  }
+  uint32_t L = 0;
+#pragma unroll
+  for (int u = 0; u < 5; u++) {
+    if ((lane >> u) & 1) L |= W[u];
+  }
+#pragma unroll
+  for (int hi = 0; hi < 8; hi++) {
+    uint32_t rr = L;
+    if (hi & 1) rr |= W[5];
+    if (hi & 2) rr |= W[6];
+    if (hi & 4) rr |= W[7];
+    ok[hi] = __ballot_sync(kFull, ((rr & (rr >> 16)) & 0xffffu) == 0);
+  }
+}
+
+// Stage 2 for one surviving outer function (r1 / r0 = OR of W[u] over the patterns u it sends to 1
+// / 0) and one ordering row (b = bit of v4 that is the g input): the middle functions that work are
+// the union, over the (c0, c1) with hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0,
+// of the cubes { fm : (fm & S) == (hv[0][c0] | hv[1][c1]) }.
+__device__ __forceinline__ void middle_cubes(uint32_t r1, uint32_t r0, int b, uint32_t (*hv)[4],
+    bool (*hok)[4], uint32_t &S, uint32_t &ov) {
+  // The four inner cells (x, g): A = middle patterns with a masked 1, B = with a masked 0
+  // (both compressed at once: they are the two halves of r1 / r0).
+  // If both are non-empty, fm must send A to one value and B to the other: fm & S in {A, B}.
+  uint32_t cs[4], ca[4], cb[4];
+#pragma unroll
+  for (int ci = 0; ci < 4; ci++) {
+    const uint32_t AB = compress16x2((ci & 2) ? r1 : r0, b, ci & 1);
+    const uint32_t A = AB & 0xffu, B = AB >> 16;
+    const bool act = A != 0 && B != 0;
+    cs[ci] = act ? (A | B) : 0u;   // inactive: empty support, both choices identical
+    ca[ci] = act ? A : 0u;
+    cb[ci] = act ? B : 0u;
+  }
+  // Combine constraints 0,1 and 2,3 (4 choices each), then cross the two halves; a
+  // combination is consistent iff its forced values agree wherever supports overlap.
+  uint32_t hs[2];
+#pragma unroll
+  for (int h2 = 0; h2 < 2; h2++) {
+    const int i = 2 * h2;
+    hs[h2] = cs[i] | cs[i + 1];
+    const uint32_t ov2 = cs[i] & cs[i + 1];
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+      const uint32_t v0 = (c & 1) ? cb[i] : ca[i];
+      const uint32_t v1 = (c & 2) ? cb[i + 1] : ca[i + 1];
+      hok[h2][c] = ((v0 ^ v1) & ov2) == 0;
+      hv[h2][c] = v0 | v1;
+    }
+  }
+  S = hs[0] | hs[1];
+  ov = hs[0] & hs[1];
+}
+
 template <int NW>
 __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restrict__ prob,
     DevCtl *__restrict__ ctl, HostOut *__restrict__ out, const DevParams7 *__restrict__ par,
@@ -2140,36 +2228,8 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
     for (int j = 0; j < 25 && !found; j++) {
       if (((pass_i >> j) & 1u) == 0) continue;   // the filter found no admissible outer function
       const uint32_t *Hs = (stale && j == 0) ? sH + 8 : sH;
-      const uint32_t srcw = s_src7[j * 32 + lane];
-      uint32_t P1[4], P0[4];
-#pragma unroll
-      for (int t4 = 0; t4 < 4; t4++) {
-        const uint32_t c = (srcw >> (8 * t4)) & 0x7fu;
-        P1[t4] = __ballot_sync(kFull, (Hs[c >> 5] >> (c & 31u)) & 1u);
-        P0[t4] = __ballot_sync(kFull, (Hs[4 + (c >> 5)] >> (c & 31u)) & 1u);
-      }
-      // W[u]: low half = the 16 cells (over the four non-outer gates) in which outer pattern u
-      // holds a masked 1, high half = the same for a masked 0.
-      uint32_t W[8];
-#pragma unroll
-      for (int u = 0; u < 8; u++) {
-        W[u] = ((P1[u >> 1] >> (16 * (u & 1))) & 0xffffu)
-            | (((P0[u >> 1] >> (16 * (u & 1))) & 0xffffu) << 16);
-      }
-      uint32_t L = 0;
-#pragma unroll
-      for (int u = 0; u < 5; u++) {
-        if ((lane >> u) & 1) L |= W[u];
-      }
-      uint32_t ok[8];
-#pragma unroll
-      for (int hi = 0; hi < 8; hi++) {
-        uint32_t rr = L;
-        if (hi & 1) rr |= W[5];
-        if (hi & 2) rr |= W[6];
-        if (hi & 4) rr |= W[7];
-        ok[hi] = __ballot_sync(kFull, ((rr & (rr >> 16)) & 0xffffu) == 0);
-      }
+      uint32_t W[8], ok[8];
+      outer_ok7(Hs, s_src7[j * 32 + lane], lane, W, ok);
       uint32_t any = 0;
       uint32_t my_surv = 0;
 #pragma unroll
@@ -2217,39 +2277,9 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
         }
 #pragma unroll 1
         for (int row = 0; row < nrows; row++) {
-          const int b = c_row_b[k0 + row];
-          // The four inner cells (x, g): A = middle patterns with a masked 1, B = with a masked 0
-          // (both compressed at once: they are the two halves of r1 / r0).
-          // If both are non-empty, fm must send A to one value and B to the other: fm & S in {A, B}.
-          uint32_t cs[4], ca[4], cb[4];
-#pragma unroll
-          for (int ci = 0; ci < 4; ci++) {
-            const uint32_t AB = compress16x2((ci & 2) ? r1 : r0, b, ci & 1);
-            const uint32_t A = AB & 0xffu, B = AB >> 16;
-            const bool act = A != 0 && B != 0;
-            cs[ci] = act ? (A | B) : 0u;   // inactive: empty support, both choices identical
-            ca[ci] = act ? A : 0u;
-            cb[ci] = act ? B : 0u;
-          }
-          // Combine constraints 0,1 and 2,3 (4 choices each), then cross the two halves; a
-          // combination is consistent iff its forced values agree wherever supports overlap.
-          uint32_t hs[2], hv[2][4];
+          uint32_t hv[2][4], S, ov;
           bool hok[2][4];
-#pragma unroll
-          for (int h2 = 0; h2 < 2; h2++) {
-            const int i = 2 * h2;
-            hs[h2] = cs[i] | cs[i + 1];
-            const uint32_t ov = cs[i] & cs[i + 1];
-#pragma unroll
-            for (int c = 0; c < 4; c++) {
-              const uint32_t v0 = (c & 1) ? cb[i] : ca[i];
-              const uint32_t v1 = (c & 2) ? cb[i + 1] : ca[i + 1];
-              hok[h2][c] = ((v0 ^ v1) & ov) == 0;
-              hv[h2][c] = v0 | v1;
-            }
-          }
-          const uint32_t S = hs[0] | hs[1];
-          const uint32_t ov = hs[0] & hs[1];
+          middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
           const uint32_t p3s = s_p3[S];
           uint32_t best_pm = 256;
 #pragma unroll
@@ -2303,6 +2333,441 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
 #endif
     close_stage(ctl, out, 2, key, ctl->list_count, tuple, tuple_prev);
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Enumeration (sbg_enum5 / sbg_enum7): every match of search_5lut / search_7lut, not only the first.
+// The same decisions as the searches above with nothing thrown away, in two passes over the same
+// tickets -- a 3-gate prefix of C(n,5) (dealt to the parts as k_sweep deals them) or one list entry:
+//   count (EMIT = false): the number of matches of each ticket, and their sum;
+//   k_enum_scan: exclusive prefix sum of those counts = where each ticket's matches start in the
+//     ascending key order;
+//   emit (EMIT = true): the tickets whose matches start below K write them there, in key order,
+//     decoded into DevMatch records.
+// Tickets are numbered in key order, so the order needs no sort.  Both passes run the identical
+// sweep, so a ticket emits exactly the matches it counted.
+
+// The layout of sbg_match (include/sboxgates_b200.h; sbg_api.cu checks that the two agree).
+struct DevMatch {
+  unsigned long long key;
+  uint16_t gates[7];
+  uint8_t func_outer, func_middle, func_inner, inner_seen;
+  uint8_t width;
+  uint8_t pad[5];
+};
+
+struct EnumCtl {
+  unsigned long long total;     // matches counted so far (all windows of the call)
+  unsigned long long feasible;  // 5-LUT: feasible tuples met
+  unsigned long long carry;     // k_enum_scan: matches in front of the next window
+};
+
+struct EnumOrders {
+  uint8_t order[2][256];   // the shuffled function order(s): [0] outer (5-LUT: the only one), [1] middle
+};
+
+__constant__ uint8_t c_rows5[10][5];   // ordering rows (lut.c:189,224-229 and lut.c:396-415)
+__constant__ uint8_t c_rows7[70][7];
+
+// Output of LUT(func; x, y, z) on one table word (state.c:202-230).
+__device__ __forceinline__ uint32_t lut_word(uint32_t func, uint32_t x, uint32_t y, uint32_t z) {
+  uint32_t r = 0;
+#pragma unroll
+  for (int m = 0; m < 8; m++) {
+    if ((func >> m) & 1u) r |= ((m & 4) ? x : ~x) & ((m & 2) ? y : ~y) & ((m & 1) ? z : ~z);
+  }
+  return r;
+}
+
+// A match's record: gates in reference order (tuple positions of ordering row k), func_inner = solved bits only
+// and inner_seen = cells with a masked position (sbg_solve_inner's closed form, on the compressed
+// tables; a match has no conflicting cell).  width 5: func_middle unused.
+template <int NW, int WIDTH>
+__device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned long long key,
+    const int *tuple, int k, uint32_t fo, uint32_t fm, const uint32_t *s_tabs, int npad,
+    const uint32_t *T, const uint32_t *M) {
+  int G[WIDTH];
+#pragma unroll
+  for (int i = 0; i < WIDTH; i++) G[i] = tuple[WIDTH == 5 ? c_rows5[k][i] : c_rows7[k][i]];
+  uint32_t ones = 0, seen = 0;
+#pragma unroll
+  for (int w = 0; w < NW; w++) {
+    const uint32_t *t = s_tabs + w * npad;
+    const uint32_t x = lut_word(fo, t[G[0]], t[G[1]], t[G[2]]);
+    const uint32_t y = WIDTH == 7 ? lut_word(fm, t[G[3]], t[G[4]], t[G[5]]) : t[G[3]];
+    const uint32_t z = t[G[WIDTH - 1]];
+#pragma unroll
+    for (int c = 0; c < 8; c++) {
+      const uint32_t in_cell = M[w] & ((c & 4) ? x : ~x) & ((c & 2) ? y : ~y) & ((c & 1) ? z : ~z);
+      if (in_cell & T[w]) ones |= 1u << c;
+      if (in_cell) seen |= 1u << c;
+    }
+  }
+  DevMatch m;
+  m.key = key;
+#pragma unroll
+  for (int i = 0; i < 7; i++) m.gates[i] = i < WIDTH ? (uint16_t)G[i] : (uint16_t)0;
+  m.func_outer = (uint8_t)fo;
+  m.func_middle = WIDTH == 7 ? (uint8_t)fm : (uint8_t)0;
+  m.func_inner = (uint8_t)ones;
+  m.inner_seen = (uint8_t)seen;
+  m.width = (uint8_t)WIDTH;
+#pragma unroll
+  for (int i = 0; i < 5; i++) m.pad[i] = 0;
+  *dst = m;
+}
+
+// The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
+// 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
+// feasible tuple and ordering the set of working outer functions from outer_ok5.
+template <int NW, bool EMIT>
+__global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab) {
+  constexpr int P = 3, K = 5, NC = 1 << P;
+  extern __shared__ uint32_t smem[];
+  __shared__ uint8_t s_ord[256];
+  const int n = prob->n;
+  const int npad = (n + 3) & ~3;
+  uint32_t *s_tabs = smem;
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  uint32_t *cells = smem + NW * npad + warp * (NC * 2 * NW);  // per prefix cell: C1[NW], C0[NW]
+  stage_tables(s_tabs, prob, NW, npad);
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) s_ord[i] = ord.order[0][i];
+  __syncthreads();
+  uint32_t T[NW], M[NW];
+#pragma unroll
+  for (int w = 0; w < NW; w++) {
+    T[w] = prob->T[w];
+    M[w] = prob->M[w];
+  }
+  const uint32_t inmask = prob->inmask;
+  const uint64_t total = c_binom[n - 2][P];
+  const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
+  unsigned long long feasible_local = 0, matches_local = 0;
+
+  for (unsigned long long t = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
+       t < t_end; t += nwarps) {
+    unsigned long long base = 0;
+    if (EMIT) {
+      if (counts[t] == 0 || offsets[t] >= max_out) continue;
+      base = offsets[t];
+    }
+    // prefixes are dealt to the parts in blocks of kDeal, as k_sweep deals them
+    const uint64_t dealt = (t / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal + t % kDeal;
+    uint32_t count = 0;
+    if (dealt < total) {
+      int pre[P];
+      uint64_t base_rank;
+      unrank_prefix_warp<P, K, true>(dealt, n, pre, base_rank, lane);
+      bool rejected = false;
+#pragma unroll
+      for (int i = 0; i < P; i++) rejected |= (pre[i] < 8) && ((inmask >> pre[i]) & 1u);
+      const int last = pre[P - 1];
+      const int r = n - last - 1;
+      const uint32_t Q = rejected ? 0u : (uint32_t)(r * (r - 1) / 2);
+      uint32_t mixed = 0;
+      if (Q != 0) {
+        // prefix cell `lane` (first prefix gate = most significant bit), kept if mixed
+        bool mx = false;
+        if (lane < NC) {
+          uint32_t ones = 0, zeros = 0;
+#pragma unroll
+          for (int w = 0; w < NW; w++) {
+            uint32_t tt = M[w];
+#pragma unroll
+            for (int i = 0; i < P; i++) {
+              const uint32_t tv = s_tabs[w * npad + pre[i]];
+              tt &= ((lane >> (P - 1 - i)) & 1) ? tv : ~tv;
+            }
+            cells[lane * 2 * NW + w] = tt & T[w];
+            cells[lane * 2 * NW + NW + w] = tt & ~T[w];
+            ones |= tt & T[w];
+            zeros |= tt & ~T[w];
+          }
+          mx = ones != 0 && zeros != 0;
+        }
+        mixed = __ballot_sync(kFull, mx);
+        __syncwarp();
+      }
+      bool done = false;
+      for (uint32_t q0 = 0; q0 < Q && !done; q0 += 32) {
+        const uint32_t q = q0 + lane;
+        bool alive = q < Q;
+        int pi = 0, pj = 1;
+        if (alive) unrank_pair(q, r, pi, pj);
+        const int gf = last + 1 + pi, gg = last + 1 + pj;
+        if ((gf < 8 && ((inmask >> gf) & 1u)) || (gg < 8 && ((inmask >> gg) & 1u))) alive = false;
+        for (uint32_t mc = mixed; mc != 0 && alive; mc &= mc - 1) {
+          const int cj = __ffs(mc) - 1;
+          uint32_t a11 = 0, a10 = 0, a01 = 0, a00 = 0, b11 = 0, b10 = 0, b01 = 0, b00 = 0;
+#pragma unroll
+          for (int w = 0; w < NW; w++) {
+            const uint32_t tf = s_tabs[w * npad + gf], tg = s_tabs[w * npad + gg];
+            const uint32_t c1 = cells[cj * 2 * NW + w], c0 = cells[cj * 2 * NW + NW + w];
+            a11 |= c1 & tf & tg; b11 |= c0 & tf & tg;
+            a10 |= c1 & tf & ~tg; b10 |= c0 & tf & ~tg;
+            a01 |= c1 & ~tf & tg; b01 |= c0 & ~tf & tg;
+            a00 |= c1 & ~(tf | tg); b00 |= c0 & ~(tf | tg);
+          }
+          if ((a11 && b11) || (a10 && b10) || (a01 && b01) || (a00 && b00)) alive = false;
+        }
+        for (uint32_t fb = __ballot_sync(kFull, alive); fb != 0 && !done; fb &= fb - 1) {
+          const int src = __ffs(fb) - 1;
+          int g5[5] = {pre[0], pre[1], pre[2], __shfl_sync(kFull, gf, src),
+                       __shfl_sync(kFull, gg, src)};
+          feasible_local++;
+          uint32_t H1, H0;
+          summary5<NW>(s_tabs, npad, g5, T, M, lane, H1, H0);
+          for (int k = 0; k < 10 && !done; k++) {
+            uint32_t ok[8], surv_mine = 0;
+            outer_ok5(H1, H0, k, lane, tab, ok);
+            uint32_t c = 0;
+#pragma unroll
+            for (int hi = 0; hi < 8; hi++) {
+              const uint32_t surv = ok[hi] & __brev(ok[7 - hi]);
+              c += __popc(surv);
+              if (lane == hi) surv_mine = surv;
+            }
+            if (!EMIT) {
+              count += c;
+              continue;
+            }
+            if (c == 0) continue;
+            // positions in ascending order: lane takes position 32 * w + lane
+            const unsigned long long key_hi = ((base_rank + q0 + src) << 12) | ((uint64_t)k << 8);
+#pragma unroll 1
+            for (int w = 0; w < 8; w++) {
+              const uint32_t pos = 32u * w + lane;
+              const uint32_t fo = s_ord[pos];
+              const bool hit = (__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u;
+              const uint32_t bal = __ballot_sync(kFull, hit);
+              const unsigned long long at = base + count + __popc(bal & lanemask_lt());
+              if (hit && at < max_out) {
+                write_match<NW, 5>(out + at, key_hi | pos, g5, k, fo, 0, s_tabs, npad, T, M);
+              }
+              count += __popc(bal);
+            }
+            done = base + count >= max_out;
+          }
+        }
+      }
+    }
+    if (!EMIT) {
+      if (lane == 0) counts[t] = count;
+      matches_local += count;
+    }
+  }
+  if (!EMIT && lane == 0) {
+    if (matches_local != 0) atomicAdd(&ectl->total, matches_local);
+    if (feasible_local != 0) atomicAdd(&ectl->feasible, feasible_local);
+  }
+}
+
+// Middle functions of one cube set (see middle_cubes) as a 256-bit set over fm, word wd = fm >> 5.
+__device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (*hok)[4],
+    uint32_t S, uint32_t ov, uint32_t *bits) {
+#pragma unroll
+  for (int wd = 0; wd < 8; wd++) bits[wd] = 0;
+#pragma unroll
+  for (int c0 = 0; c0 < 4; c0++) {
+#pragma unroll
+    for (int c1 = 0; c1 < 4; c1++) {
+      if (!(hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0)) continue;
+      const uint32_t V = hv[0][c0] | hv[1][c1];
+      uint32_t low = 0xffffffffu;   // fm & 31 with (fm & S & 31) == (V & 31)
+#pragma unroll
+      for (int i = 0; i < 5; i++) {
+        if ((S >> i) & 1u) low &= ((V >> i) & 1u) ? colour_pattern(i, 0) : ~colour_pattern(i, 0);
+      }
+#pragma unroll
+      for (int wd = 0; wd < 8; wd++) {
+        if ((((uint32_t)wd << 5) & S) == (V & 0xe0u)) bits[wd] |= low;
+      }
+    }
+  }
+}
+
+// The 7-LUT sweep of one part over the list, tickets t_begin .. t_end-1 of it (entry idx = t *
+// nparts + part), one warp per entry: the summary and stage-1 filter of k_decomp7 on the TRUE gate
+// tables (no stale outer cache), then per surviving outer function and ordering row the union of
+// the middle-function cubes.  Count: one lane per outer function; emit: positions in ascending
+// order, outer position in the loop, middle position across the lanes.
+template <int NW, bool EMIT>
+__global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
+    unsigned int list_count, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab) {
+  extern __shared__ uint32_t smem[];
+  __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
+  __shared__ uint8_t s_fo[kWarpsPerCta][256];
+  __shared__ uint32_t s_src7[25 * 32];
+  __shared__ uint32_t s_H[kWarpsPerCta][16];
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int n = prob->n;
+  const int npad = (n + 3) & ~3;
+  uint32_t *s_tabs = smem;
+  stage_tables(s_tabs, prob, NW, npad);
+  for (int i = threadIdx.x; i < 25 * 32; i += blockDim.x) s_src7[i] = tab->src7[i >> 5][i & 31];
+  for (int i = threadIdx.x; i < 512; i += blockDim.x) s_ord[i >> 8][i & 255] = ord.order[i >> 8][i & 255];
+  __syncthreads();
+  uint32_t T[NW], M[NW];
+#pragma unroll
+  for (int w = 0; w < NW; w++) {
+    T[w] = prob->T[w];
+    M[w] = prob->M[w];
+  }
+  uint32_t *sH = s_H[warp];
+  uint8_t *fo_list = s_fo[warp];
+  const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
+  unsigned long long matches_local = 0;
+
+  for (unsigned long long t = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
+       t < t_end; t += nwarps) {
+    const uint64_t idx = t * (uint64_t)nparts + (uint64_t)part;
+    unsigned long long base = 0;
+    if (EMIT) {
+      if (counts[t] == 0 || offsets[t] >= max_out) continue;
+      base = offsets[t];
+    }
+    uint32_t count = 0;
+    if (idx < list_count) {
+      const uint64_t cur = list[idx];
+      int g[7];
+#pragma unroll
+      for (int i = 0; i < 7; i++) g[i] = (int)((cur >> (9 * (6 - i))) & 0x1ffu);
+      tuple_summary<NW>(s_tabs, npad, g, T, M, lane, sH);
+      const uint32_t pass_j = triples_with_colourings(sH, lane);
+      bool done = false;
+      for (int j = 0; j < 25 && !done; j++) {
+        if (((pass_j >> j) & 1u) == 0) continue;
+        uint32_t W[8], ok[8];
+        outer_ok7(sH, s_src7[j * 32 + lane], lane, W, ok);
+        uint32_t any = 0, surv_mine = 0;
+#pragma unroll
+        for (int hi = 0; hi < 8; hi++) {
+          const uint32_t sv = ok[hi] & __brev(ok[7 - hi]);
+          any |= sv;
+          if (lane == hi) surv_mine = sv;
+        }
+        if (any == 0) continue;
+        const int k0 = c_j_first_k[j];
+        const int nrows = c_j_rows[j];
+        if (!EMIT) {
+          int ns = 0;
+          __syncwarp();
+#pragma unroll
+          for (int hi = 0; hi < 8; hi++) {
+            const uint32_t sv = __shfl_sync(kFull, surv_mine, hi);
+            if ((sv >> lane) & 1u) fo_list[ns + __popc(sv & lanemask_lt())] = (uint8_t)(hi * 32 + lane);
+            ns += __popc(sv);
+          }
+          __syncwarp();
+          for (int i0 = 0; i0 < ns; i0 += 32) {
+            const bool have = i0 + lane < ns;
+            const int fo = have ? fo_list[i0 + lane] : 0;
+            uint32_t r1 = 0, r0 = 0;
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+              if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
+            }
+            uint32_t c = 0;
+#pragma unroll 1
+            for (int row = 0; row < nrows; row++) {
+              uint32_t hv[2][4], S, ov, bits[8];
+              bool hok[2][4];
+              middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
+              cube_union(hv, hok, S, ov, bits);
+#pragma unroll
+              for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd]);
+            }
+            count += __reduce_add_sync(kFull, have ? c : 0u);
+          }
+        }
+#pragma unroll 1
+        for (int row = 0; EMIT && row < nrows && !done; row++) {
+          const int k = k0 + row;
+#pragma unroll 1
+          for (int po = 0; po < 256 && !done; po++) {
+            const uint32_t fo = s_ord[0][po];
+            if (((__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u) == 0) continue;
+            uint32_t r1 = 0, r0 = 0;
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+              if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
+            }
+            uint32_t hv[2][4], S, ov;
+            bool hok[2][4];
+            middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
+            const unsigned long long key_hi = (idx << 23) | ((uint64_t)k << 16) | ((uint64_t)po << 8);
+#pragma unroll 1
+            for (int w = 0; w < 8; w++) {
+              const uint32_t pm = 32u * w + lane;
+              const uint32_t fm = s_ord[1][pm];
+              bool hit = false;
+#pragma unroll
+              for (int c0 = 0; c0 < 4; c0++) {
+#pragma unroll
+                for (int c1 = 0; c1 < 4; c1++) {
+                  hit |= hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0
+                      && (fm & S) == (hv[0][c0] | hv[1][c1]);
+                }
+              }
+              const uint32_t bal = __ballot_sync(kFull, hit);
+              const unsigned long long at = base + count + __popc(bal & lanemask_lt());
+              if (hit && at < max_out) {
+                write_match<NW, 7>(out + at, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
+              }
+              count += __popc(bal);
+            }
+            done = base + count >= max_out;
+          }
+        }
+      }
+    }
+    if (!EMIT) {
+      if (lane == 0) counts[t] = count;
+      matches_local += count;
+    }
+  }
+  if (!EMIT && lane == 0 && matches_local != 0) atomicAdd(&ectl->total, matches_local);
+}
+
+// Exclusive prefix sum of counts[t_begin .. t_end-1] into offsets, continuing from ectl->carry
+// (the matches of earlier windows), which it advances.  One CTA of 1,024 threads, a tile of 1,024
+// tickets at a time.
+__global__ void __launch_bounds__(1024) k_enum_scan(EnumCtl *__restrict__ ectl,
+    const uint32_t *__restrict__ counts, unsigned long long *__restrict__ offsets,
+    unsigned long long t_begin, unsigned long long t_end) {
+  __shared__ unsigned long long s_warp[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long carry = ectl->carry;
+  for (unsigned long long t0 = t_begin; t0 < t_end; t0 += blockDim.x) {
+    const unsigned long long t = t0 + threadIdx.x;
+    const unsigned long long c = t < t_end ? counts[t] : 0ull;
+    unsigned long long incl = c;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const unsigned long long up = __shfl_up_sync(kFull, incl, d);
+      if (lane >= d) incl += up;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    unsigned long long before = 0;
+    for (int i = 0; i < warp; i++) before += s_warp[i];
+    unsigned long long tile = 0;
+    for (int i = 0; i < (int)(blockDim.x >> 5); i++) tile += s_warp[i];
+    if (t < t_end) offsets[t] = carry + before + incl - c;
+    carry += tile;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) ectl->carry = carry;
 }
 
 }  // namespace sbg

@@ -8,13 +8,14 @@ the state, target, mask, the used input bits -- plus the RNG the reference keeps
 """
 import ctypes as C
 from dataclasses import dataclass, field
-from typing import List
+from typing import List, Optional
 
 import numpy as np
 
 from . import native
 from .native import (SbgResult, SbgJob, SbgNodeResult, NativeLibraryError, SBG_KEY_NONE,
-                     SBG_LIST_CAP, SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7)
+                     SBG_LIST_CAP, SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7, MATCH_DTYPE,
+                     SBG_ENUM_MAX_MATCHES)
 
 NO_GATE = 0xFFFF  # state.h:30
 
@@ -32,6 +33,17 @@ class SearchResult:
     gates: List[int] = field(default_factory=list)
     pos_outer: int = 0             # position of func_outer / func_middle in the shuffled orders
     pos_middle: int = 0
+
+
+@dataclass
+class Enumeration:
+    """The matches of one search state (sbg_enum5 / sbg_enum7): `total` = how many there are in the
+    share (None if the count was skipped), `feasible` = feasible 5-combinations met / length of the
+    7-LUT list, `matches` = the first min(max_matches, total) of them in ascending key order (the
+    reference's enumeration order), a structured array of dtype MATCH_DTYPE."""
+    total: Optional[int]
+    feasible: int
+    matches: np.ndarray
 
 
 def shuffled_order(rng):
@@ -340,6 +352,29 @@ class LutEngine:
                                          _order_ptr(middle_order), C.byref(res)))
         return res
 
+    # -- enumeration ---------------------------------------------------------------------------
+    def _enumerate(self, fn, orders, max_matches, count, part, nparts):
+        max_matches = int(max_matches)
+        if not 0 <= max_matches <= SBG_ENUM_MAX_MATCHES:
+            raise ValueError("max_matches must lie in 0..%d" % SBG_ENUM_MAX_MATCHES)
+        out = np.zeros(max(max_matches, 1), dtype=MATCH_DTYPE)
+        n_out, total, feasible = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        bufs = [_order_ptr(o) for o in orders]
+        self._check(fn(self._h, part, nparts, *bufs, max_matches, out.ctypes.data_as(C.c_void_p),
+                       C.byref(n_out), C.byref(total) if count else None, C.byref(feasible)))
+        return Enumeration(int(total.value) if count else None, int(feasible.value),
+                           out[:n_out.value].copy())
+
+    def enumerate5(self, func_order, max_matches, count=True, part=0, nparts=1):
+        """Every match of search_5lut on the current problem: the total (count=True) and the first
+        max_matches in key order.  count=False may stop as soon as those are known."""
+        return self._enumerate(self.lib.sbg_enum5, [func_order], max_matches, count, part, nparts)
+
+    def enumerate7(self, outer_order, middle_order, max_matches, count=True, part=0, nparts=1):
+        """The same for search_7lut, over the installed phase-1 list (run here if there is none)."""
+        return self._enumerate(self.lib.sbg_enum7, [outer_order, middle_order], max_matches, count,
+                               part, nparts)
+
 
 def unpack_tuple7(packed):
     """63-bit packed 7-combination -> list of gate numbers."""
@@ -354,15 +389,22 @@ def pack_tuple7(gates):
     return p
 
 
+def _fill(func_inner, inner_seen, rng):
+    """The random don't-care fill of get_lut_function (lut.c:104-106): one draw iff a cell is
+    unseen."""
+    fi = int(func_inner)
+    if inner_seen != 0xFF:
+        fi |= (~int(inner_seen) & 0xFF) & (rng.next() & 0xFF)
+    return fi
+
+
 def result5_to_ret(res, rng):
     """sbg_result -> the reference's ret[10] for search_5lut (lut.c:202-211), applying the random
     don't-care fill of get_lut_function (lut.c:104-106)."""
     if not res.found:
         return SearchResult(False, [0] * 10, key=int(res.key), tuples_feasible=int(res.tuples_feasible),
                             tuples_swept=int(res.tuples_swept))
-    fi = res.func_inner
-    if res.inner_seen != 0xFF:
-        fi |= (~res.inner_seen & 0xFF) & (rng.next() & 0xFF)
+    fi = _fill(res.func_inner, res.inner_seen, rng)
     gates = [int(g) for g in res.gates[:5]]
     ret = [res.func_outer, fi] + gates + [0, 0, 0]
     return SearchResult(True, ret, ordering=res.ordering, key=int(res.key), index=int(res.index),
@@ -375,9 +417,7 @@ def result7_to_ret(res, rng):
     if not res.found:
         return SearchResult(False, [0] * 10, key=int(res.key), tuples_feasible=int(res.tuples_feasible),
                             tuples_swept=int(res.tuples_swept))
-    fi = res.func_inner
-    if res.inner_seen != 0xFF:
-        fi |= (~res.inner_seen & 0xFF) & (rng.next() & 0xFF)
+    fi = _fill(res.func_inner, res.inner_seen, rng)
     gates = [int(g) for g in res.gates[:7]]
     ret = [res.func_outer, res.func_middle, fi] + gates
     return SearchResult(True, ret, ordering=res.ordering, key=int(res.key), index=int(res.index),
@@ -404,6 +444,49 @@ def search_7lut(engine, tables, target, mask, inbits, rng):
     outer, middle = shuffled_orders7(rng)
     engine.load(tables, target, mask, inbits)
     return result7_to_ret(engine.search7(outer, middle), rng)
+
+
+def match_to_ret(match, rng):
+    """One enumerated match (a record of Enumeration.matches) -> the reference's ret[10]
+    (lut.c:202-211 / 453-462), the don't-care bits of the inner function filled from `rng` as
+    get_lut_function would fill them."""
+    fi = _fill(match["func_inner"], match["inner_seen"], rng)
+    gates = [int(g) for g in match["gates"]]
+    if int(match["width"]) == 5:
+        return [int(match["func_outer"]), fi] + gates[:5] + [0, 0, 0]
+    return [int(match["func_outer"]), int(match["func_middle"]), fi] + gates
+
+
+def decode_key5(key):
+    """5-LUT key -> (rank of the combination, ordering k, position in the function order)."""
+    key = int(key)
+    return key >> 12, (key >> 8) & 0xF, key & 0xFF
+
+
+def decode_key7(key):
+    """7-LUT key -> (list index, ordering k, outer position, middle position)."""
+    key = int(key)
+    return key >> 23, (key >> 16) & 0x7F, (key >> 8) & 0xFF, key & 0xFF
+
+
+def enumerate_5lut(engine, tables, target, mask, inbits, order, max_matches, count=True, part=0,
+                   nparts=1):
+    """Every realisation of the state by search_5lut's decomposition under the function order
+    `order` (an Enumeration).  Consumes no RNG; match_to_ret applies the fill per match."""
+    if len(tables) < 5:
+        raise ValueError("search_5lut needs at least 5 gates (lut.c:119)")
+    engine.load(tables, target, mask, inbits)
+    return engine.enumerate5(order, max_matches, count, part, nparts)
+
+
+def enumerate_7lut(engine, tables, target, mask, inbits, outer, middle, max_matches, count=True,
+                   part=0, nparts=1):
+    """The same for search_7lut, over the state's phase-1 list (the first SBG_LIST_CAP feasible
+    7-combinations), decided on the true gate tables."""
+    if len(tables) < 7:
+        raise ValueError("search_7lut needs at least 7 gates (lut.c:259)")
+    engine.load(tables, target, mask, inbits)
+    return engine.enumerate7(outer, middle, max_matches, count, part, nparts)
 
 
 @dataclass

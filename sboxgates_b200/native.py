@@ -6,6 +6,8 @@ missing, loading fails loudly -- there is deliberately no fallback implementatio
 import ctypes as C
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # SBG_LIB: another build of the same library (A/B measurements of kernel variants)
 LIB_PATH = os.environ.get("SBG_LIB") or os.path.join(_HERE, "libsboxgates_b200.so")
@@ -39,6 +41,19 @@ class SbgNodeResult(C.Structure):
     _fields_ = [("found_stage", C.c_int32), ("gates3", C.c_uint16 * 3), ("func3", C.c_uint8),
                 ("seen3", C.c_uint8), ("key3", C.c_uint64), ("r5", SbgResult), ("r7", SbgResult)]
 
+
+class SbgMatch(C.Structure):
+    """One enumerated match (sbg_match, 32 bytes)."""
+    _fields_ = [("key", C.c_uint64), ("gates", C.c_uint16 * 7), ("func_outer", C.c_uint8),
+                ("func_middle", C.c_uint8), ("func_inner", C.c_uint8), ("inner_seen", C.c_uint8),
+                ("width", C.c_uint8), ("pad", C.c_uint8 * 5)]
+
+
+# The same layout as a numpy structured dtype: enumeration results arrive as one array.
+MATCH_DTYPE = np.dtype([("key", "<u8"), ("gates", "<u2", (7,)), ("func_outer", "u1"),
+                        ("func_middle", "u1"), ("func_inner", "u1"), ("inner_seen", "u1"),
+                        ("width", "u1"), ("pad", "u1", (5,))])
+SBG_ENUM_MAX_MATCHES = 1 << 24
 
 SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7 = 1, 2, 4
 SBG_LANES = 8
@@ -83,6 +98,10 @@ SIGNATURES = {
     "sbg_ordering_row": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "sbg_solve_inner": (C.c_int, [u64p, u64p, u64p, u64p, u64p, u8p, u8p]),
     "sbg_lut_table": (None, [C.c_uint8, u64p, u64p, u64p, u64p]),
+    "sbg_enum5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, C.c_uint64, C.c_void_p, u64p, u64p,
+                            u64p]),
+    "sbg_enum7": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, C.c_uint64, C.c_void_p, u64p,
+                            u64p, u64p]),
 }
 
 _lib = None
