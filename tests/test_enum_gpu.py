@@ -18,11 +18,24 @@ pytestmark = pytest.mark.gpu
 K = 300          # matches compared record for record
 MUX = [[], [(3, 1)], [(0, 0), (5, 1)], [(1, 1), (4, 0), (6, 1)]]
 
-# (n, mask depth, excluded input bits)
+# (n, mask, excluded input bits); mask 0-3 = mux mask of that depth, larger = a random mask of that
+# many positions, whose last 32-bit word is partly padding
 CASES5 = [(12, 0, []), (12, 1, [0]), (12, 3, [2]), (16, 2, [0, 5]), (16, 3, []), (20, 1, []),
-          (20, 2, [0]), (24, 0, [1]), (24, 1, [0, 2])]
-CASES7 = [(10, 0, []), (10, 2, [0]), (12, 1, [0, 3]), (12, 3, []), (14, 2, [0]), (14, 3, [4])]
+          (20, 2, [0]), (24, 0, [1]), (24, 1, [0, 2]), (16, 33, [0]), (20, 65, []), (20, 129, [0]),
+          (24, 200, [])]
+CASES7 = [(10, 0, []), (10, 2, [0]), (12, 1, [0, 3]), (12, 3, []), (14, 2, [0]), (14, 3, [4]),
+          (12, 33, [0]), (14, 65, []), (12, 129, []), (10, 200, [0])]
 LIST7 = 3        # list entries the 7-LUT oracle comparisons enumerate
+
+
+def _mask(spec, seed):
+    if spec < len(MUX):
+        return S.mux_mask(MUX[spec])
+    rs = np.random.RandomState(seed)
+    mask = np.zeros(4, dtype=np.uint64)
+    for p in rs.choice(256, spec, replace=False):
+        mask[p >> 6] |= np.uint64(1) << np.uint64(p & 63)
+    return mask
 
 
 def _state(n, depth, inb, seed, width):
@@ -35,7 +48,7 @@ def _state(n, depth, inb, seed, width):
     outer = S.lut_table(f[0], tabs[g[0]], tabs[g[1]], tabs[g[2]])
     mid = tabs[g[3]] if width == 5 else S.lut_table(f[1], tabs[g[3]], tabs[g[4]], tabs[g[5]])
     tgt = S.lut_table(f[2], outer, mid, tabs[g[-1]])
-    return tabs, tgt, S.mux_mask(MUX[depth]), inb
+    return tabs, tgt, _mask(depth, seed), inb
 
 
 def _states5():

@@ -16,9 +16,11 @@ pytestmark = pytest.mark.gpu
 
 CAP = 100000
 
-# (n, mux-fixed (bit, value) pairs, excluded input bits, oracle entries compared or None = all).
-# The oracle walks the combinations one by one, so the largest states are compared on the first
-# entries of their lists; the last case is a sparse mask whose list reaches the 100,000 cap.
+# (n, mux-fixed (bit, value) pairs or the size of a random mask, excluded input bits, oracle entries
+# compared or None = all).  The oracle walks the combinations one by one, so the largest states are
+# compared on the first entries of their lists; the last case is a sparse mask whose list reaches
+# the 100,000 cap.  Random masks of 33, 65, 129 and 200 positions leave their last 32-bit word
+# partly padding.
 CASES = [
     (12, [], [], None),
     (12, [(1, 1)], [1], None),
@@ -42,6 +44,11 @@ CASES = [
     (47, [(1, 1), (7, 0)], [], 300),
     (63, [(0, 1), (3, 0), (5, 1)], [0, 3, 5], None),
     (63, [(4, 0), (6, 1), (7, 1)], [], None),
+    (31, 33, [0], None),
+    (31, 65, [], None),
+    (32, 129, [0, 4], None),
+    (40, 200, [], None),
+    (47, 33, [], 2000),
 ]
 
 
@@ -53,21 +60,27 @@ def _pack(lst):
     return out
 
 
+def _random_mask(positions, seed):
+    rs = np.random.RandomState(seed)
+    mask = np.zeros(4, dtype=np.uint64)
+    for p in rs.choice(256, positions, replace=False):
+        mask[p >> 6] |= np.uint64(1) << np.uint64(p & 63)
+    return mask
+
+
 def _sparse_cap_case():
     """n = 63 under 12 random positions: most combinations are feasible, the list is capped."""
-    rs = np.random.RandomState(63)
-    mask = np.zeros(4, dtype=np.uint64)
-    for p in rs.choice(256, 12, replace=False):
-        mask[p >> 6] |= np.uint64(1) << np.uint64(p & 63)
-    return 63, S.synthetic_state(63, seed=6300), S.sbox_target(S.rijndael_sbox(), 5), mask, [2]
+    return (63, S.synthetic_state(63, seed=6300), S.sbox_target(S.rijndael_sbox(), 5),
+            _random_mask(12, 63), [2])
 
 
 def _states():
     sbox = S.rijndael_sbox()
     out = []
     for i, (n, fixed, inb, cmp) in enumerate(CASES):
-        out.append((n, S.synthetic_state(n, seed=8100 + i), S.sbox_target(sbox, i % 8),
-                    S.mux_mask(fixed), inb, cmp))
+        mask = _random_mask(fixed, 8200 + i) if isinstance(fixed, int) else S.mux_mask(fixed)
+        out.append((n, S.synthetic_state(n, seed=8100 + i), S.sbox_target(sbox, i % 8), mask, inb,
+                    cmp))
     n, tabs, tgt, mask, inb = _sparse_cap_case()
     out.append((n, tabs, tgt, mask, inb, None))
     return out
