@@ -212,12 +212,14 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
    of func_inner's don't-care bits stays with the caller, as for sbg_result).  32 bytes: */
 typedef struct {
   uint64_t key;            /* offset 0 */
-  uint16_t gates[7];       /* 8: LUT inputs in reference order a..e (5-LUT; then 0) or a..g */
-  uint8_t func_outer;      /* 22: the function at position (key >> 8) & 0xff of the outer order */
+  uint16_t gates[7];       /* 8: LUT inputs in reference order a..c (3-LUT), a..e (5-LUT; then 0)
+                              or a..g */
+  uint8_t func_outer;      /* 22: the function at position (key >> 8) & 0xff of the outer order
+                              (3-LUT: 0) */
   uint8_t func_middle;     /* 23: 7-LUT: the function at position key & 0xff of the middle order */
-  uint8_t func_inner;      /* 24: solved bits only; don't-care bits are 0 */
+  uint8_t func_inner;      /* 24: solved bits only; don't-care bits are 0 (3-LUT: the LUT) */
   uint8_t inner_seen;      /* 25: bit c set = inner cell c occurs under the mask */
-  uint8_t width;           /* 26: 5 or 7 */
+  uint8_t width;           /* 26: 3, 5 or 7 */
   uint8_t pad[5];          /* 27: 0 */
 } sbg_match;
 #define SBG_ENUM_MAX_MATCHES (1u << 24)   /* largest max_matches of one call */
@@ -239,6 +241,23 @@ int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, ui
 int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
     uint64_t *total, uint64_t *feasible);
+/* The matches of lut_search's 3-LUT scan (lut.c:501-523) over the caller's shuffled gate order
+   (n entries): the position triples i < k < m whose gates gate_order[i], gate_order[k],
+   gate_order[m] pass check_n_lut_possible(3, ...) under the mask (get_lut_function then cannot
+   fail, so each feasible triple is exactly one match).  inbits plays no part, as in the scan.
+   Key i << 18 | k << 9 | m, as sbg_node_result::key3, so the first match is the triple the scan of
+   sbg_search_node(SBG_DO_SCAN3) returns.  Record: width 3; gates[0..2] = gate_order[i],
+   gate_order[k], gate_order[m] (add_lut's argument order, as sbg_node_result::gates3), gates[3..6]
+   = 0; func_outer = func_middle = 0; func_inner / inner_seen as sbg_solve_inner gives them, cell
+   a<<2 | b<<1 | c with a the gate at position i.  The work is the n(n-1)/2 position pairs (i, k);
+   part/nparts, max_matches, total and the count-free stop behave as for sbg_enum5, and *feasible =
+   the feasible triples met, which is the number of matches counted.  The call does not touch the
+   installed 7-LUT list: an sbg_search7 / sbg_enum7 after it sees what it would have seen without
+   it.  sbg_search_node takes its gate order as given; sbg_enum3 checks that gate_order is a
+   permutation of 0..n-1 (as every order create_circuit builds is, sboxgates.c:285-299) and returns
+   SBG_ERR_ARG otherwise, or when n < 3. */
+int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
+    uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible);
 
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense

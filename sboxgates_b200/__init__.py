@@ -10,13 +10,15 @@ does not.
 from .rng import Xorshift1024
 from .lut import LutEngine, SearchResult, NO_GATE, search_5lut, search_7lut, shuffled_order, \
     shuffled_orders7, ordering_row, solve_inner, lut_table, lut_search, LutSearchResult, \
-    Enumeration, enumerate_5lut, enumerate_7lut, match_to_ret, decode_key5, decode_key7
+    Enumeration, enumerate_3lut, enumerate_5lut, enumerate_7lut, enumerate_lut_search, \
+    match_to_ret, match_to_lut3, decode_key3, decode_key5, decode_key7
 from .native import load_library, NativeLibraryError, MATCH_DTYPE
 
 __all__ = [
     "Xorshift1024", "LutEngine", "SearchResult", "NO_GATE", "search_5lut", "search_7lut",
     "shuffled_order", "shuffled_orders7", "ordering_row", "solve_inner", "lut_table",
-    "lut_search", "LutSearchResult", "Enumeration", "enumerate_5lut", "enumerate_7lut",
-    "match_to_ret", "decode_key5", "decode_key7", "MATCH_DTYPE",
+    "lut_search", "LutSearchResult", "Enumeration", "enumerate_3lut", "enumerate_5lut",
+    "enumerate_7lut", "enumerate_lut_search", "match_to_ret", "match_to_lut3", "decode_key3",
+    "decode_key5", "decode_key7", "MATCH_DTYPE",
     "load_library", "NativeLibraryError",
 ]

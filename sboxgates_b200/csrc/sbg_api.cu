@@ -1348,7 +1348,7 @@ int finish7_slot(sbg_handle *h, const sbg_handle::HostProblem &hp, uint64_t key,
   return SBG_OK;
 }
 
-// ---- enumeration (sbg_enum5 / sbg_enum7) -------------------------------------------------------
+// ---- enumeration (sbg_enum3 / sbg_enum5 / sbg_enum7) -------------------------------------------
 
 static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
     && offsetof(sbg_match, gates) == offsetof(DevMatch, gates)
@@ -1359,8 +1359,16 @@ static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
 // Count-free windows start at this many tickets and double: a first-match search then costs a few
 // windows of work past the first match, a search without one about twice the counting sweep's
 // launches (log2 of the tickets) and no more work.
+constexpr uint64_t kEnumWindow3 = kNominalWarps;
 constexpr uint64_t kEnumWindow5 = kNominalWarps;
 constexpr uint64_t kEnumWindow7 = kNominalWarps / 4;
+
+// What the enumeration kernels of one width read besides the problem block: the function order(s)
+// (widths 5 and 7) or the gate order (width 3).
+struct EnumInputs {
+  EnumOrders ord;
+  EnumGateOrder gates;
+};
 
 int ensure_enum(sbg_handle *h, sbg_lane &L, uint64_t tickets, uint64_t matches) {
   if (L.d_ectl == nullptr) SBG_CUDA(h, cudaMalloc(&L.d_ectl, sizeof(EnumCtl)));
@@ -1386,17 +1394,27 @@ int ensure_enum(sbg_handle *h, sbg_lane &L, uint64_t tickets, uint64_t matches) 
   return SBG_OK;
 }
 
-// One enumeration pass (count or emit) over tickets [a, b) of the lane's problem.
-template <bool SEVEN, bool EMIT>
-int launch_enum(sbg_handle *h, sbg_lane &L, const EnumOrders &ord, int part, int nparts,
+// One enumeration pass (count or emit) of width 3, 5 or 7 over tickets [a, b) of the lane's problem.
+template <int WIDTH, bool EMIT>
+int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int nparts,
     uint64_t max_out, uint64_t a, uint64_t b) {
+  static_assert(WIDTH == 3 || WIDTH == 5 || WIDTH == 7, "enumeration widths are 3, 5 and 7");
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const int n = hp.n;
+  const EnumOrders &ord = in.ord;
   cudaError_t e = cudaSuccess;
   int rc = SBG_OK;
 #define SBG_LAUNCH_ENUM(NWV)                                                                   \
   {                                                                                            \
-    if (SEVEN) {                                                                               \
+    if (WIDTH == 3) {                                                                          \
+      const size_t smem = decomp_smem<NWV>(n);                                                 \
+      auto kern = k_enum3<NWV, EMIT>;                                                          \
+      if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
+      e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
+          h->d_slots + L.slot, L.d_ectl, in.gates, L.d_ecount,                                 \
+          (const unsigned long long *)L.d_eoffset, L.d_ematch, (unsigned long long)max_out,    \
+          (unsigned long long)a, (unsigned long long)b, part, nparts);                         \
+    } else if (WIDTH == 7) {                                                                   \
       const size_t smem = decomp_smem<NWV>(n);                                                 \
       auto kern = k_enum7<NWV, EMIT>;                                                          \
       if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
@@ -1434,21 +1452,22 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumOrders &ord, int part, int
 
 // Count pass (in windows when only the first max_matches are wanted), offsets, emit pass, copy-out.
 // The lane's problem is prepared on the device.
-template <bool SEVEN>
-int run_enum(sbg_handle *h, sbg_lane &L, const EnumOrders &ord, int part, int nparts,
+template <int WIDTH>
+int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int nparts,
     uint64_t tickets, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
     uint64_t *feasible) {
   int rc;
   if ((rc = ensure_enum(h, L, std::max<uint64_t>(tickets, 1), 0)) != SBG_OK) return rc;
   SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
   const bool count_all = total != nullptr;
-  uint64_t window = count_all ? tickets : (SEVEN ? kEnumWindow7 : kEnumWindow5);
+  uint64_t window = count_all ? tickets
+      : (WIDTH == 3 ? kEnumWindow3 : WIDTH == 5 ? kEnumWindow5 : kEnumWindow7);
   uint64_t done = 0;
   EnumCtl ec;
   memset(&ec, 0, sizeof(ec));
   while (done < tickets) {
     const uint64_t end = std::min(tickets, done + window);
-    if ((rc = launch_enum<SEVEN, false>(h, L, ord, part, nparts, 0, done, end)) != SBG_OK) return rc;
+    if ((rc = launch_enum<WIDTH, false>(h, L, in, part, nparts, 0, done, end)) != SBG_OK) return rc;
     done = end;
     window *= 2;
     if (!count_all) {
@@ -1463,7 +1482,7 @@ int run_enum(sbg_handle *h, sbg_lane &L, const EnumOrders &ord, int part, int np
   const uint64_t emit = std::min<uint64_t>(max_matches, ec.carry);
   if (emit > 0) {
     if ((rc = ensure_enum(h, L, 0, emit)) != SBG_OK) return rc;
-    if ((rc = launch_enum<SEVEN, true>(h, L, ord, part, nparts, emit, 0, done)) != SBG_OK) return rc;
+    if ((rc = launch_enum<WIDTH, true>(h, L, in, part, nparts, emit, 0, done)) != SBG_OK) return rc;
     SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, emit * sizeof(sbg_match), cudaMemcpyDeviceToHost,
         L.stream));
     SBG_CUDA(h, cudaStreamSynchronize(L.stream));
@@ -1471,7 +1490,7 @@ int run_enum(sbg_handle *h, sbg_lane &L, const EnumOrders &ord, int part, int np
   }
   *n_out = emit;
   if (total != nullptr) *total = ec.carry;
-  if (feasible != nullptr) *feasible = SEVEN ? (uint64_t)L.list_count : ec.feasible;
+  if (feasible != nullptr) *feasible = WIDTH == 7 ? (uint64_t)L.list_count : ec.feasible;
   return SBG_OK;
 }
 
@@ -2326,10 +2345,10 @@ int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, ui
   // this part's tickets: its deal blocks of kDeal prefixes (the last one may be cut short)
   const uint64_t blocks = (h_binom[hp.n - 2][3] + kDeal - 1) / kDeal;
   const uint64_t mine = blocks > (uint64_t)part ? (blocks - part + nparts - 1) / nparts : 0;
-  EnumOrders ord;
-  memcpy(ord.order[0], func_order, 256);
-  memset(ord.order[1], 0, 256);
-  return run_enum<false>(h, L, ord, part, nparts, mine * kDeal, max_matches, out, n_out, total,
+  EnumInputs in5;
+  memcpy(in5.ord.order[0], func_order, 256);
+  memset(in5.ord.order[1], 0, 256);
+  return run_enum<5>(h, L, in5, part, nparts, mine * kDeal, max_matches, out, n_out, total,
       feasible);
 }
 
@@ -2359,10 +2378,43 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
   }
   const uint64_t count = L.list_count;
   const uint64_t mine = count > (uint64_t)part ? (count - part + nparts - 1) / nparts : 0;
-  EnumOrders ord;
-  memcpy(ord.order[0], outer_order, 256);
-  memcpy(ord.order[1], middle_order, 256);
-  return run_enum<true>(h, L, ord, part, nparts, mine, max_matches, out, n_out, total, feasible);
+  EnumInputs in7;
+  memcpy(in7.ord.order[0], outer_order, 256);
+  memcpy(in7.ord.order[1], middle_order, 256);
+  return run_enum<7>(h, L, in7, part, nparts, mine, max_matches, out, n_out, total, feasible);
+}
+
+int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
+    uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  int rc;
+  if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
+  const int n = cur(h).n;
+  if (n < 3) return fail(h, SBG_ERR_ARG, "the 3-LUT enumeration needs n >= 3 gates");
+  if (gate_order == nullptr) return fail(h, SBG_ERR_ARG, "no gate order");
+  // unlike the scan of sbg_search_node, which takes the order as given, the enumeration checks it
+  bool seen[SBG_MAX_GATES] = {};
+  for (int i = 0; i < n; i++) {
+    if (gate_order[i] >= n || seen[gate_order[i]]) {
+      return fail(h, SBG_ERR_ARG, "gate_order is not a permutation of 0..%d", n - 1);
+    }
+    seen[gate_order[i]] = true;
+  }
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
+  // only bring the problem block up to date: the control words of an installed 7-LUT list stay
+  L.seq++;
+  CallInputs none;
+  if ((rc = enqueue_begin(h, L, kBeginKeepCtl, none, 0)) != SBG_OK) return rc;
+  // this part's tickets: its deal blocks of kDeal position pairs (the last one may be cut short)
+  const uint64_t blocks = (h_binom[n][2] + kDeal - 1) / kDeal;
+  const uint64_t mine = blocks > (uint64_t)part ? (blocks - part + nparts - 1) / nparts : 0;
+  EnumInputs in3;
+  memset(&in3, 0, sizeof(in3));
+  memcpy(in3.gates.order, gate_order, sizeof(uint16_t) * (size_t)n);
+  return run_enum<3>(h, L, in3, part, nparts, mine * kDeal, max_matches, out, n_out, total,
+      feasible);
 }
 
 }  // extern "C"

@@ -2336,9 +2336,10 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
 }
 
 // ------------------------------------------------------------------------------------------------
-// Enumeration (sbg_enum5 / sbg_enum7): every match of search_5lut / search_7lut, not only the first.
-// The same decisions as the searches above with nothing thrown away, in two passes over the same
-// tickets -- a 3-gate prefix of C(n,5) (dealt to the parts as k_sweep deals them) or one list entry:
+// Enumeration (sbg_enum3 / sbg_enum5 / sbg_enum7): every match of lut_search's 3-LUT scan /
+// search_5lut / search_7lut, not only the first.  The same decisions as the searches above with
+// nothing thrown away, in two passes over the same tickets -- a position pair of the gate order, a
+// 3-gate prefix of C(n,5) (dealt to the parts as k_sweep deals them) or one list entry:
 //   count (EMIT = false): the number of matches of each ticket, and their sum;
 //   k_enum_scan: exclusive prefix sum of those counts = where each ticket's matches start in the
 //     ascending key order;
@@ -2737,6 +2738,121 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
     }
   }
   if (!EMIT && lane == 0 && matches_local != 0) atomicAdd(&ectl->total, matches_local);
+}
+
+// The caller's shuffled gate order of the 3-LUT enumeration: position -> gate.
+struct EnumGateOrder {
+  uint16_t order[kMaxGatesPad];
+};
+
+// The 3-LUT scan of lut_search (lut.c:501-523) with nothing thrown away, tickets t_begin .. t_end-1
+// of one part: a ticket is a position pair (i, k) of the gate order in lexicographic order (dealt to
+// the parts in blocks of kDeal, as k_enum5 deals its prefixes), one warp per pair, lanes over the
+// third position m.  The triple matches iff no cell a<<2 | b<<1 | c holds a masked 1 and a masked 0
+// of the target (scan3_blocks' test, here on the compressed tables).  Key i << 18 | k << 9 | m, so a
+// ticket's matches are consecutive keys in the order of its lanes.  A match's record: the gates in
+// position order, func_inner = cells holding a masked 1, inner_seen = cells holding a masked
+// position (sbg_solve_inner's closed form).
+template <int NW, bool EMIT>
+__global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts) {
+  extern __shared__ uint32_t smem[];
+  __shared__ uint16_t s_order[kMaxGatesPad];
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int n = prob->n;
+  const int npad = (n + 3) & ~3;
+  uint32_t *s_tabs = smem;
+  stage_tables(s_tabs, prob, NW, npad);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) s_order[i] = go.order[i];
+  __syncthreads();
+  uint32_t T[NW], Z[NW];   // masked positions with target 1 / with target 0
+#pragma unroll
+  for (int w = 0; w < NW; w++) {
+    T[w] = prob->T[w];
+    Z[w] = prob->M[w] & ~prob->T[w];
+  }
+  const uint64_t pairs = (uint64_t)(n * (n - 1) / 2);
+  const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
+  unsigned long long matches_local = 0;
+
+  for (unsigned long long t = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
+       t < t_end; t += nwarps) {
+    unsigned long long base = 0;
+    if (EMIT) {
+      if (counts[t] == 0 || offsets[t] >= max_out) continue;
+      base = offsets[t];
+    }
+    const uint64_t dealt = (t / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal + t % kDeal;
+    uint32_t count = 0;
+    if (dealt < pairs) {
+      int pi, pk;
+      unrank_pair((uint32_t)dealt, n, pi, pk);
+      const uint32_t *ta = s_tabs + s_order[pi], *tb = s_tabs + s_order[pk];
+      bool done = false;
+      for (int m0 = pk + 1; m0 < n && !done; m0 += 32) {
+        const int pm = m0 + lane;
+        const uint32_t *tc = s_tabs + s_order[pm < n ? pm : pk];
+        uint32_t one[8], zero[8];
+#pragma unroll
+        for (int c = 0; c < 8; c++) one[c] = zero[c] = 0;
+#pragma unroll
+        for (int w = 0; w < NW; w++) {
+          const uint32_t va = ta[w * npad], vb = tb[w * npad], vc = tc[w * npad];
+#pragma unroll
+          for (int c = 0; c < 8; c++) {
+            const uint32_t ab = ((c & 4) ? va : ~va) & ((c & 2) ? vb : ~vb);   // warp-uniform
+            const uint32_t cell = ab & ((c & 1) ? vc : ~vc);
+            one[c] |= cell & T[w];
+            zero[c] |= cell & Z[w];
+          }
+        }
+        uint32_t ones = 0, seen = 0;   // bit c: cell c holds a masked 1 / any masked position
+        bool ok = pm < n;
+#pragma unroll
+        for (int c = 0; c < 8; c++) {
+          ok &= !(one[c] != 0 && zero[c] != 0);
+          if (one[c] != 0) ones |= 1u << c;
+          if ((one[c] | zero[c]) != 0) seen |= 1u << c;
+        }
+        const uint32_t bal = __ballot_sync(kFull, ok);
+        if (EMIT) {
+          const unsigned long long at = base + count + __popc(bal & lanemask_lt());
+          if (ok && at < max_out) {
+            DevMatch m;
+            m.key = ((unsigned long long)pi << 18) | ((unsigned long long)pk << 9) | (unsigned)pm;
+            m.gates[0] = s_order[pi];
+            m.gates[1] = s_order[pk];
+            m.gates[2] = s_order[pm];
+#pragma unroll
+            for (int i = 3; i < 7; i++) m.gates[i] = 0;
+            m.func_outer = 0;
+            m.func_middle = 0;
+            m.func_inner = (uint8_t)ones;
+            m.inner_seen = (uint8_t)seen;
+            m.width = 3;
+#pragma unroll
+            for (int i = 0; i < 5; i++) m.pad[i] = 0;
+            out[at] = m;
+          }
+        }
+        count += __popc(bal);
+        done = EMIT && base + count >= max_out;
+      }
+    }
+    if (!EMIT) {
+      if (lane == 0) counts[t] = count;
+      matches_local += count;
+    }
+  }
+  // every feasible triple is a match: the two sums are the same number
+  if (!EMIT && lane == 0 && matches_local != 0) {
+    atomicAdd(&ectl->total, matches_local);
+    atomicAdd(&ectl->feasible, matches_local);
+  }
 }
 
 // Exclusive prefix sum of counts[t_begin .. t_end-1] into offsets, continuing from ectl->carry

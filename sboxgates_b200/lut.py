@@ -37,9 +37,10 @@ class SearchResult:
 
 @dataclass
 class Enumeration:
-    """The matches of one search state (sbg_enum5 / sbg_enum7): `total` = how many there are in the
-    share (None if the count was skipped), `feasible` = feasible 5-combinations met / length of the
-    7-LUT list, `matches` = the first min(max_matches, total) of them in ascending key order (the
+    """The matches of one search state (sbg_enum3 / sbg_enum5 / sbg_enum7): `total` = how many there
+    are in the share (None if the count was skipped), `feasible` = feasible triples met (= the
+    matches counted) / feasible 5-combinations met / length of the 7-LUT list, `matches` = the
+    first min(max_matches, total) of them in ascending key order (the
     reference's enumeration order), a structured array of dtype MATCH_DTYPE."""
     total: Optional[int]
     feasible: int
@@ -359,7 +360,8 @@ class LutEngine:
             raise ValueError("max_matches must lie in 0..%d" % SBG_ENUM_MAX_MATCHES)
         out = np.zeros(max(max_matches, 1), dtype=MATCH_DTYPE)
         n_out, total, feasible = C.c_uint64(), C.c_uint64(), C.c_uint64()
-        bufs = [_order_ptr(o) for o in orders]
+        # function orders as 256 bytes; a ctypes array (the gate order) as it is
+        bufs = [o if isinstance(o, C.Array) else _order_ptr(o) for o in orders]
         self._check(fn(self._h, part, nparts, *bufs, max_matches, out.ctypes.data_as(C.c_void_p),
                        C.byref(n_out), C.byref(total) if count else None, C.byref(feasible)))
         return Enumeration(int(total.value) if count else None, int(feasible.value),
@@ -374,6 +376,15 @@ class LutEngine:
         """The same for search_7lut, over the installed phase-1 list (run here if there is none)."""
         return self._enumerate(self.lib.sbg_enum7, [outer_order, middle_order], max_matches, count,
                                part, nparts)
+
+    def enumerate3(self, gate_order, max_matches, count=True, part=0, nparts=1):
+        """Every match of lut_search's 3-LUT scan over `gate_order` (a permutation of the current
+        problem's gates): the feasible position triples, keys i << 18 | k << 9 | m."""
+        go = np.ascontiguousarray(gate_order, dtype=np.uint16)
+        if go.ndim != 1 or go.shape[0] != self.n:
+            raise ValueError("gate_order must list the problem's %d gates" % self.n)
+        buf = (C.c_uint16 * go.shape[0]).from_buffer_copy(go.tobytes())
+        return self._enumerate(self.lib.sbg_enum3, [buf], max_matches, count, part, nparts)
 
 
 def unpack_tuple7(packed):
@@ -449,12 +460,30 @@ def search_7lut(engine, tables, target, mask, inbits, rng):
 def match_to_ret(match, rng):
     """One enumerated match (a record of Enumeration.matches) -> the reference's ret[10]
     (lut.c:202-211 / 453-462), the don't-care bits of the inner function filled from `rng` as
-    get_lut_function would fill them."""
+    get_lut_function would fill them.  A 3-LUT match has no ret[10]: see match_to_lut3."""
+    if int(match["width"]) == 3:
+        raise ValueError("a 3-LUT match has no ret[10]; use match_to_lut3")
     fi = _fill(match["func_inner"], match["inner_seen"], rng)
     gates = [int(g) for g in match["gates"]]
     if int(match["width"]) == 5:
         return [int(match["func_outer"]), fi] + gates[:5] + [0, 0, 0]
     return [int(match["func_outer"]), int(match["func_middle"]), fi] + gates
+
+
+def match_to_lut3(match, rng):
+    """One enumerated 3-LUT match -> the add_lut call lut_search would make for it (lut.c:510-518):
+    (function, gi, gk, gm), the don't-care bits filled from `rng` as get_lut_function fills them
+    (one draw iff a cell is unseen)."""
+    if int(match["width"]) != 3:
+        raise ValueError("not a 3-LUT match (width %d)" % int(match["width"]))
+    fi = _fill(match["func_inner"], match["inner_seen"], rng)
+    return (fi, int(match["gates"][0]), int(match["gates"][1]), int(match["gates"][2]))
+
+
+def decode_key3(key):
+    """3-LUT key -> (i, k, m), the positions of the triple in the gate order."""
+    key = int(key)
+    return key >> 18, (key >> 9) & 0x1FF, key & 0x1FF
 
 
 def decode_key5(key):
@@ -487,6 +516,42 @@ def enumerate_7lut(engine, tables, target, mask, inbits, outer, middle, max_matc
         raise ValueError("search_7lut needs at least 7 gates (lut.c:259)")
     engine.load(tables, target, mask, inbits)
     return engine.enumerate7(outer, middle, max_matches, count, part, nparts)
+
+
+def enumerate_3lut(engine, tables, target, mask, inbits, gate_order, max_matches, count=True,
+                   part=0, nparts=1):
+    """Every realisation of the state by lut_search's 3-LUT scan over `gate_order` (an
+    Enumeration; inbits plays no part, as in the scan).  Consumes no RNG; match_to_lut3 applies
+    the fill per match."""
+    if len(tables) < 3:
+        raise ValueError("the 3-LUT scan needs at least 3 gates")
+    engine.load(tables, target, mask, inbits)
+    return engine.enumerate3(gate_order, max_matches, count, part, nparts)
+
+
+def enumerate_lut_search(engine, tables, target, mask, inbits, gate_order, rng, max_matches,
+                         count=True, allow5=True, allow7=True):
+    """Every realisation of a node by each stage of lut_search (lut.c:489-631):
+    {3: Enumeration, 5: Enumeration or None, 7: Enumeration or None}.  Stage 5 and stage 7 get the
+    function orders lut_search would use, drawn from a COPY of `rng` in lut_search's sequence
+    (order5, then outer / middle); `rng` itself is not advanced.  A stage lut_search would not run
+    (allow5 / allow7 = check_num_gates_possible(st, 2 / 3), lut.c:525, 582; too few gates) is None.
+    Stage 3 needs n >= 3 (None otherwise); stage 7 runs over the state's phase-1 list."""
+    n = len(tables)
+    ahead = rng.copy()
+    order5 = shuffled_order(ahead) if (allow5 and n >= 5) else None
+    outer = middle = None
+    if allow5 and allow7 and n >= 7:
+        outer, middle = shuffled_orders7(ahead)
+    engine.load(tables, target, mask, inbits)
+    out = {3: None, 5: None, 7: None}
+    if n >= 3:
+        out[3] = engine.enumerate3(gate_order, max_matches, count)
+    if order5 is not None:
+        out[5] = engine.enumerate5(order5, max_matches, count)
+    if outer is not None:
+        out[7] = engine.enumerate7(outer, middle, max_matches, count)
+    return out
 
 
 @dataclass

@@ -102,6 +102,8 @@ SIGNATURES = {
                             u64p]),
     "sbg_enum7": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, C.c_uint64, C.c_void_p, u64p,
                             u64p, u64p]),
+    "sbg_enum3": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint16), C.c_uint64,
+                            C.c_void_p, u64p, u64p, u64p]),
 }
 
 _lib = None

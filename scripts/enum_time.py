@@ -1,7 +1,10 @@
 """Cost of enumeration next to the first-match searches, on bench.py's synthetic states.
 
 For each state (n = 40: masks of mux depth 0..3, i.e. the full mask and 128 / 64 / 32 positions;
-n = 64 likewise) it times with CUDA events, median of --reps runs after one warm-up:
+n = 64 likewise; a seeded shuffled gate order per state) it times with CUDA events, median of
+--reps runs after one warm-up:
+  scan3               lut_search's 3-LUT scan alone (search_node with SBG_DO_SCAN3 only)
+  count3  / first3    its full enumeration (count only) and count-free with max_matches = 1
   search5 / search7   the first-match searches (search7 includes phase 1)
   count5  / count7    full enumeration, count only (max_matches = 0); count7 on the list search7
                       left installed, i.e. phase 2 only
@@ -18,6 +21,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import bench  # noqa: E402
@@ -48,12 +52,17 @@ def main():
     print("%s, %d SMs, power limit %s W" % (
         torch.cuda.get_device_name(0), torch.cuda.get_device_properties(0).multi_processor_count,
         bench.power_limit_w(0)))
-    print("%4s %5s %4s | %10s %9s %9s %9s | %11s %7s %9s %9s %9s" % (
-        "n", "mask", "inb", "matches5", "search5", "count5", "first5", "matches7", "list",
-        "search7", "count7", "first7"))
+    print("%4s %5s %4s | %8s %7s %7s %7s | %10s %9s %9s %9s | %11s %7s %9s %9s %9s" % (
+        "n", "mask", "inb", "matches3", "scan3", "count3", "first3", "matches5", "search5",
+        "count5", "first5", "matches7", "list", "search7", "count7", "first7"))
     for n in args.n:
-        for st in bench.build_batch(n, 4, args.seed):
+        for j, st in enumerate(bench.build_batch(n, 4, args.seed)):
             eng.load(st["tables"], st["target"], st["mask"], st["inbits"])
+            gate_order = np.random.RandomState(1000 * args.seed + j).permutation(n)
+            ms_s3, r3 = timed(lambda: eng.search_node(0, gate_order=gate_order), args.reps)
+            ms_c3, e3 = timed(lambda: eng.enumerate3(gate_order, 0), args.reps)
+            ms_f3, f3 = timed(lambda: eng.enumerate3(gate_order, 1, count=False), args.reps)
+            assert (list(f3.matches["key"]) or [sb.lut.SBG_KEY_NONE])[0] == r3.key3
             ms_s5, r5 = timed(lambda: eng.search5(st["order5"]), args.reps)
             ms_c5, e5 = timed(lambda: eng.enumerate5(st["order5"], 0), args.reps)
             ms_f5, f5 = timed(lambda: eng.enumerate5(st["order5"], 1, count=False), args.reps)
@@ -63,9 +72,11 @@ def main():
             ms_f7, f7 = timed(lambda: eng.enumerate7(st["outer"], st["middle"], 1, count=False),
                               args.reps)
             positions = sum(bin(int(w)).count("1") for w in st["mask"])
-            print("%4d %5d %4s | %10d %9.3f %9.3f %9.3f | %11d %7d %9.3f %9.3f %9.3f" % (
-                n, positions, ",".join(map(str, st["inbits"])) or "-", e5.total, ms_s5, ms_c5,
-                ms_f5, e7.total, e7.feasible, ms_s7, ms_c7, ms_f7), flush=True)
+            print("%4d %5d %4s | %8d %7.3f %7.3f %7.3f | %10d %9.3f %9.3f %9.3f | %11d %7d %9.3f "
+                  "%9.3f %9.3f" % (
+                      n, positions, ",".join(map(str, st["inbits"])) or "-", e3.total, ms_s3,
+                      ms_c3, ms_f3, e5.total, ms_s5, ms_c5, ms_f5, e7.total, e7.feasible, ms_s7,
+                      ms_c7, ms_f7), flush=True)
     eng.close()
 
 
