@@ -259,6 +259,35 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
 int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
     uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible);
 
+/* ---- matches at any rank: the enumeration cursor ---------------------------------------------- */
+/* The cursor is the last sbg_enum3 / sbg_enum5 / sbg_enum7 call on the handle that counted
+   (total != NULL; max_matches may be 0).  Ranks are positions in that call's share (part/nparts),
+   in ascending key order: 0 .. total-1.  The device keeps what that count found (matches per
+   ticket and where each ticket's matches start), so a fetch or pick emits the matches of the
+   tickets it touches and counts nothing again; records are byte-identical to the ones the counted
+   call emits at the same ranks.  Neither call consumes RNG or changes the problem, the installed
+   7-LUT list or the cursor: any number of them may follow one count.  The cursor keeps the orders
+   it was counted with; the caller's buffers of that call are not read again.  Cursor lifetime:
+     - a counted sbg_enum* call replaces it; a count-free one ends it;
+     - any call of sbg_load_problem, sbg_stage_problem, sbg_use_problem, sbg_search5, sbg_search7,
+       sbg_search_node, sbg_search_batch, sbg_search5_part, sbg_finish5, sbg_filter7_part,
+       sbg_set_list7, sbg_list7_device, sbg_set_list7_device, sbg_allgather_merge7 (every handle
+       given), sbg_decomp7_part, sbg_finish7 or sbg_alu_peak ends it, whatever the call returns;
+     - sbg_last_error, sbg_launch_count, sbg_transfer_stats, sbg_host_seconds, sbg_last_kernel_ms,
+       sbg_set_timing, sbg_set_stream, sbg_enum_fetch and sbg_enum_pick keep it.
+   Without a cursor both calls return SBG_ERR_STATE.
+   A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
+   a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT) or a list
+   entry (7-LUT, up to 70 * 65,536 matches), so one deep rank can cost a whole ticket's sweep. */
+/* The matches at ranks first .. min(first + count, total) - 1, in key order, to out[0..]; *n_out =
+   how many (0 when first >= total).  count <= SBG_ENUM_MAX_MATCHES; out may be NULL iff count ==
+   0. */
+int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out, uint64_t *n_out);
+/* out[i] = the match at rank ranks[i], i < nranks <= SBG_ENUM_MAX_MATCHES.  The ranks may come in
+   any order and repeat.  A rank >= total: SBG_ERR_ARG and nothing written.  (The ranks are sorted
+   on the host and located on the device; each ticket holding one is swept once.) */
+int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_match *out);
+
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense
    states").  width = 7 with prefix_gates = 4 or 5 (search_7lut phase 1), width = 5 with

@@ -12,6 +12,7 @@
 #include <ctime>
 #include <map>
 #include <utility>
+#include <vector>
 
 #include "../../include/sboxgates_b200.h"
 
@@ -142,6 +143,30 @@ struct sbg_lane {
   unsigned long long *d_eoffset = nullptr;  // their exclusive prefix sum
   DevMatch *d_ematch = nullptr;             // the emitted records
   uint64_t ecount_cap = 0, ematch_cap = 0;
+  // fetch and pick on an enumeration cursor (allocated on the first call)
+  unsigned long long *d_pranks = nullptr;   // requested ranks, ascending
+  unsigned int *d_pslots = nullptr;         // their output slots
+  unsigned long long *d_ptickets = nullptr; // ticket of each rank, then the distinct tickets
+  unsigned int *d_pfirst = nullptr;         // each distinct ticket's first rank in d_pranks
+  uint64_t pick_cap = 0;
+};
+
+// What the enumeration kernels of one width read besides the problem block: the function order(s)
+// (widths 5 and 7) or the gate order (width 3).
+struct EnumInputs {
+  EnumOrders ord;
+  EnumGateOrder gates;
+};
+
+// The enumeration cursor: what sbg_enum_fetch / sbg_enum_pick need of the last counted enumeration
+// besides the counts and offsets it left in lane 0.  Valid while seq equals the handle's api_seq.
+struct EnumCursor {
+  bool made = false;
+  uint64_t seq = 0;
+  int width = 0, part = 0, nparts = 1, slot = -1;
+  EnumInputs in;
+  uint64_t tickets = 0, total = 0;
+  uint32_t list_count = 0;   // width 7
 };
 
 struct sbg_handle {
@@ -211,6 +236,10 @@ struct sbg_handle {
   double host_s[2] = {0, 0};               // host seconds: enqueueing chains, waiting + decoding
   double wait_s[3] = {0, 0, 0};            // of the waiting: for the 3-LUT scan, search_5lut, search_7lut
   char err[512] = {0};
+  // bumped by every entry point that launches device work or changes a problem, a list or the
+  // enumeration buffers; the enumeration cursor lives as long as it does not change
+  uint64_t api_seq = 0;
+  EnumCursor cursor;
 };
 
 namespace {
@@ -1363,13 +1392,6 @@ constexpr uint64_t kEnumWindow3 = kNominalWarps;
 constexpr uint64_t kEnumWindow5 = kNominalWarps;
 constexpr uint64_t kEnumWindow7 = kNominalWarps / 4;
 
-// What the enumeration kernels of one width read besides the problem block: the function order(s)
-// (widths 5 and 7) or the gate order (width 3).
-struct EnumInputs {
-  EnumOrders ord;
-  EnumGateOrder gates;
-};
-
 int ensure_enum(sbg_handle *h, sbg_lane &L, uint64_t tickets, uint64_t matches) {
   if (L.d_ectl == nullptr) SBG_CUDA(h, cudaMalloc(&L.d_ectl, sizeof(EnumCtl)));
   if (L.ecount_cap < tickets) {
@@ -1394,8 +1416,9 @@ int ensure_enum(sbg_handle *h, sbg_lane &L, uint64_t tickets, uint64_t matches) 
   return SBG_OK;
 }
 
-// One enumeration pass (count or emit) of width 3, 5 or 7 over tickets [a, b) of the lane's problem.
-template <int WIDTH, bool EMIT>
+// One enumeration pass (MODE: count, first-K, range or pick emit) of width 3, 5 or 7 over tickets
+// [a, b) of the lane's problem (pick: entries [a, b) of the ticket list in EnumCtl::sel).
+template <int WIDTH, int MODE>
 int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int nparts,
     uint64_t max_out, uint64_t a, uint64_t b) {
   static_assert(WIDTH == 3 || WIDTH == 5 || WIDTH == 7, "enumeration widths are 3, 5 and 7");
@@ -1408,7 +1431,7 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
   {                                                                                            \
     if (WIDTH == 3) {                                                                          \
       const size_t smem = decomp_smem<NWV>(n);                                                 \
-      auto kern = k_enum3<NWV, EMIT>;                                                          \
+      auto kern = k_enum3<NWV, MODE>;                                                          \
       if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
       e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
           h->d_slots + L.slot, L.d_ectl, in.gates, L.d_ecount,                                 \
@@ -1416,7 +1439,7 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
           (unsigned long long)a, (unsigned long long)b, part, nparts);                         \
     } else if (WIDTH == 7) {                                                                   \
       const size_t smem = decomp_smem<NWV>(n);                                                 \
-      auto kern = k_enum7<NWV, EMIT>;                                                          \
+      auto kern = k_enum7<NWV, MODE>;                                                          \
       if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
       e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
           h->d_slots + L.slot, L.d_ectl, ord, (const uint64_t *)L.d_sorted,                    \
@@ -1425,7 +1448,7 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
           (unsigned long long)b, part, nparts, (const DevTables *)h->d_tab);                   \
     } else {                                                                                   \
       const size_t smem = sweep_smem<NWV>(n);                                                  \
-      auto kern = k_enum5<NWV, EMIT>;                                                          \
+      auto kern = k_enum5<NWV, MODE>;                                                          \
       if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
       e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
           h->d_slots + L.slot, L.d_ectl, ord, L.d_ecount,                                      \
@@ -1442,7 +1465,7 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
   }
 #undef SBG_LAUNCH_ENUM
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "enumeration launch: %s", cudaGetErrorString(e));
-  if (!EMIT) {
+  if (MODE == kEnumCount) {
     e = launch(h, k_enum_scan, 1, 1024, 0, L.stream, false, L.d_ectl, (const uint32_t *)L.d_ecount,
         L.d_eoffset, (unsigned long long)a, (unsigned long long)b);
     if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_scan: %s", cudaGetErrorString(e));
@@ -1467,7 +1490,7 @@ int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int npa
   memset(&ec, 0, sizeof(ec));
   while (done < tickets) {
     const uint64_t end = std::min(tickets, done + window);
-    if ((rc = launch_enum<WIDTH, false>(h, L, in, part, nparts, 0, done, end)) != SBG_OK) return rc;
+    if ((rc = launch_enum<WIDTH, kEnumCount>(h, L, in, part, nparts, 0, done, end)) != SBG_OK) return rc;
     done = end;
     window *= 2;
     if (!count_all) {
@@ -1482,13 +1505,27 @@ int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int npa
   const uint64_t emit = std::min<uint64_t>(max_matches, ec.carry);
   if (emit > 0) {
     if ((rc = ensure_enum(h, L, 0, emit)) != SBG_OK) return rc;
-    if ((rc = launch_enum<WIDTH, true>(h, L, in, part, nparts, emit, 0, done)) != SBG_OK) return rc;
+    if ((rc = launch_enum<WIDTH, kEnumFirst>(h, L, in, part, nparts, emit, 0, done)) != SBG_OK) return rc;
     SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, emit * sizeof(sbg_match), cudaMemcpyDeviceToHost,
         L.stream));
     SBG_CUDA(h, cudaStreamSynchronize(L.stream));
     h->d2h_bytes += emit * sizeof(sbg_match);
   }
   *n_out = emit;
+  if (count_all) {
+    // every ticket counted: any rank of the share can be emitted again from counts and offsets
+    EnumCursor &c = h->cursor;
+    c.made = true;
+    c.seq = h->api_seq;
+    c.width = WIDTH;
+    c.part = part;
+    c.nparts = nparts;
+    c.slot = L.slot;
+    c.in = in;
+    c.tickets = tickets;
+    c.total = ec.carry;
+    c.list_count = L.list_count;
+  }
   if (total != nullptr) *total = ec.carry;
   if (feasible != nullptr) *feasible = WIDTH == 7 ? (uint64_t)L.list_count : ec.feasible;
   return SBG_OK;
@@ -1504,6 +1541,68 @@ int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, s
   if (nparts < 1 || part < 0 || part >= nparts) return fail(h, SBG_ERR_ARG, "bad part %d/%d", part, nparts);
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   return SBG_OK;
+}
+
+// ---- fetch and pick on the enumeration cursor (sbg_enum_fetch / sbg_enum_pick) ---------------------
+
+int ensure_pick(sbg_handle *h, sbg_lane &L, uint64_t nranks) {
+  if (L.pick_cap >= nranks) return SBG_OK;
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  cudaFree(L.d_pranks);
+  cudaFree(L.d_pslots);
+  cudaFree(L.d_ptickets);
+  cudaFree(L.d_pfirst);
+  L.d_pranks = nullptr;
+  L.d_pslots = nullptr;
+  L.d_ptickets = nullptr;
+  L.d_pfirst = nullptr;
+  L.pick_cap = 0;
+  SBG_CUDA(h, cudaMalloc(&L.d_pranks, nranks * sizeof(unsigned long long)));
+  SBG_CUDA(h, cudaMalloc(&L.d_pslots, nranks * sizeof(unsigned int)));
+  SBG_CUDA(h, cudaMalloc(&L.d_ptickets, nranks * sizeof(unsigned long long)));
+  SBG_CUDA(h, cudaMalloc(&L.d_pfirst, (nranks + 1) * sizeof(unsigned int)));
+  L.pick_cap = nranks;
+  return SBG_OK;
+}
+
+// The cursor, if it is still valid (nothing has run on the handle since the count that made it).
+int check_cursor(sbg_handle *h) {
+  const EnumCursor &c = h->cursor;
+  if (!c.made || c.seq != h->api_seq) {
+    return fail(h, SBG_ERR_STATE, "no enumeration cursor: fetch and pick follow a counted "
+        "sbg_enum3 / sbg_enum5 / sbg_enum7 call with nothing in between");
+  }
+  const sbg_lane &L = h->lane[0];
+  if (L.slot != c.slot || L.ecount_cap < c.tickets || (c.width == 7 && L.list_count != c.list_count)) {
+    return fail(h, SBG_ERR_STATE, "internal: enumeration cursor out of step with its buffers");
+  }
+  return SBG_OK;
+}
+
+// Ticket of each of ranks[0..nranks-1] (already in L.d_pranks) into L.d_ptickets.
+int locate_tickets(sbg_handle *h, sbg_lane &L, uint64_t nranks) {
+  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nranks + 255) / 256,
+      (uint64_t)h->sm_count * 8));
+  const cudaError_t e = launch(h, k_enum_locate, grid, 256, 0, L.stream, false,
+      (const unsigned long long *)L.d_eoffset, (unsigned long long)h->cursor.tickets,
+      (const unsigned long long *)L.d_pranks, (unsigned long long)nranks, L.d_ptickets);
+  if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_locate: %s", cudaGetErrorString(e));
+  return SBG_OK;
+}
+
+// A range or pick emit pass of the cursor's width over tickets [a, b) (pick: entries [a, b) of
+// sel.tickets) into L.d_ematch; sel travels in the lane's EnumCtl block.
+template <int MODE>
+int emit_sel(sbg_handle *h, sbg_lane &L, uint64_t max_out, uint64_t a, uint64_t b,
+    const EnumSel &sel) {
+  const EnumCursor &c = h->cursor;
+  SBG_CUDA(h, cudaMemcpyAsync(reinterpret_cast<char *>(L.d_ectl) + offsetof(EnumCtl, sel), &sel,
+      sizeof(sel), cudaMemcpyHostToDevice, L.stream));
+  switch (c.width) {
+    case 3: return launch_enum<3, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
+    case 5: return launch_enum<5, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
+    default: return launch_enum<7, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
+  }
 }
 
 // LOP3 issue-rate microbenchmark (sbg_alu_peak): CHAINS independent dependent chains per thread.
@@ -1839,6 +1938,7 @@ void sbg_destroy(sbg_handle *h) {
       cudaFree(L.d_hits); cudaFree(L.d_aux); cudaFree(L.d_sorted);
       cudaFree(L.d_tcount); cudaFree(L.d_toffset); cudaFree(L.d_gcount);
       cudaFree(L.d_ectl); cudaFree(L.d_ecount); cudaFree(L.d_eoffset); cudaFree(L.d_ematch);
+      cudaFree(L.d_pranks); cudaFree(L.d_pslots); cudaFree(L.d_ptickets); cudaFree(L.d_pfirst);
       if (L.h_out != nullptr) cudaFreeHost(L.h_out);
       if (L.h_ctl != nullptr) cudaFreeHost(L.h_ctl);
       for (int k = 0; k < 8; k++) if (L.ev[k] != nullptr) cudaEventDestroy(L.ev[k]);
@@ -1904,6 +2004,7 @@ float sbg_last_kernel_ms(const sbg_handle *h, int which) {
 
 int sbg_alu_peak(sbg_handle *h, double *warp_instr_per_s) {
   if (h == nullptr || warp_instr_per_s == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   SBG_CUDA(h, cudaSetDevice(h->device));
   const int blocks = h->sm_count * 8, threads = 256, iters = 2048;
   constexpr int CH = 8;
@@ -1927,6 +2028,7 @@ int sbg_alu_peak(sbg_handle *h, double *warp_instr_per_s) {
 
 int sbg_use_problem(sbg_handle *h, int slot) {
   if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   if (slot < 0 || slot >= kSlots) return fail(h, SBG_ERR_ARG, "slot %d out of range", slot);
   if (!h->slots[slot].ready) return fail(h, SBG_ERR_STATE, "slot %d holds no problem", slot);
   h->cur_slot = slot;
@@ -1939,6 +2041,7 @@ int sbg_use_problem(sbg_handle *h, int slot) {
 int sbg_stage_problem(sbg_handle *h, int slot, const uint64_t *tables, int n,
     const uint64_t *target, const uint64_t *mask, const int8_t *inbits) {
   if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   SBG_CUDA(h, cudaSetDevice(h->device));
   return stage_problem(h, slot, tables, n, target, mask, inbits, true);
 }
@@ -1946,6 +2049,7 @@ int sbg_stage_problem(sbg_handle *h, int slot, const uint64_t *tables, int n,
 int sbg_load_problem(sbg_handle *h, const uint64_t *tables, int n, const uint64_t *target,
     const uint64_t *mask, const int8_t *inbits) {
   if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   SBG_CUDA(h, cudaSetDevice(h->device));
   // lazily: the difference to the resident state rides in the next chain's first kernel
   int rc = stage_problem(h, 0, tables, n, target, mask, inbits, false);
@@ -1956,6 +2060,7 @@ int sbg_load_problem(sbg_handle *h, const uint64_t *tables, int n, const uint64_
 int sbg_search5_part(sbg_handle *h, int part, int nparts, const uint8_t *func_order,
     uint64_t *key) {
   if (h == nullptr || key == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   const sbg_handle::HostProblem &hp = cur(h);
   if (hp.n < 5) return fail(h, SBG_ERR_ARG, "search_5lut needs n >= 5 (lut.c:119)");
@@ -1990,6 +2095,7 @@ int sbg_search5_part(sbg_handle *h, int part, int nparts, const uint8_t *func_or
 
 int sbg_finish5(sbg_handle *h, uint64_t key, const uint8_t *func_order, sbg_result *res) {
   if (h == nullptr || res == nullptr || func_order == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   return finish5_slot(h, cur(h), key, func_order, h->feasible, h->swept, res);
 }
@@ -2003,6 +2109,7 @@ int sbg_search5(sbg_handle *h, const uint8_t *func_order, sbg_result *res) {
 
 int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *count) {
   if (h == nullptr || count == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   if (cur(h).n < 7) return fail(h, SBG_ERR_ARG, "search_7lut needs n >= 7 (lut.c:259)");
   if (nparts < 1 || part < 0 || part >= nparts) return fail(h, SBG_ERR_ARG, "bad part %d/%d", part, nparts);
@@ -2030,6 +2137,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
 
 int sbg_list7_device(sbg_handle *h, const uint64_t **list, int *count) {
   if (h == nullptr || list == nullptr || count == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   *list = h->lane[0].d_sorted;
   *count = (int)h->lane[0].list_count;
   return SBG_OK;
@@ -2039,6 +2147,7 @@ int sbg_list7_device(sbg_handle *h, const uint64_t **list, int *count) {
 int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, const int *counts,
     int nruns) {
   if (h == nullptr || counts == nullptr || nruns < 0 || nruns > kMaxRuns) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
   int rc;
@@ -2064,6 +2173,7 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
 
 int sbg_set_list7(sbg_handle *h, const uint64_t *list, int count) {
   if (h == nullptr || count < 0 || (count > 0 && list == nullptr)) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
   int rc;
@@ -2113,6 +2223,7 @@ int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total) {
   *total = 0;
   for (int i = 0; i < nh; i++) {
     if (hs[i] == nullptr) return SBG_ERR_ARG;
+    hs[i]->api_seq++;   // ends the enumeration cursor
     counts[i] = (int)hs[i]->lane[0].list_count;
     stride = std::max<uint64_t>(stride, (uint64_t)counts[i]);
     *total += counts[i];
@@ -2156,6 +2267,7 @@ int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total) {
 int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t *key) {
   if (h == nullptr || key == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   sbg_lane &L = h->lane[0];
   if (!L.list_ready) return fail(h, SBG_ERR_STATE, "no 7-LUT list installed");
@@ -2193,6 +2305,7 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
   if (h == nullptr || res == nullptr || outer_order == nullptr || middle_order == nullptr) {
     return SBG_ERR_ARG;
   }
+  h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   sbg_lane &L = h->lane[0];
   uint64_t pair[2] = {0, 0};
@@ -2221,6 +2334,7 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
 
 int sbg_search_node(sbg_handle *h, const sbg_job *job, sbg_node_result *res) {
   if (h == nullptr || job == nullptr || res == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   int rc;
   const double t0 = wall_now();
   if ((rc = check_job(h, job)) != SBG_OK) return rc;
@@ -2255,6 +2369,7 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
   if (h == nullptr || njobs < 0 || (njobs > 0 && (jobs == nullptr || results == nullptr))) {
     return SBG_ERR_ARG;
   }
+  h->api_seq++;   // ends the enumeration cursor
   int rc;
   for (int j = 0; j < njobs; j++) {
     if ((rc = check_job(h, &jobs[j])) != SBG_OK) return rc;
@@ -2312,6 +2427,7 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
 int sbg_search7(sbg_handle *h, const uint8_t *outer_order, const uint8_t *middle_order,
     sbg_result *res) {
   if (h == nullptr || res == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   if (cur(h).n < 7) return fail(h, SBG_ERR_ARG, "search_7lut needs n >= 7 (lut.c:259)");
   sbg_job job;
@@ -2330,6 +2446,7 @@ int sbg_search7(sbg_handle *h, const uint8_t *outer_order, const uint8_t *middle
 int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, uint64_t max_matches,
     sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible) {
   if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   int rc;
   if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
   const sbg_handle::HostProblem &hp = cur(h);
@@ -2356,6 +2473,7 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
     uint64_t *total, uint64_t *feasible) {
   if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   int rc;
   if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
   if (cur(h).n < 7) return fail(h, SBG_ERR_ARG, "search_7lut needs n >= 7 (lut.c:259)");
@@ -2387,6 +2505,7 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
 int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
     uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible) {
   if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
   int rc;
   if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
   const int n = cur(h).n;
@@ -2415,6 +2534,110 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
   memcpy(in3.gates.order, gate_order, sizeof(uint16_t) * (size_t)n);
   return run_enum<3>(h, L, in3, part, nparts, mine * kDeal, max_matches, out, n_out, total,
       feasible);
+}
+
+int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out, uint64_t *n_out) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  if (n_out == nullptr || (count > 0 && out == nullptr)) return fail(h, SBG_ERR_ARG, "null output");
+  if (count > SBG_ENUM_MAX_MATCHES) {
+    return fail(h, SBG_ERR_ARG, "count %llu above %u", (unsigned long long)count,
+        SBG_ENUM_MAX_MATCHES);
+  }
+  int rc;
+  if ((rc = check_cursor(h)) != SBG_OK) return rc;
+  const EnumCursor &c = h->cursor;
+  *n_out = 0;
+  if (first >= c.total || count == 0) return SBG_OK;
+  const uint64_t n = std::min(count, c.total - first);
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  if ((rc = ensure_pick(h, L, 2)) != SBG_OK) return rc;
+  if ((rc = ensure_enum(h, L, 0, n)) != SBG_OK) return rc;
+  // the tickets of the window's first and last rank; the launch covers them and those between
+  const unsigned long long ends[2] = {first, first + n - 1};
+  unsigned long long tk[2] = {0, 0};
+  SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, ends, sizeof(ends), cudaMemcpyHostToDevice, L.stream));
+  if ((rc = locate_tickets(h, L, 2)) != SBG_OK) return rc;
+  SBG_CUDA(h, cudaMemcpyAsync(tk, L.d_ptickets, sizeof(tk), cudaMemcpyDeviceToHost, L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  EnumSel sel;
+  memset(&sel, 0, sizeof(sel));
+  sel.lo = first;
+  if ((rc = emit_sel<kEnumRange>(h, L, first + n, tk[0], tk[1] + 1, sel)) != SBG_OK) return rc;
+  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, n * sizeof(sbg_match), cudaMemcpyDeviceToHost,
+      L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  h->d2h_bytes += n * sizeof(sbg_match);
+  *n_out = n;
+  return SBG_OK;
+}
+
+int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_match *out) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  if (nranks > 0 && (ranks == nullptr || out == nullptr)) return fail(h, SBG_ERR_ARG, "null ranks or output");
+  if (nranks > SBG_ENUM_MAX_MATCHES) {
+    return fail(h, SBG_ERR_ARG, "nranks %llu above %u", (unsigned long long)nranks,
+        SBG_ENUM_MAX_MATCHES);
+  }
+  int rc;
+  if ((rc = check_cursor(h)) != SBG_OK) return rc;
+  const EnumCursor &c = h->cursor;
+  for (uint64_t i = 0; i < nranks; i++) {
+    if (ranks[i] >= c.total) {
+      return fail(h, SBG_ERR_ARG, "ranks[%llu] = %llu is not below the total %llu",
+          (unsigned long long)i, (unsigned long long)ranks[i], (unsigned long long)c.total);
+    }
+  }
+  if (nranks == 0) return SBG_OK;
+  // host: the ranks in ascending order with the slots that asked for them
+  std::vector<std::pair<uint64_t, uint32_t>> req(nranks);
+  for (uint64_t i = 0; i < nranks; i++) req[i] = std::make_pair(ranks[i], (uint32_t)i);
+  std::sort(req.begin(), req.end());
+  std::vector<unsigned long long> sorted(nranks);
+  std::vector<unsigned int> slots(nranks);
+  for (uint64_t i = 0; i < nranks; i++) {
+    sorted[i] = req[i].first;
+    slots[i] = req[i].second;
+  }
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  if ((rc = ensure_pick(h, L, nranks)) != SBG_OK) return rc;
+  if ((rc = ensure_enum(h, L, 0, nranks)) != SBG_OK) return rc;
+  // device: the ticket of every rank; host: the distinct tickets and their slices of the ranks
+  SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, sorted.data(), nranks * sizeof(unsigned long long),
+      cudaMemcpyHostToDevice, L.stream));
+  if ((rc = locate_tickets(h, L, nranks)) != SBG_OK) return rc;
+  std::vector<unsigned long long> tickets(nranks);
+  SBG_CUDA(h, cudaMemcpyAsync(tickets.data(), L.d_ptickets, nranks * sizeof(unsigned long long),
+      cudaMemcpyDeviceToHost, L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  std::vector<unsigned int> firsts;
+  uint64_t d = 0;
+  for (uint64_t i = 0; i < nranks; i++) {
+    if (i == 0 || tickets[i] != tickets[d - 1]) {
+      tickets[d++] = tickets[i];
+      firsts.push_back((unsigned int)i);
+    }
+  }
+  firsts.push_back((unsigned int)nranks);
+  SBG_CUDA(h, cudaMemcpyAsync(L.d_ptickets, tickets.data(), d * sizeof(unsigned long long),
+      cudaMemcpyHostToDevice, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(L.d_pfirst, firsts.data(), (d + 1) * sizeof(unsigned int),
+      cudaMemcpyHostToDevice, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(L.d_pslots, slots.data(), nranks * sizeof(unsigned int),
+      cudaMemcpyHostToDevice, L.stream));
+  EnumSel sel;
+  sel.lo = 0;
+  sel.ranks = L.d_pranks;
+  sel.slots = L.d_pslots;
+  sel.tickets = L.d_ptickets;
+  sel.first = L.d_pfirst;
+  if ((rc = emit_sel<kEnumPick>(h, L, 0, 0, d, sel)) != SBG_OK) return rc;
+  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, nranks * sizeof(sbg_match), cudaMemcpyDeviceToHost,
+      L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  h->d2h_bytes += nranks * sizeof(sbg_match);
+  return SBG_OK;
 }
 
 }  // extern "C"

@@ -2347,6 +2347,45 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
 //     decoded into DevMatch records.
 // Tickets are numbered in key order, so the order needs no sort.  Both passes run the identical
 // sweep, so a ticket emits exactly the matches it counted.
+//
+// After a count, any rank of the share can be emitted again from counts and offsets alone
+// (sbg_enum_fetch / sbg_enum_pick): the emit pass of the same sweep, run over the tickets that hold
+// the wanted ranks only (k_enum_locate finds them).  The pass's mode (template parameter MODE):
+//   kEnumCount  the count pass;
+//   kEnumFirst  the first K (max_out = K), ranks [0, K) to out[rank];
+//   kEnumRange  ranks [sel.lo, max_out) to out[rank - sel.lo];
+//   kEnumPick   one warp per ticket of sel.tickets, writing each rank of its slice of sel.ranks to
+//               out[sel.slots[...]] (duplicate ranks: every slot that asked for it).
+// The kernels keep one parameter list for all modes; sel reaches the range and pick forms in the
+// lane's EnumCtl block.
+enum EnumMode : int { kEnumCount = 0, kEnumFirst = 1, kEnumRange = 2, kEnumPick = 3 };
+
+struct EnumSel {
+  unsigned long long lo;                  // kEnumRange: first rank of the window
+  const unsigned long long *ranks;        // kEnumPick: the requested ranks, ascending, duplicates kept
+  const unsigned int *slots;              //   the output slot of each of them
+  const unsigned long long *tickets;      //   the distinct tickets holding them, ascending
+  const unsigned int *first;              //   ticket j's ranks: ranks[first[j] .. first[j+1]-1]
+};
+
+// One step of an emit sweep: the warp's ballot covers ranks [step_end - popc(ballot), step_end), the
+// lane's own match (if hit) has rank `at`.  write(i) writes the lane's match to out[i].  Pick: the
+// requests of this step are consumed in order from req (warp-uniform), each written by the lane that
+// holds its rank.
+template <int MODE, class Write>
+__device__ __forceinline__ void emit_step(bool hit, unsigned long long at, unsigned long long step_end,
+    unsigned long long max_out, const EnumSel &sel, unsigned int &req, unsigned int req_end,
+    Write write) {
+  if (MODE == kEnumPick) {
+    for (; req < req_end; req++) {
+      const unsigned long long r = sel.ranks[req];
+      if (r >= step_end) break;
+      if (hit && at == r) write((unsigned long long)sel.slots[req]);
+    }
+  } else if (hit && at < max_out && (MODE != kEnumRange || at >= sel.lo)) {
+    write(MODE == kEnumRange ? at - sel.lo : at);
+  }
+}
 
 // The layout of sbg_match (include/sboxgates_b200.h; sbg_api.cu checks that the two agree).
 struct DevMatch {
@@ -2361,6 +2400,7 @@ struct EnumCtl {
   unsigned long long total;     // matches counted so far (all windows of the call)
   unsigned long long feasible;  // 5-LUT: feasible tuples met
   unsigned long long carry;     // k_enum_scan: matches in front of the next window
+  EnumSel sel;                  // range / pick emit: what to emit (set by the host before the pass)
 };
 
 struct EnumOrders {
@@ -2420,13 +2460,17 @@ __device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned
 
 // The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
 // 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
-// feasible tuple and ordering the set of working outer functions from outer_ok5.
-template <int NW, bool EMIT>
+// feasible tuple and ordering the set of working outer functions from outer_ok5.  Pick: j runs over
+// sel.tickets instead.
+template <int NW, int MODE>
 __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts, const DevTables *__restrict__ tab) {
+  constexpr bool EMIT = MODE != kEnumCount;
+  EnumSel sel = {};
+  if (MODE == kEnumRange || MODE == kEnumPick) sel = ectl->sel;
   constexpr int P = 3, K = 5, NC = 1 << P;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[256];
@@ -2450,11 +2494,18 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
   const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
   unsigned long long feasible_local = 0, matches_local = 0;
 
-  for (unsigned long long t = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
-       t < t_end; t += nwarps) {
+  for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
+       j < t_end; j += nwarps) {
+    const unsigned long long t = MODE == kEnumPick ? sel.tickets[j] : j;
     unsigned long long base = 0;
+    unsigned int req = 0, req_end = 0;
     if (EMIT) {
-      if (counts[t] == 0 || offsets[t] >= max_out) continue;
+      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
+      if (MODE == kEnumRange && offsets[t] + counts[t] <= sel.lo) continue;
+      if (MODE == kEnumPick) {
+        req = sel.first[j];
+        req_end = sel.first[j + 1];
+      }
       base = offsets[t];
     }
     // prefixes are dealt to the parts in blocks of kDeal, as k_sweep deals them
@@ -2547,12 +2598,13 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
               const bool hit = (__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u;
               const uint32_t bal = __ballot_sync(kFull, hit);
               const unsigned long long at = base + count + __popc(bal & lanemask_lt());
-              if (hit && at < max_out) {
-                write_match<NW, 5>(out + at, key_hi | pos, g5, k, fo, 0, s_tabs, npad, T, M);
-              }
+              emit_step<MODE>(hit, at, base + count + __popc(bal), max_out, sel, req, req_end,
+                  [&](unsigned long long i) {
+                    write_match<NW, 5>(out + i, key_hi | pos, g5, k, fo, 0, s_tabs, npad, T, M);
+                  });
               count += __popc(bal);
             }
-            done = base + count >= max_out;
+            done = MODE == kEnumPick ? req >= req_end : base + count >= max_out;
           }
         }
       }
@@ -2596,14 +2648,18 @@ __device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (
 // nparts + part), one warp per entry: the summary and stage-1 filter of k_decomp7 on the TRUE gate
 // tables (no stale outer cache), then per surviving outer function and ordering row the union of
 // the middle-function cubes.  Count: one lane per outer function; emit: positions in ascending
-// order, outer position in the loop, middle position across the lanes.
-template <int NW, bool EMIT>
+// order, outer position in the loop, middle position across the lanes.  Pick: j runs over
+// sel.tickets instead.
+template <int NW, int MODE>
 __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts, const DevTables *__restrict__ tab) {
+  constexpr bool EMIT = MODE != kEnumCount;
+  EnumSel sel = {};
+  if (MODE == kEnumRange || MODE == kEnumPick) sel = ectl->sel;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
   __shared__ uint8_t s_fo[kWarpsPerCta][256];
@@ -2629,12 +2685,19 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
   const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
   unsigned long long matches_local = 0;
 
-  for (unsigned long long t = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
-       t < t_end; t += nwarps) {
+  for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
+       j < t_end; j += nwarps) {
+    const unsigned long long t = MODE == kEnumPick ? sel.tickets[j] : j;
     const uint64_t idx = t * (uint64_t)nparts + (uint64_t)part;
     unsigned long long base = 0;
+    unsigned int req = 0, req_end = 0;
     if (EMIT) {
-      if (counts[t] == 0 || offsets[t] >= max_out) continue;
+      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
+      if (MODE == kEnumRange && offsets[t] + counts[t] <= sel.lo) continue;
+      if (MODE == kEnumPick) {
+        req = sel.first[j];
+        req_end = sel.first[j + 1];
+      }
       base = offsets[t];
     }
     uint32_t count = 0;
@@ -2722,12 +2785,13 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
               }
               const uint32_t bal = __ballot_sync(kFull, hit);
               const unsigned long long at = base + count + __popc(bal & lanemask_lt());
-              if (hit && at < max_out) {
-                write_match<NW, 7>(out + at, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
-              }
+              emit_step<MODE>(hit, at, base + count + __popc(bal), max_out, sel, req, req_end,
+                  [&](unsigned long long i) {
+                    write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
+                  });
               count += __popc(bal);
             }
-            done = base + count >= max_out;
+            done = MODE == kEnumPick ? req >= req_end : base + count >= max_out;
           }
         }
       }
@@ -2739,6 +2803,7 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
   }
   if (!EMIT && lane == 0 && matches_local != 0) atomicAdd(&ectl->total, matches_local);
 }
+
 
 // The caller's shuffled gate order of the 3-LUT enumeration: position -> gate.
 struct EnumGateOrder {
@@ -2752,13 +2817,16 @@ struct EnumGateOrder {
 // of the target (scan3_blocks' test, here on the compressed tables).  Key i << 18 | k << 9 | m, so a
 // ticket's matches are consecutive keys in the order of its lanes.  A match's record: the gates in
 // position order, func_inner = cells holding a masked 1, inner_seen = cells holding a masked
-// position (sbg_solve_inner's closed form).
-template <int NW, bool EMIT>
+// position (sbg_solve_inner's closed form).  Pick: j runs over sel.tickets instead.
+template <int NW, int MODE>
 __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts) {
+  constexpr bool EMIT = MODE != kEnumCount;
+  EnumSel sel = {};
+  if (MODE == kEnumRange || MODE == kEnumPick) sel = ectl->sel;
   extern __shared__ uint32_t smem[];
   __shared__ uint16_t s_order[kMaxGatesPad];
   const int lane = threadIdx.x & 31;
@@ -2779,11 +2847,18 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
   const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
   unsigned long long matches_local = 0;
 
-  for (unsigned long long t = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
-       t < t_end; t += nwarps) {
+  for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
+       j < t_end; j += nwarps) {
+    const unsigned long long t = MODE == kEnumPick ? sel.tickets[j] : j;
     unsigned long long base = 0;
+    unsigned int req = 0, req_end = 0;
     if (EMIT) {
-      if (counts[t] == 0 || offsets[t] >= max_out) continue;
+      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
+      if (MODE == kEnumRange && offsets[t] + counts[t] <= sel.lo) continue;
+      if (MODE == kEnumPick) {
+        req = sel.first[j];
+        req_end = sel.first[j + 1];
+      }
       base = offsets[t];
     }
     const uint64_t dealt = (t / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal + t % kDeal;
@@ -2821,26 +2896,27 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
         const uint32_t bal = __ballot_sync(kFull, ok);
         if (EMIT) {
           const unsigned long long at = base + count + __popc(bal & lanemask_lt());
-          if (ok && at < max_out) {
-            DevMatch m;
-            m.key = ((unsigned long long)pi << 18) | ((unsigned long long)pk << 9) | (unsigned)pm;
-            m.gates[0] = s_order[pi];
-            m.gates[1] = s_order[pk];
-            m.gates[2] = s_order[pm];
+          emit_step<MODE>(ok, at, base + count + __popc(bal), max_out, sel, req, req_end,
+              [&](unsigned long long dst) {
+                DevMatch m;
+                m.key = ((unsigned long long)pi << 18) | ((unsigned long long)pk << 9) | (unsigned)pm;
+                m.gates[0] = s_order[pi];
+                m.gates[1] = s_order[pk];
+                m.gates[2] = s_order[pm];
 #pragma unroll
-            for (int i = 3; i < 7; i++) m.gates[i] = 0;
-            m.func_outer = 0;
-            m.func_middle = 0;
-            m.func_inner = (uint8_t)ones;
-            m.inner_seen = (uint8_t)seen;
-            m.width = 3;
+                for (int i = 3; i < 7; i++) m.gates[i] = 0;
+                m.func_outer = 0;
+                m.func_middle = 0;
+                m.func_inner = (uint8_t)ones;
+                m.inner_seen = (uint8_t)seen;
+                m.width = 3;
 #pragma unroll
-            for (int i = 0; i < 5; i++) m.pad[i] = 0;
-            out[at] = m;
-          }
+                for (int i = 0; i < 5; i++) m.pad[i] = 0;
+                out[dst] = m;
+              });
         }
         count += __popc(bal);
-        done = EMIT && base + count >= max_out;
+        done = EMIT && (MODE == kEnumPick ? req >= req_end : base + count >= max_out);
       }
     }
     if (!EMIT) {
@@ -2852,6 +2928,25 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
   if (!EMIT && lane == 0 && matches_local != 0) {
     atomicAdd(&ectl->total, matches_local);
     atomicAdd(&ectl->feasible, matches_local);
+  }
+}
+
+
+// The ticket of each requested rank (ranks[i] < the count pass's total): the last t < tickets with
+// offsets[t] <= ranks[i], by binary search over the count pass's offsets.  A ticket without matches
+// has its successor's offset, so it is never the answer.
+__global__ void __launch_bounds__(256) k_enum_locate(const unsigned long long *__restrict__ offsets,
+    unsigned long long tickets, const unsigned long long *__restrict__ ranks,
+    unsigned long long nranks, unsigned long long *__restrict__ ticket_of) {
+  for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nranks;
+       i += (unsigned long long)gridDim.x * blockDim.x) {
+    const unsigned long long r = ranks[i];
+    unsigned long long lo = 0, hi = tickets;   // offsets[lo] <= r (offsets[0] = 0), offsets[hi] > r
+    while (hi - lo > 1) {
+      const unsigned long long mid = lo + (hi - lo) / 2;
+      if (offsets[mid] <= r) lo = mid; else hi = mid;
+    }
+    ticket_of[i] = lo;
   }
 }
 

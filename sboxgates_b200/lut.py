@@ -386,6 +386,57 @@ class LutEngine:
         buf = (C.c_uint16 * go.shape[0]).from_buffer_copy(go.tobytes())
         return self._enumerate(self.lib.sbg_enum3, [buf], max_matches, count, part, nparts)
 
+    # -- matches at any rank of the last counted enumeration (the cursor) -----------------------
+    def fetch_matches(self, first, count):
+        """The matches at ranks first .. min(first + count, total) - 1 of the last counted
+        enumeration on this engine (ranks within its share, ascending key order), as a MATCH_DTYPE
+        array: the same records that enumeration emits at those ranks.  Nothing is counted again.
+        Raises RuntimeError if something other than a fetch, a pick or a query ran on the engine
+        since that enumeration (the cursor is gone)."""
+        first, count = int(first), int(count)
+        if not 0 <= first < 2**64:
+            raise ValueError("first must lie in 0..2**64-1")
+        if not 0 <= count <= SBG_ENUM_MAX_MATCHES:
+            raise ValueError("count must lie in 0..%d" % SBG_ENUM_MAX_MATCHES)
+        out = np.zeros(max(count, 1), dtype=MATCH_DTYPE)
+        n_out = C.c_uint64()
+        self._check(self.lib.sbg_enum_fetch(self._h, first, count, out.ctypes.data_as(C.c_void_p),
+                                            C.byref(n_out)))
+        return out[:n_out.value].copy()
+
+    def pick_matches(self, ranks):
+        """The matches at the given ranks of the last counted enumeration, in the order of `ranks`
+        (a 1-D integer array; any order, repeats allowed, each below the total)."""
+        r = np.asarray(ranks)
+        if r.ndim != 1 or (r.size > 0 and r.dtype.kind not in "iu"):
+            raise ValueError("ranks must be a 1-D integer array")
+        if r.shape[0] > SBG_ENUM_MAX_MATCHES:
+            raise ValueError("at most %d ranks per pick" % SBG_ENUM_MAX_MATCHES)
+        if r.size > 0 and r.dtype.kind == "i" and int(r.min()) < 0:
+            raise ValueError("ranks must not be negative")
+        r = np.ascontiguousarray(r, dtype=np.uint64)
+        out = np.zeros(max(r.shape[0], 1), dtype=MATCH_DTYPE)
+        self._check(self.lib.sbg_enum_pick(self._h, r.ctypes.data_as(native.u64p), r.shape[0],
+                                           out.ctypes.data_as(C.c_void_p)))
+        return out[:r.shape[0]].copy()
+
+
+def sample_matches(engine, enumeration, k, seed=None):
+    """k distinct matches drawn uniformly from the whole match set of `enumeration`, which must be
+    the last counted enumeration on `engine` (its cursor): returns (ranks, matches) with the ranks
+    ascending and matches[i] the match at ranks[i].  The ranks come from
+    numpy.random.default_rng(seed).choice(total, k, replace=False); the reference has no sampling,
+    so no xorshift1024 stream is involved and the caller's RNG stays untouched."""
+    if enumeration.total is None:
+        raise ValueError("the enumeration was not counted (count=False): it has no cursor")
+    k, total = int(k), int(enumeration.total)
+    if not 0 <= k <= total:
+        raise ValueError("k must lie in 0..%d (the enumeration's total)" % total)
+    if k > SBG_ENUM_MAX_MATCHES:
+        raise ValueError("at most %d matches per sample" % SBG_ENUM_MAX_MATCHES)
+    ranks = np.sort(np.random.default_rng(seed).choice(total, k, replace=False)).astype(np.uint64)
+    return ranks, engine.pick_matches(ranks)
+
 
 def unpack_tuple7(packed):
     """63-bit packed 7-combination -> list of gate numbers."""

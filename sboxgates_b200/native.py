@@ -104,6 +104,8 @@ SIGNATURES = {
                             u64p, u64p]),
     "sbg_enum3": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint16), C.c_uint64,
                             C.c_void_p, u64p, u64p, u64p]),
+    "sbg_enum_fetch": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, u64p]),
+    "sbg_enum_pick": (C.c_int, [C.c_void_p, u64p, C.c_uint64, C.c_void_p]),
 }
 
 _lib = None
