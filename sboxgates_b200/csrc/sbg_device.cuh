@@ -2129,6 +2129,78 @@ __device__ __forceinline__ void middle_cubes(uint32_t r1, uint32_t r0, int b, ui
   ov = hs[0] & hs[1];
 }
 
+// Moves index bit b of both 16-bit halves of r to bit 3, bits b+1..3 one place down (the other
+// bits keep their order), so that compress16x2(r, b, z) == compress16x2(index_bit_to_top(r, b), 3, z).
+// Branch-free: b differs from lane to lane in k_decomp7's stage 2.
+__device__ __forceinline__ uint32_t index_bit_to_top(uint32_t r, int b) {
+  uint32_t t = ((r >> 1) ^ r) & (b <= 0 ? 0x22222222u : 0u);   // exchange index bits 0 and 1
+  r ^= t ^ (t << 1);
+  t = ((r >> 2) ^ r) & (b <= 1 ? 0x0c0c0c0cu : 0u);            // 1 and 2
+  r ^= t ^ (t << 2);
+  t = ((r >> 4) ^ r) & (b <= 2 ? 0x00f000f0u : 0u);            // 2 and 3
+  return r ^ t ^ (t << 4);
+}
+
+// k_decomp7's stage 2 for entries p0 .. min(p0 + 32, nent) - 1 of a tuple's entry list, one lane
+// each.  Entry = j << 9 | row << 7 | fo: outer function fo (bit 7 clear; it stands for fo and ~fo)
+// of outer triple j, ordering row `row` of that triple.  sW[9 j + u] = W[u] of triple j (outer_ok7),
+// sW[9 j + 8] = its first ordering number | (bit of v4 that is the g input, 2 bits per row) << 8.
+// Complementing fo swaps r1 and r0, which middle_cubes answers with the same S, ov and set of cubes,
+// so both members of a pair have the same best middle position and the pair's outer position is the
+// smaller of the two (s_pmin).  Returns the smallest k << 16 | po << 8 | pm with a match over the
+// warp's entries, 0xffffffff if none.
+__device__ __forceinline__ uint32_t decomp7_entries(const uint16_t *ent, int p0, int nent,
+    const uint32_t *sW, const uint8_t *s_pmin, const uint8_t *s_minpos, const uint16_t *s_p3,
+    int lane) {
+  const bool have = p0 + lane < nent;
+  const uint32_t e = have ? ent[p0 + lane] : 0u;
+  const uint32_t fo = e & 0x7fu, row = (e >> 7) & 3u;
+  const uint32_t *w = sW + 9 * (e >> 9);   // stride 9: lanes on different triples, different banks
+  uint32_t r1 = 0, r0 = 0;
+#pragma unroll
+  for (int u = 0; u < 8; u++) {
+    const uint32_t wu = w[u];
+    if ((fo >> u) & 1) r1 |= wu; else r0 |= wu;
+  }
+  const uint32_t info = w[8];
+  const int b = (int)((info >> (8 + 2 * row)) & 3u);
+  uint32_t hv[2][4], S, ov;
+  bool hok[2][4];
+  middle_cubes(index_bit_to_top(r1, b), index_bit_to_top(r0, b), 3, hv, hok, S, ov);
+  // which of the 16 ways to pick are consistent; every consistent way is a non-empty cube, i.e. a
+  // match.  Entries of dense lists almost never match, so the warp looks positions up only when
+  // one of its lanes has a match.
+  uint32_t picks = 0;
+#pragma unroll
+  for (int c0 = 0; c0 < 4; c0++) {
+#pragma unroll
+    for (int c1 = 0; c1 < 4; c1++) {
+      const bool ok2 = hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0;
+      if (ok2) picks |= 1u << (4 * c0 + c1);
+    }
+  }
+  if (!have) picks = 0;
+  if (!__any_sync(kFull, picks != 0)) return 0xffffffffu;
+  const uint32_t p3s = s_p3[S];
+  uint32_t best_pm = 256;
+#pragma unroll
+  for (int c0 = 0; c0 < 4; c0++) {
+#pragma unroll
+    for (int c1 = 0; c1 < 4; c1++) {
+      if ((picks >> (4 * c0 + c1)) & 1u) {
+        const uint32_t V = hv[0][c0] | hv[1][c1];
+        best_pm = min(best_pm, (uint32_t)s_minpos[p3s + s_p3[V]]);
+      }
+    }
+  }
+  uint32_t cand = 0xffffffffu;
+  if (picks != 0) cand = (((info & 0x7fu) + row) << 16) | ((uint32_t)s_pmin[fo] << 8) | best_pm;
+  return __reduce_min_sync(kFull, cand);
+}
+
+// k_decomp7's per-warp entry list: at most 31 entries carried over + 128 pairs x 4 rows of a triple
+constexpr int kDecompEntries = 31 + 128 * 4;
+
 template <int NW>
 __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restrict__ prob,
     DevCtl *__restrict__ ctl, HostOut *__restrict__ out, const DevParams7 *__restrict__ par,
@@ -2137,12 +2209,11 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_minpos[kMinpos3 + 3];
   __shared__ uint16_t s_p3[256];
-  __shared__ uint8_t s_pos[256];         // outer function -> its position in the shuffled order
-  __shared__ uint8_t s_ord[256];         // position -> outer function
-  __shared__ uint8_t s_fo[kWarpsPerCta][256];
+  __shared__ uint8_t s_pmin[128];        // fo < 128 -> smaller shuffled position of fo and ~fo
   __shared__ uint32_t s_src7[25 * 32];   // copy of DevTables::src7
-  __shared__ uint32_t s_H[kWarpsPerCta][24];
-  __shared__ uint32_t s_row_best[kWarpsPerCta][4];
+  __shared__ uint32_t s_H[kWarpsPerCta][16];
+  __shared__ uint32_t s_W[kWarpsPerCta][25 * 9];            // per outer triple: W[8], row info
+  __shared__ uint16_t s_ent[kWarpsPerCta][kDecompEntries];  // (triple, row, outer pair) entries
 
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -2171,10 +2242,8 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
       ? (count - (unsigned int)part + (unsigned int)nparts - 1) / (unsigned int)nparts : 0u;
   if (blockIdx.x * kWarpsPerCta < share) {
   for (int i = threadIdx.x; i < kMinpos3; i += blockDim.x) s_minpos[i] = par->minpos3[i];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-    const uint8_t po = par->pos_outer[i];
-    s_pos[i] = po;
-    s_ord[po] = (uint8_t)i;
+  for (int i = threadIdx.x; i < 128; i += blockDim.x) {
+    s_pmin[i] = min(par->pos_outer[i], par->pos_outer[255 - i]);
   }
   __syncthreads();
 
@@ -2223,95 +2292,100 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
       tuple_summary<NW>(s_tabs, npad, g2, T, M, lane, sH + 8);
     }
 
-    bool found = false;
-    uint64_t key = 0;
-    for (int j = 0; j < 25 && !found; j++) {
+    // Stage 1 proper per passing outer triple, in order j; its survivors come in complementary
+    // pairs (fo, ~fo), and each pair goes on the warp's entry list once per ordering row of the
+    // triple.  Stage 2 then takes 32 (pair, row) entries at a time, one lane each, so that rows and
+    // triples with few survivors share passes.  Ordering numbers grow with j, so the smallest
+    // k << 16 | po << 8 | pm over all entries is the first match: full passes run as the list
+    // fills, and once one of them matches, the entries left over and nothing after them decide.
+    uint32_t *sW = s_W[warp];
+    uint16_t *ent = s_ent[warp];
+    uint32_t best = 0xffffffffu;
+    int nent = 0;
+#ifdef SBG_COUNT_STAGE1
+    unsigned long long n_pairs = 0, n_passes = 0, n_row_passes = 0;
+#endif
+    for (int j = 0; j < 25; j++) {
       if (((pass_i >> j) & 1u) == 0) continue;   // the filter found no admissible outer function
       const uint32_t *Hs = (stale && j == 0) ? sH + 8 : sH;
       uint32_t W[8], ok[8];
       outer_ok7(Hs, s_src7[j * 32 + lane], lane, W, ok);
-      uint32_t any = 0;
-      uint32_t my_surv = 0;
+      uint32_t sv[4], any = 0;
 #pragma unroll
-      for (int hi = 0; hi < 8; hi++) {
-        const uint32_t sv = ok[hi] & __brev(ok[7 - hi]);
-        any |= sv;
-        if (lane == hi) my_surv = sv;
+      for (int hi = 0; hi < 4; hi++) {   // the pair's member without bit 7
+        sv[hi] = ok[hi] & __brev(ok[7 - hi]);
+        any |= sv[hi];
       }
 #ifdef SBG_COUNT_STAGE1
       if (lane == 0) atomicAdd(&ctl->pad0[0], 1ull);                    // (tuple, outer triple) pairs
       if (lane == 0 && any != 0) atomicAdd(&ctl->pad0[1], 1ull);        // ... with survivors
 #endif
       if (any == 0) continue;  // no outer function leaves a conflict-free 5-input remainder
-      uint32_t *surv = sH + 16;
-      __syncwarp();
-      if (lane < 8) surv[lane] = my_surv;
-      __syncwarp();
-
-      // Stage 2, one lane per surviving outer function.  First compact the survivors.
-      uint8_t *fo_list = s_fo[warp];
-      int ns = 0;
-#pragma unroll
-      for (int hi = 0; hi < 8; hi++) {
-        const uint32_t sv = surv[hi];
-        if ((sv >> lane) & 1u) fo_list[ns + __popc(sv & lanemask_lt())] = (uint8_t)(hi * 32 + lane);
-        ns += __popc(sv);
-      }
-      __syncwarp();
-
       const int k0 = c_j_first_k[j];
       const int nrows = c_j_rows[j];
-      // per row of this outer triple: minimum (outer position, middle position) over the survivors;
-      // the survivors' merged sets r1 / r0 do not depend on the row, so the rows are the inner loop
-      uint32_t *row_best = s_row_best[warp];   // (shared memory: registers are short here)
-      __syncwarp();
-      if (lane < 4) row_best[lane] = 0xffffffffu;
-      __syncwarp();
-      for (int i0 = 0; i0 < ns; i0 += 32) {
-        const bool have = i0 + lane < ns;
-        const int fo = have ? fo_list[i0 + lane] : 0;
-        uint32_t r1 = 0, r0 = 0;
+      uint32_t mine = 0;
 #pragma unroll
-        for (int u = 0; u < 8; u++) {
-          if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
-        }
-#pragma unroll 1
-        for (int row = 0; row < nrows; row++) {
-          uint32_t hv[2][4], S, ov;
-          bool hok[2][4];
-          middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
-          const uint32_t p3s = s_p3[S];
-          uint32_t best_pm = 256;
+      for (int u = 0; u < 8; u++) {
+        if (lane == u) mine = W[u];
+      }
+      if (lane == 8) {
+        mine = (uint32_t)k0;
 #pragma unroll
-          for (int c0 = 0; c0 < 4; c0++) {
-#pragma unroll
-            for (int c1 = 0; c1 < 4; c1++) {
-              const bool ok2 = hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0;
-              if (ok2) {
-                const uint32_t V = hv[0][c0] | hv[1][c1];
-                best_pm = min(best_pm, (uint32_t)s_minpos[p3s + s_p3[V]]);
-              }
-            }
-          }
-          uint32_t cand = 0xffffffffu;
-          if (have && best_pm < 256) cand = ((uint32_t)s_pos[fo] << 8) | best_pm;
-          cand = __reduce_min_sync(kFull, cand);
-          if (lane == 0 && cand < row_best[row]) row_best[row] = cand;
+        for (int row = 0; row < 4; row++) {
+          if (row < nrows) mine |= (uint32_t)c_row_b[k0 + row] << (8 + 2 * row);
         }
       }
       __syncwarp();
-      // the first row (= the smallest ordering number) with a match decides
-      const uint32_t mine = lane < nrows ? row_best[lane] : 0xffffffffu;
-      const uint32_t hit_rows = __ballot_sync(kFull, mine != 0xffffffffu);
-      if (hit_rows != 0) {
-        const int row_hit = __ffs(hit_rows) - 1;
-        key = (idx << 23) | ((uint64_t)(k0 + row_hit) << 16)
-            | (uint64_t)__shfl_sync(kFull, mine, row_hit);
-        found = true;
+      if (lane < 9) sW[9 * j + lane] = mine;
+#pragma unroll
+      for (int hi = 0; hi < 4; hi++) {
+        if ((sv[hi] >> lane) & 1u) {
+          const int at = nent + __popc(sv[hi] & lanemask_lt()) * nrows;
+          const uint32_t e = (uint32_t)j << 9 | (uint32_t)(hi * 32 + lane);
+          for (int row = 0; row < nrows; row++) ent[at + row] = (uint16_t)(e | (uint32_t)row << 7);
+        }
+        nent += __popc(sv[hi]) * nrows;
       }
+#ifdef SBG_COUNT_STAGE1
+      {
+        const int np = __popc(sv[0]) + __popc(sv[1]) + __popc(sv[2]) + __popc(sv[3]);
+        n_pairs += np;
+        n_row_passes += (unsigned long long)((2 * np + 31) / 32 * nrows);  // one lane per fo and row
+      }
+#endif
+      if (nent < 32) continue;
+      __syncwarp();
+      const int full = nent & ~31;
+      for (int p0 = 0; p0 < full; p0 += 32) {
+        best = min(best, decomp7_entries(ent, p0, nent, sW, s_pmin, s_minpos, s_p3, lane));
+#ifdef SBG_COUNT_STAGE1
+        n_passes++;
+#endif
+      }
+      if (best != 0xffffffffu) break;
+      // carry the partial pass over to the front
+      const int rest = nent - full;
+      const uint16_t e = lane < rest ? ent[full + lane] : (uint16_t)0;
+      __syncwarp();
+      if (lane < rest) ent[lane] = e;
+      nent = rest;
     }
-    if (found) {
-      if (lane == 0) atomicMin(&ctl->best, (unsigned long long)key);
+    if (nent & 31) {
+      __syncwarp();
+      best = min(best, decomp7_entries(ent, nent & ~31, nent, sW, s_pmin, s_minpos, s_p3, lane));
+#ifdef SBG_COUNT_STAGE1
+      n_passes++;
+#endif
+    }
+#ifdef SBG_COUNT_STAGE1
+    if (lane == 0) {
+      atomicAdd(&ctl->pad0[2], n_pairs);        // complementary pairs of survivors
+      atomicAdd(&ctl->pad0[3], n_passes);       // 32-lane passes of stage 2
+      atomicAdd(&ctl->pad0[4], n_row_passes);   // the same triples one lane per fo, row by row
+    }
+#endif
+    if (best != 0xffffffffu) {
+      if (lane == 0) atomicMin(&ctl->best, (unsigned long long)((idx << 23) | best));
       break;  // later tickets of this warp have larger list indices
     }
   }
@@ -2327,9 +2401,9 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
       if (idx > 0) tuple_prev = list[idx - 1];
     }
 #ifdef SBG_COUNT_STAGE1
-    printf("S1 list %u pairs %llu with_survivors %llu\n", ctl->list_count, ctl->pad0[0], ctl->pad0[1]);
-    ctl->pad0[0] = 0;
-    ctl->pad0[1] = 0;
+    printf("S1 list %u pairs %llu with_survivors %llu outer_pairs %llu passes %llu row_passes %llu\n",
+        ctl->list_count, ctl->pad0[0], ctl->pad0[1], ctl->pad0[2], ctl->pad0[3], ctl->pad0[4]);
+    for (int i = 0; i < 5; i++) ctl->pad0[i] = 0;
 #endif
     close_stage(ctl, out, 2, key, ctl->list_count, tuple, tuple_prev);
   }
