@@ -274,7 +274,8 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
        sbg_set_list7, sbg_list7_device, sbg_set_list7_device, sbg_allgather_merge7 (every handle
        given), sbg_decomp7_part, sbg_finish7 or sbg_alu_peak ends it, whatever the call returns;
      - sbg_last_error, sbg_launch_count, sbg_transfer_stats, sbg_host_seconds, sbg_last_kernel_ms,
-       sbg_set_timing, sbg_set_stream, sbg_enum_fetch and sbg_enum_pick keep it.
+       sbg_set_timing, sbg_set_stream, sbg_enum_fetch, sbg_enum_pick, sbg_enum_block_sums and
+       sbg_enum_set_global keep it.
    Without a cursor both calls return SBG_ERR_STATE.
    A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
    a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT) or a list
@@ -287,6 +288,37 @@ int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out
    any order and repeat.  A rank >= total: SBG_ERR_ARG and nothing written.  (The ranks are sorted
    on the host and located on the device; each ticket holding one is swept once.) */
 int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_match *out);
+
+/* ---- global ranks across shares --------------------------------------------------------------- */
+/* A share's tickets fall into deal blocks, in the order the parts are dealt them: blocks of 16
+   position pairs (3-LUT) or 3-gate prefixes (5-LUT), local block j being the whole's block
+   j * nparts + part; or single list entries (7-LUT), local entry t being list entry
+   t * nparts + part.  The whole's blocks are in key order, so from every share's block sums each
+   share can turn its ranks into ranks of the whole (a global cursor):
+     1. every share counts (sbg_enum* with part = its part, nparts, total != NULL);
+     2. sbg_enum_block_sums on each; the rows are gathered in part order;
+     3. sbg_enum_set_global on each with all the rows;
+     4. sbg_enum_fetch / sbg_enum_pick on each with the same ranks; the shares' outputs, summed (or
+        OR-ed) as 64-bit words, are the records one handle's whole-share cursor (part 0 of 1)
+        returns for those ranks.
+   Both calls need a counted cursor (SBG_ERR_STATE without one) and keep it, whatever they return.
+   On a global cursor fetch and pick take ranks of the whole; the first >= total checks and *n_out
+   use the whole's total, so every share returns the same n_out.  Each share writes the records of
+   the ranks it owns and an all-zero record (width == 0) at every other slot of out[0 .. n_out)
+   (fetch) or out[0 .. nranks) (pick); it sweeps only the tickets holding the ranks it owns.  The
+   calls that end a cursor end a global one. */
+/* *nblocks = the number of the share's deal blocks; out != NULL: out[j] = the matches of its local
+   block j.  out may be host or device memory (the copy is cudaMemcpyDefault). */
+int sbg_enum_block_sums(sbg_handle *h, uint64_t *out, uint64_t *nblocks);
+/* Makes the cursor global and sets *total (and the cursor's total) to the whole's total.  Part q's
+   block sums are sums[q * stride .. q * stride + counts[q] - 1]; sums may be host or device memory,
+   counts is host memory.  SBG_ERR_ARG, with the cursor left local and usable: nparts is not the
+   cursor's nparts, a counts[q] is not the number of blocks the dealing gives part q, stride is below
+   the largest counts[q], or the row of the cursor's own part is not its block sums (compared on the
+   device: catches a gather in the wrong part order).  SBG_ERR_STATE: no cursor, or it is already
+   global.  nparts == 1 is allowed and changes nothing observable. */
+int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
+    const uint64_t *counts, int nparts, uint64_t *total);
 
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense

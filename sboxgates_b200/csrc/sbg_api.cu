@@ -149,6 +149,11 @@ struct sbg_lane {
   unsigned long long *d_ptickets = nullptr; // ticket of each rank, then the distinct tickets
   unsigned int *d_pfirst = nullptr;         // each distinct ticket's first rank in d_pranks
   uint64_t pick_cap = 0;
+  // global ranks (sbg_enum_block_sums / sbg_enum_set_global; allocated on the first call)
+  unsigned long long *d_bsums = nullptr;    // the share's block sums
+  unsigned long long *d_delta = nullptr;    // what k_enum_rebase adds to each of its blocks
+  unsigned long long *d_gsums = nullptr;    // every share's block sums, one row per part
+  uint64_t bsums_cap = 0, delta_cap = 0, gsums_cap = 0;
 };
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
@@ -167,6 +172,8 @@ struct EnumCursor {
   EnumInputs in;
   uint64_t tickets = 0, total = 0;
   uint32_t list_count = 0;   // width 7
+  uint64_t blocks = 0;       // the whole's deal blocks (every part's)
+  bool global = false;       // sbg_enum_set_global ran: offsets and total are the whole's
 };
 
 struct sbg_handle {
@@ -1477,7 +1484,7 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
 // The lane's problem is prepared on the device.
 template <int WIDTH>
 int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int nparts,
-    uint64_t tickets, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
+    uint64_t blocks, uint64_t tickets, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
     uint64_t *feasible) {
   int rc;
   if ((rc = ensure_enum(h, L, std::max<uint64_t>(tickets, 1), 0)) != SBG_OK) return rc;
@@ -1525,6 +1532,8 @@ int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int npa
     c.tickets = tickets;
     c.total = ec.carry;
     c.list_count = L.list_count;
+    c.blocks = blocks;
+    c.global = false;
   }
   if (total != nullptr) *total = ec.carry;
   if (feasible != nullptr) *feasible = WIDTH == 7 ? (uint64_t)L.list_count : ec.feasible;
@@ -1579,14 +1588,51 @@ int check_cursor(sbg_handle *h) {
   return SBG_OK;
 }
 
-// Ticket of each of ranks[0..nranks-1] (already in L.d_pranks) into L.d_ptickets.
-int locate_tickets(sbg_handle *h, sbg_lane &L, uint64_t nranks) {
+// Ticket of each of ranks[0..nranks-1] (already in L.d_pranks) into L.d_ptickets.  owned: ranks
+// outside their ticket's range (global ranks other shares hold) get kEnumUnowned.
+int locate_tickets(sbg_handle *h, sbg_lane &L, uint64_t nranks, bool owned = false) {
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nranks + 255) / 256,
       (uint64_t)h->sm_count * 8));
   const cudaError_t e = launch(h, k_enum_locate, grid, 256, 0, L.stream, false,
       (const unsigned long long *)L.d_eoffset, (unsigned long long)h->cursor.tickets,
-      (const unsigned long long *)L.d_pranks, (unsigned long long)nranks, L.d_ptickets);
+      (const unsigned long long *)L.d_pranks, (unsigned long long)nranks, L.d_ptickets,
+      owned ? (const uint32_t *)L.d_ecount : (const uint32_t *)nullptr);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_locate: %s", cudaGetErrorString(e));
+  return SBG_OK;
+}
+
+// ---- global ranks across shares (sbg_enum_block_sums / sbg_enum_set_global) ---------------------
+
+// Deal blocks part q of nparts holds out of `blocks` (blocks q, q + nparts, ...).
+uint64_t deal_share(uint64_t blocks, int q, int nparts) {
+  return blocks > (uint64_t)q ? (blocks - q + nparts - 1) / nparts : 0;
+}
+
+// Tickets per deal block of the cursor's width.
+unsigned int cursor_block_size(const EnumCursor &c) { return c.width == 7 ? 1u : (unsigned)kDeal; }
+
+int grow_u64(sbg_handle *h, sbg_lane &L, unsigned long long *&p, uint64_t &cap, uint64_t need) {
+  if (cap >= need) return SBG_OK;
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  cudaFree(p);
+  p = nullptr;
+  cap = 0;
+  SBG_CUDA(h, cudaMalloc(&p, need * sizeof(unsigned long long)));
+  cap = need;
+  return SBG_OK;
+}
+
+// The cursor's block sums into L.d_bsums (and room for as many deltas in L.d_delta).
+int block_sums(sbg_handle *h, sbg_lane &L, uint64_t nblocks) {
+  int rc;
+  if ((rc = grow_u64(h, L, L.d_bsums, L.bsums_cap, nblocks)) != SBG_OK) return rc;
+  if ((rc = grow_u64(h, L, L.d_delta, L.delta_cap, nblocks)) != SBG_OK) return rc;
+  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nblocks + 255) / 256,
+      (uint64_t)h->sm_count * 8));
+  const cudaError_t e = launch(h, k_enum_block_sums, grid, 256, 0, L.stream, false,
+      (const uint32_t *)L.d_ecount, (unsigned long long)nblocks, cursor_block_size(h->cursor),
+      L.d_bsums);
+  if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_block_sums: %s", cudaGetErrorString(e));
   return SBG_OK;
 }
 
@@ -1939,6 +1985,7 @@ void sbg_destroy(sbg_handle *h) {
       cudaFree(L.d_tcount); cudaFree(L.d_toffset); cudaFree(L.d_gcount);
       cudaFree(L.d_ectl); cudaFree(L.d_ecount); cudaFree(L.d_eoffset); cudaFree(L.d_ematch);
       cudaFree(L.d_pranks); cudaFree(L.d_pslots); cudaFree(L.d_ptickets); cudaFree(L.d_pfirst);
+      cudaFree(L.d_bsums); cudaFree(L.d_delta); cudaFree(L.d_gsums);
       if (L.h_out != nullptr) cudaFreeHost(L.h_out);
       if (L.h_ctl != nullptr) cudaFreeHost(L.h_ctl);
       for (int k = 0; k < 8; k++) if (L.ev[k] != nullptr) cudaEventDestroy(L.ev[k]);
@@ -2465,7 +2512,7 @@ int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, ui
   EnumInputs in5;
   memcpy(in5.ord.order[0], func_order, 256);
   memset(in5.ord.order[1], 0, 256);
-  return run_enum<5>(h, L, in5, part, nparts, mine * kDeal, max_matches, out, n_out, total,
+  return run_enum<5>(h, L, in5, part, nparts, blocks, mine * kDeal, max_matches, out, n_out, total,
       feasible);
 }
 
@@ -2499,7 +2546,7 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
   EnumInputs in7;
   memcpy(in7.ord.order[0], outer_order, 256);
   memcpy(in7.ord.order[1], middle_order, 256);
-  return run_enum<7>(h, L, in7, part, nparts, mine, max_matches, out, n_out, total, feasible);
+  return run_enum<7>(h, L, in7, part, nparts, count, mine, max_matches, out, n_out, total, feasible);
 }
 
 int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
@@ -2532,7 +2579,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
   EnumInputs in3;
   memset(&in3, 0, sizeof(in3));
   memcpy(in3.gates.order, gate_order, sizeof(uint16_t) * (size_t)n);
-  return run_enum<3>(h, L, in3, part, nparts, mine * kDeal, max_matches, out, n_out, total,
+  return run_enum<3>(h, L, in3, part, nparts, blocks, mine * kDeal, max_matches, out, n_out, total,
       feasible);
 }
 
@@ -2553,7 +2600,10 @@ int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out
   sbg_lane &L = h->lane[0];
   if ((rc = ensure_pick(h, L, 2)) != SBG_OK) return rc;
   if ((rc = ensure_enum(h, L, 0, n)) != SBG_OK) return rc;
+  // global ranks: the share writes the ranks it owns, zero records elsewhere
+  if (c.global) SBG_CUDA(h, cudaMemsetAsync(L.d_ematch, 0, n * sizeof(sbg_match), L.stream));
   // the tickets of the window's first and last rank; the launch covers them and those between
+  // (global: the range emit skips the tickets whose ranks lie outside the window)
   const unsigned long long ends[2] = {first, first + n - 1};
   unsigned long long tk[2] = {0, 0};
   SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, ends, sizeof(ends), cudaMemcpyHostToDevice, L.stream));
@@ -2563,7 +2613,9 @@ int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out
   EnumSel sel;
   memset(&sel, 0, sizeof(sel));
   sel.lo = first;
-  if ((rc = emit_sel<kEnumRange>(h, L, first + n, tk[0], tk[1] + 1, sel)) != SBG_OK) return rc;
+  if (c.tickets > 0 && (rc = emit_sel<kEnumRange>(h, L, first + n, tk[0], tk[1] + 1, sel)) != SBG_OK) {
+    return rc;
+  }
   SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, n * sizeof(sbg_match), cudaMemcpyDeviceToHost,
       L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
@@ -2603,28 +2655,47 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
   sbg_lane &L = h->lane[0];
   if ((rc = ensure_pick(h, L, nranks)) != SBG_OK) return rc;
   if ((rc = ensure_enum(h, L, 0, nranks)) != SBG_OK) return rc;
-  // device: the ticket of every rank; host: the distinct tickets and their slices of the ranks
+  // global ranks: the share writes the ranks it owns, zero records elsewhere
+  if (c.global) SBG_CUDA(h, cudaMemsetAsync(L.d_ematch, 0, nranks * sizeof(sbg_match), L.stream));
+  if (c.tickets == 0) {   // a share without tickets (global ranks only) owns no rank
+    SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, nranks * sizeof(sbg_match), cudaMemcpyDeviceToHost,
+        L.stream));
+    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+    h->d2h_bytes += nranks * sizeof(sbg_match);
+    return SBG_OK;
+  }
+  // device: the ticket of every rank; host: the distinct tickets and their slices of the ranks.
+  // Global ranks another share owns are dropped here, so that no warp sweeps a ticket for a rank
+  // it never meets.
   SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, sorted.data(), nranks * sizeof(unsigned long long),
       cudaMemcpyHostToDevice, L.stream));
-  if ((rc = locate_tickets(h, L, nranks)) != SBG_OK) return rc;
+  if ((rc = locate_tickets(h, L, nranks, c.global)) != SBG_OK) return rc;
   std::vector<unsigned long long> tickets(nranks);
   SBG_CUDA(h, cudaMemcpyAsync(tickets.data(), L.d_ptickets, nranks * sizeof(unsigned long long),
       cudaMemcpyDeviceToHost, L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   std::vector<unsigned int> firsts;
-  uint64_t d = 0;
+  uint64_t d = 0, m = 0;   // distinct tickets, owned ranks
   for (uint64_t i = 0; i < nranks; i++) {
-    if (i == 0 || tickets[i] != tickets[d - 1]) {
+    if (tickets[i] == kEnumUnowned) continue;
+    if (m == 0 || tickets[i] != tickets[d - 1]) {
       tickets[d++] = tickets[i];
-      firsts.push_back((unsigned int)i);
+      firsts.push_back((unsigned int)m);
     }
+    sorted[m] = sorted[i];
+    slots[m] = slots[i];
+    m++;
   }
-  firsts.push_back((unsigned int)nranks);
+  firsts.push_back((unsigned int)m);
+  if (m < nranks) {
+    SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, sorted.data(), m * sizeof(unsigned long long),
+        cudaMemcpyHostToDevice, L.stream));
+  }
   SBG_CUDA(h, cudaMemcpyAsync(L.d_ptickets, tickets.data(), d * sizeof(unsigned long long),
       cudaMemcpyHostToDevice, L.stream));
   SBG_CUDA(h, cudaMemcpyAsync(L.d_pfirst, firsts.data(), (d + 1) * sizeof(unsigned int),
       cudaMemcpyHostToDevice, L.stream));
-  SBG_CUDA(h, cudaMemcpyAsync(L.d_pslots, slots.data(), nranks * sizeof(unsigned int),
+  SBG_CUDA(h, cudaMemcpyAsync(L.d_pslots, slots.data(), m * sizeof(unsigned int),
       cudaMemcpyHostToDevice, L.stream));
   EnumSel sel;
   sel.lo = 0;
@@ -2632,11 +2703,97 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
   sel.slots = L.d_pslots;
   sel.tickets = L.d_ptickets;
   sel.first = L.d_pfirst;
-  if ((rc = emit_sel<kEnumPick>(h, L, 0, 0, d, sel)) != SBG_OK) return rc;
+  if (d > 0 && (rc = emit_sel<kEnumPick>(h, L, 0, 0, d, sel)) != SBG_OK) return rc;
   SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, nranks * sizeof(sbg_match), cudaMemcpyDeviceToHost,
       L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   h->d2h_bytes += nranks * sizeof(sbg_match);
+  return SBG_OK;
+}
+
+int sbg_enum_block_sums(sbg_handle *h, uint64_t *out, uint64_t *nblocks) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  if (nblocks == nullptr) return fail(h, SBG_ERR_ARG, "null nblocks");
+  int rc;
+  if ((rc = check_cursor(h)) != SBG_OK) return rc;
+  const EnumCursor &c = h->cursor;
+  const uint64_t nb = c.tickets / cursor_block_size(c);
+  *nblocks = nb;
+  if (out == nullptr || nb == 0) return SBG_OK;
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  if ((rc = block_sums(h, L, nb)) != SBG_OK) return rc;
+  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_bsums, nb * sizeof(uint64_t), cudaMemcpyDefault, L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  return SBG_OK;
+}
+
+int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
+    const uint64_t *counts, int nparts, uint64_t *total) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  int rc;
+  if ((rc = check_cursor(h)) != SBG_OK) return rc;
+  EnumCursor &c = h->cursor;
+  if (c.global) return fail(h, SBG_ERR_STATE, "the enumeration cursor is already global");
+  if (total == nullptr || counts == nullptr) return fail(h, SBG_ERR_ARG, "null counts or total");
+  if (nparts != c.nparts) {
+    return fail(h, SBG_ERR_ARG, "nparts %d, but the cursor's share is part %d of %d", nparts,
+        c.part, c.nparts);
+  }
+  uint64_t widest = 0;
+  for (int q = 0; q < nparts; q++) {
+    const uint64_t want = deal_share(c.blocks, q, nparts);
+    if (counts[q] != want) {
+      return fail(h, SBG_ERR_ARG, "counts[%d] = %llu, but part %d of %d holds %llu deal blocks", q,
+          (unsigned long long)counts[q], q, nparts, (unsigned long long)want);
+    }
+    widest = std::max(widest, want);
+  }
+  if (stride < widest) {
+    return fail(h, SBG_ERR_ARG, "stride %llu below the widest row (%llu blocks)",
+        (unsigned long long)stride, (unsigned long long)widest);
+  }
+  if (sums == nullptr && widest > 0) return fail(h, SBG_ERR_ARG, "null sums");
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  const unsigned int B = cursor_block_size(c);
+  const uint64_t nb = c.tickets / B;
+  uint64_t whole = 0;
+  if (c.blocks > 0) {
+    // the rows, packed at stride `widest` on the device
+    if ((rc = grow_u64(h, L, L.d_gsums, L.gsums_cap, (uint64_t)nparts * widest)) != SBG_OK) return rc;
+    for (int q = 0; q < nparts; q++) {
+      if (counts[q] == 0) continue;
+      SBG_CUDA(h, cudaMemcpyAsync(L.d_gsums + (uint64_t)q * widest, sums + (uint64_t)q * stride,
+          counts[q] * sizeof(uint64_t), cudaMemcpyDefault, L.stream));
+    }
+    if (nb > 0 && (rc = block_sums(h, L, nb)) != SBG_OK) return rc;
+    cudaError_t e = launch(h, k_enum_globalize, 1, 1024, 0, L.stream, false, L.d_ectl,
+        (const unsigned long long *)L.d_gsums, (unsigned long long)widest,
+        (unsigned long long)c.blocks, c.part, nparts, (const unsigned long long *)L.d_bsums,
+        (const unsigned long long *)L.d_eoffset, B, L.d_delta);
+    if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_globalize: %s", cudaGetErrorString(e));
+    EnumCtl ec;
+    SBG_CUDA(h, cudaMemcpyAsync(&ec, L.d_ectl, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
+    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+    if (ec.gbad != 0) {
+      return fail(h, SBG_ERR_ARG, "row %d of sums is not this share's block sums (rows gathered "
+          "out of part order?)", c.part);
+    }
+    // only now, with the check passed: the local offsets become global
+    if (nb > 0) {
+      const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((c.tickets + 255) / 256,
+          (uint64_t)h->sm_count * 8));
+      e = launch(h, k_enum_rebase, grid, 256, 0, L.stream, false, L.d_eoffset,
+          (unsigned long long)c.tickets, B, (const unsigned long long *)L.d_delta);
+      if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_rebase: %s", cudaGetErrorString(e));
+      SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+    }
+    whole = ec.gtotal;
+  }
+  c.global = true;
+  c.total = whole;
+  *total = whole;
   return SBG_OK;
 }
 

@@ -2475,6 +2475,8 @@ struct EnumCtl {
   unsigned long long feasible;  // 5-LUT: feasible tuples met
   unsigned long long carry;     // k_enum_scan: matches in front of the next window
   EnumSel sel;                  // range / pick emit: what to emit (set by the host before the pass)
+  unsigned long long gtotal;    // k_enum_globalize: the whole's total
+  unsigned int gbad;            //   1 if the share's own row of block sums differs from its own
 };
 
 struct EnumOrders {
@@ -3006,21 +3008,107 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
 }
 
 
+// k_enum_locate's mark for a rank no ticket of the share holds (global ranks only).
+constexpr unsigned long long kEnumUnowned = ~0ull;
+
 // The ticket of each requested rank (ranks[i] < the count pass's total): the last t < tickets with
 // offsets[t] <= ranks[i], by binary search over the count pass's offsets.  A ticket without matches
 // has its successor's offset, so it is never the answer.
+// Global offsets (k_enum_rebase) hold the share's ranks only, so the answer's range
+// [offsets[t], offsets[t] + counts[t]) may miss the rank, and offsets[0] may exceed it (the search
+// then ends at lo = 0); given counts, such a rank gets kEnumUnowned instead.  A global fetch passes
+// no counts: its launch runs from the first rank's ticket (0 if the rank lies below offsets[0]) to
+// the last rank's, and the range emit skips every ticket whose matches lie outside the window.
 __global__ void __launch_bounds__(256) k_enum_locate(const unsigned long long *__restrict__ offsets,
     unsigned long long tickets, const unsigned long long *__restrict__ ranks,
-    unsigned long long nranks, unsigned long long *__restrict__ ticket_of) {
+    unsigned long long nranks, unsigned long long *__restrict__ ticket_of,
+    const uint32_t *__restrict__ counts) {
   for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nranks;
        i += (unsigned long long)gridDim.x * blockDim.x) {
     const unsigned long long r = ranks[i];
-    unsigned long long lo = 0, hi = tickets;   // offsets[lo] <= r (offsets[0] = 0), offsets[hi] > r
+    // offsets[lo] <= r (local offsets: offsets[0] = 0; global ones: unless lo = 0), offsets[hi] > r
+    unsigned long long lo = 0, hi = tickets;
     while (hi - lo > 1) {
       const unsigned long long mid = lo + (hi - lo) / 2;
       if (offsets[mid] <= r) lo = mid; else hi = mid;
     }
-    ticket_of[i] = lo;
+    const bool owned = counts == nullptr || (r >= offsets[lo] && r - offsets[lo] < counts[lo]);
+    ticket_of[i] = owned ? lo : kEnumUnowned;
+  }
+}
+
+// ---- global ranks across shares (sbg_enum_block_sums / sbg_enum_set_global) ----------------------
+// A share's tickets fall into deal blocks of B tickets: B = kDeal for widths 3 and 5 (local block j
+// is the whole's block j * nparts + part, the `dealt` numbering of the kernels above), B = 1 for
+// width 7 (local ticket t is list entry t * nparts + part).  The whole's blocks are in key order, so
+// a ticket's global offset is the whole's exclusive prefix of block sums at its block plus its
+// offset within the block.
+
+// The match count of each of the share's deal blocks: out[j] = counts[j*B .. j*B + B-1] summed (a
+// widening copy for B = 1).  tickets is a multiple of B.
+__global__ void __launch_bounds__(256) k_enum_block_sums(const uint32_t *__restrict__ counts,
+    unsigned long long nblocks, unsigned int B, unsigned long long *__restrict__ out) {
+  for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < nblocks;
+       j += (unsigned long long)gridDim.x * blockDim.x) {
+    unsigned long long s = 0;
+    for (unsigned int i = 0; i < B; i++) s += counts[j * B + i];
+    out[j] = s;
+  }
+}
+
+// Exclusive prefix sum over the whole's deal blocks g = 0 .. nblocks-1, block g being part
+// q = g % nparts's local block g / nparts with sums[q * stride + g / nparts] matches.  For this
+// share's blocks (q == part): delta[j] = (global start of block j) - offsets[j * B], the amount
+// k_enum_rebase adds to the block's local offsets; ectl->gbad = 1 if the share's row of sums differs
+// from its own block sums `own` (a gather in the wrong part order), ectl->gtotal = the whole's total.
+// One CTA of 1,024 threads, a tile of 1,024 blocks at a time, as k_enum_scan.
+__global__ void __launch_bounds__(1024) k_enum_globalize(EnumCtl *__restrict__ ectl,
+    const unsigned long long *__restrict__ sums, unsigned long long stride,
+    unsigned long long nblocks, int part, int nparts, const unsigned long long *__restrict__ own,
+    const unsigned long long *__restrict__ offsets, unsigned int B,
+    unsigned long long *__restrict__ delta) {
+  __shared__ unsigned long long s_warp[32];
+  __shared__ unsigned int s_bad;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) s_bad = 0;
+  unsigned long long carry = 0;
+  for (unsigned long long g0 = 0; g0 < nblocks; g0 += blockDim.x) {
+    const unsigned long long g = g0 + threadIdx.x;
+    const unsigned long long j = g / (unsigned long long)nparts;
+    const int q = (int)(g % (unsigned long long)nparts);
+    const unsigned long long c = g < nblocks ? sums[(unsigned long long)q * stride + j] : 0ull;
+    unsigned long long incl = c;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const unsigned long long up = __shfl_up_sync(kFull, incl, d);
+      if (lane >= d) incl += up;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    unsigned long long before = 0;
+    for (int i = 0; i < warp; i++) before += s_warp[i];
+    unsigned long long tile = 0;
+    for (int i = 0; i < (int)(blockDim.x >> 5); i++) tile += s_warp[i];
+    if (g < nblocks && q == part) {
+      delta[j] = carry + before + incl - c - offsets[j * B];
+      if (c != own[j]) s_bad = 1;
+    }
+    carry += tile;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    ectl->gtotal = carry;
+    ectl->gbad = s_bad;
+  }
+}
+
+// offsets[t] += delta[t / B]: the share's local offsets become global ones.  delta is computed
+// beforehand so that no thread reads a block-start offset another thread has already rebased.
+__global__ void __launch_bounds__(256) k_enum_rebase(unsigned long long *__restrict__ offsets,
+    unsigned long long tickets, unsigned int B, const unsigned long long *__restrict__ delta) {
+  for (unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; t < tickets;
+       t += (unsigned long long)gridDim.x * blockDim.x) {
+    offsets[t] += delta[t / B];
   }
 }
 

@@ -10,6 +10,12 @@ RNG state, takes an interleaved share of the work items, and the ranks agree on 
 Because the key orders candidates exactly as the reference's single-rank loop visits them, the
 result is the reference's size == 1 result for any number of GPUs.
 
+Enumeration (enumerate3/5/7, fetch_matches, pick_matches, sample_matches) always shards when
+world > 1: every rank counts its share, one all-gather of (blocks, feasible) and one of the block
+sums make every rank's cursor global (sbg_enum_set_global), and each fetch or pick is the engine
+call plus one all-reduce(SUM) of the records, where every rank holds the ranks it owns and zero
+records elsewhere.
+
 The engine is any object with the `LutEngine` part-methods; the CPU tests drive this module over
 `gloo` with an oracle-backed stand-in engine, the product uses `LutEngine` (CUDA) over `nccl`.
 """
@@ -20,8 +26,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .lut import (SBG_KEY_NONE, SBG_LIST_CAP, result5_to_ret, result7_to_ret, shuffled_order,
-                  shuffled_orders7)
+from .lut import (MATCH_DTYPE, SBG_KEY_NONE, SBG_LIST_CAP, Enumeration, result5_to_ret,
+                  result7_to_ret, sample_matches, shuffled_order, shuffled_orders7)
 
 _I64_MAX = (1 << 63) - 1
 
@@ -130,22 +136,26 @@ class DistributedLutSearch:
         key = self._allreduce_min_key(key)
         return self.engine.finish5(key, order)
 
-    def search7_sharded(self, outer, middle):
+    def _install_list7(self):
+        """search_7lut phase 1: every rank installs the same list, built sharded (and merged) when
+        the space is large, else by each rank alone.  Returns its length."""
         n = self.engine.n
         self.last_phase1_sharded = not (self.world == 1 or math.comb(n, 7) < self.shard_min_tuples7)
         if not self.last_phase1_sharded:
             # phase 1 replicated: every rank builds (and keeps on its device) the same full list
-            count = self.engine.filter7_keep_local()
-        elif self.device.type == "cuda" and hasattr(self.engine, "filter7_part_device"):
-            count = self._allgather_merge_on_device(
+            return self.engine.filter7_keep_local()
+        if self.device.type == "cuda" and hasattr(self.engine, "filter7_part_device"):
+            return self._allgather_merge_on_device(
                 self.engine.filter7_part_device(self.rank, self.world))
-        else:
-            local = self.engine.filter7_part(self.rank, self.world)
-            merged = self._allgather_lists(local)
-            # Every rank installs the same merged list: the runs are merged and cut at
-            # SBG_LIST_CAP entries (lut.c:316-318 at size == 1).
-            self.engine.set_list7(merged)
-            count = min(len(merged), SBG_LIST_CAP)
+        local = self.engine.filter7_part(self.rank, self.world)
+        merged = self._allgather_lists(local)
+        # Every rank installs the same merged list: the runs are merged and cut at
+        # SBG_LIST_CAP entries (lut.c:316-318 at size == 1).
+        self.engine.set_list7(merged)
+        return min(len(merged), SBG_LIST_CAP)
+
+    def search7_sharded(self, outer, middle):
+        count = self._install_list7()
         if self.world == 1 or count < self.shard_min_list:
             key = self.engine.decomp7_part(0, 1, outer, middle)
         else:
@@ -162,3 +172,99 @@ class DistributedLutSearch:
         outer, middle = shuffled_orders7(rng)
         self.engine.load(tables, target, mask, inbits)
         return result7_to_ret(self.search7_sharded(outer, middle), rng)
+
+    # -- enumeration: ranks of the whole across the ranks' shares ------------------------------
+    def _globalize(self, feasible):
+        """All-gathers every rank's (deal blocks, feasible) and block sums, and makes the engine's
+        cursor global.  Returns (the whole's total, feasible summed over the ranks)."""
+        t0 = time.perf_counter()
+        nb = self.engine.enum_block_count()
+        mine = torch.tensor([nb, feasible], dtype=torch.int64, device=self.device)
+        meta = torch.empty(2 * self.world, dtype=torch.int64, device=self.device)
+        dist.all_gather_into_tensor(meta, mine, group=self.group)
+        meta = meta.view(self.world, 2).tolist()
+        self.collectives += 1
+        counts = [int(m[0]) for m in meta]
+        width = max(max(counts), 1)
+        if self.device.type == "cuda":
+            # the sums go from the engine's device straight into the gathered device buffer;
+            # set_global reads only the first counts[q] entries of each row.  enum_block_sums waits
+            # for torch's stream before the engine writes the row on its own.
+            row = torch.empty(width, dtype=torch.int64, device=self.device)
+            self.engine.enum_block_sums(out=row)
+            sums = torch.empty(self.world * width, dtype=torch.int64, device=self.device)
+            dist.all_gather_into_tensor(sums, row, group=self.group)
+            # set_global reads them on the engine's stream, the collective ran on torch's
+            torch.cuda.current_stream().synchronize()
+            sums = sums.view(self.world, width)
+        else:
+            row = torch.zeros(width, dtype=torch.int64)
+            row[:nb] = torch.from_numpy(self.engine.enum_block_sums().view(np.int64))
+            parts = [torch.empty_like(row) for _ in range(self.world)]
+            dist.all_gather(parts, row, group=self.group)
+            sums = torch.stack(parts).numpy()
+        self.collectives += 1
+        total = self.engine.enum_set_global(sums, counts)
+        self.collective_ms += 1e3 * (time.perf_counter() - t0)
+        return total, sum(int(m[1]) for m in meta)
+
+    def _sum_records(self, recs):
+        """One all-reduce(SUM) of every rank's records (the ranks it owns, zero records elsewhere)."""
+        t0 = time.perf_counter()
+        t = torch.from_numpy(recs.view(np.int64).copy()).to(self.device)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        self.collectives += 1
+        out = t.cpu().numpy().view(MATCH_DTYPE).copy()
+        self.collective_ms += 1e3 * (time.perf_counter() - t0)
+        assert not np.any(out["width"] == 0), "a rank of the whole is owned by no share"
+        return out
+
+    def _enumerate(self, run, max_matches, list_length=None):
+        if self.world == 1:
+            return run(int(max_matches), 0, 1)
+        local = run(0, self.rank, self.world)
+        total, feasible = self._globalize(local.feasible)
+        first = self.fetch_matches(0, max_matches)
+        return Enumeration(total, feasible if list_length is None else list_length, first)
+
+    def enumerate3(self, gate_order, max_matches):
+        """Every match of lut_search's 3-LUT scan of the current problem over `gate_order`: the
+        whole's total and feasible count and its first max_matches records, with this engine's
+        cursor made global for fetch_matches / pick_matches / sample_matches."""
+        return self._enumerate(
+            lambda k, part, nparts: self.engine.enumerate3(gate_order, k, True, part, nparts),
+            max_matches)
+
+    def enumerate5(self, order, max_matches):
+        """The same for search_5lut with a given function order."""
+        return self._enumerate(
+            lambda k, part, nparts: self.engine.enumerate5(order, k, True, part, nparts),
+            max_matches)
+
+    def enumerate7(self, outer, middle, max_matches):
+        """The same for search_7lut; the list is installed as search7_sharded installs it, and
+        `feasible` is its length."""
+        count = self._install_list7()
+        return self._enumerate(
+            lambda k, part, nparts: self.engine.enumerate7(outer, middle, k, True, part, nparts),
+            max_matches, list_length=count)
+
+    def fetch_matches(self, first, count):
+        """The whole's matches at ranks first .. min(first + count, total) - 1 (the last
+        enumerate* call's), the same on every rank."""
+        recs = self.engine.fetch_matches(first, count)
+        if self.world == 1 or recs.shape[0] == 0:
+            return recs
+        return self._sum_records(recs)
+
+    def pick_matches(self, ranks):
+        """The whole's matches at the given ranks, in their order, the same on every rank."""
+        recs = self.engine.pick_matches(ranks)
+        if self.world == 1 or recs.shape[0] == 0:
+            return recs
+        return self._sum_records(recs)
+
+    def sample_matches(self, enumeration, k, seed=None):
+        """k distinct matches drawn uniformly from the whole (lut.sample_matches); every rank draws
+        the same ranks from the same seed."""
+        return sample_matches(self, enumeration, k, seed)

@@ -392,7 +392,12 @@ class LutEngine:
         enumeration on this engine (ranks within its share, ascending key order), as a MATCH_DTYPE
         array: the same records that enumeration emits at those ranks.  Nothing is counted again.
         Raises RuntimeError if something other than a fetch, a pick or a query ran on the engine
-        since that enumeration (the cursor is gone)."""
+        since that enumeration (the cursor is gone).
+
+        On a global cursor (enum_set_global) the ranks are ranks of the whole and the length is
+        the same on every share: this share's records at the ranks it owns, all-zero records
+        (width 0) at every other rank.  Summing the shares' outputs as 64-bit words gives the
+        whole's records."""
         first, count = int(first), int(count)
         if not 0 <= first < 2**64:
             raise ValueError("first must lie in 0..2**64-1")
@@ -406,7 +411,11 @@ class LutEngine:
 
     def pick_matches(self, ranks):
         """The matches at the given ranks of the last counted enumeration, in the order of `ranks`
-        (a 1-D integer array; any order, repeats allowed, each below the total)."""
+        (a 1-D integer array; any order, repeats allowed, each below the total).
+
+        On a global cursor (enum_set_global) the ranks are ranks of the whole, below the whole's
+        total: this share's records at the ranks it owns, all-zero records (width 0) at every other
+        slot.  Summing the shares' outputs as 64-bit words gives the whole's records."""
         r = np.asarray(ranks)
         if r.ndim != 1 or (r.size > 0 and r.dtype.kind not in "iu"):
             raise ValueError("ranks must be a 1-D integer array")
@@ -420,13 +429,77 @@ class LutEngine:
                                            out.ctypes.data_as(C.c_void_p)))
         return out[:r.shape[0]].copy()
 
+    # -- global ranks across shares (the cursor of a sharded count) -----------------------------
+    def enum_block_count(self):
+        """The number of deal blocks of the cursor's share (the length enum_block_sums fills)."""
+        nb = C.c_uint64()
+        self._check(self.lib.sbg_enum_block_sums(self._h, None, C.byref(nb)))
+        return int(nb.value)
+
+    def enum_block_sums(self, out=None):
+        """The match count of each deal block of the cursor's share, in local block order.  out=None:
+        returns a numpy uint64 array; else out (a contiguous 64-bit torch tensor, CPU or CUDA, with
+        at least that many elements) is filled through its data pointer and returned."""
+        nb = C.c_uint64()
+        n = self.enum_block_count()
+        if out is None:
+            arr = np.zeros(max(n, 1), dtype=np.uint64)
+            if n > 0:
+                self._check(self.lib.sbg_enum_block_sums(self._h, arr.ctypes.data_as(C.c_void_p),
+                                                         C.byref(nb)))
+            return arr[:n]
+        if out.element_size() != 8 or not out.is_contiguous() or out.numel() < n:
+            raise ValueError("out must be a contiguous 64-bit tensor of at least %d elements" % n)
+        if n > 0:
+            _torch_stream_done(out)
+            self._check(self.lib.sbg_enum_block_sums(self._h, C.c_void_p(out.data_ptr()),
+                                                     C.byref(nb)))
+        return out
+
+    def enum_set_global(self, sums, counts):
+        """Makes the cursor global: `sums` is (nparts, stride) -- row q holds part q's block sums
+        in its first counts[q] entries -- as a numpy array or a torch tensor (CPU or CUDA) of
+        64-bit integers.  Returns the whole's total; fetch_matches and pick_matches then take
+        ranks of the whole."""
+        counts = np.ascontiguousarray([int(c) for c in counts], dtype=np.uint64)
+        if isinstance(sums, np.ndarray):
+            sums = np.ascontiguousarray(sums)
+            if sums.ndim != 2 or sums.dtype.itemsize != 8 or sums.dtype.kind not in "iu":
+                raise ValueError("sums must be a 2-D array of 64-bit integers")
+            ptr, stride = sums.ctypes.data, sums.shape[1]
+        else:
+            if sums.dim() != 2 or sums.element_size() != 8 or not sums.is_contiguous():
+                raise ValueError("sums must be a contiguous 2-D tensor of 64-bit integers")
+            ptr, stride = sums.data_ptr(), sums.shape[1]
+            _torch_stream_done(sums)
+        if sums.shape[0] != counts.shape[0]:
+            raise ValueError("sums has %d rows for %d parts" % (sums.shape[0], counts.shape[0]))
+        total = C.c_uint64()
+        self._check(self.lib.sbg_enum_set_global(self._h, C.c_void_p(ptr), int(stride),
+                                                 counts.ctypes.data_as(native.u64p),
+                                                 int(counts.shape[0]), C.byref(total)))
+        return int(total.value)
+
+
+def _torch_stream_done(t):
+    """Waits for the work torch has queued on a CUDA tensor's device.  The engine reads or writes
+    the tensor on its own stream, which is not ordered after torch's (a zero fill, a collective);
+    the engine's calls wait for their own stream before returning."""
+    if t.is_cuda:
+        import torch
+        torch.cuda.current_stream(t.device).synchronize()
+
 
 def sample_matches(engine, enumeration, k, seed=None):
     """k distinct matches drawn uniformly from the whole match set of `enumeration`, which must be
     the last counted enumeration on `engine` (its cursor): returns (ranks, matches) with the ranks
     ascending and matches[i] the match at ranks[i].  The ranks come from
     numpy.random.default_rng(seed).choice(total, k, replace=False); the reference has no sampling,
-    so no xorshift1024 stream is involved and the caller's RNG stays untouched."""
+    so no xorshift1024 stream is involved and the caller's RNG stays untouched.
+
+    On a global cursor pass the whole's total (enumeration.total): every share draws the same
+    ranks from the same seed, and its matches are zero records at the ranks other shares own;
+    summed over the shares they are the whole's sample."""
     if enumeration.total is None:
         raise ValueError("the enumeration was not counted (count=False): it has no cursor")
     k, total = int(k), int(enumeration.total)

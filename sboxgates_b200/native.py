@@ -106,6 +106,8 @@ SIGNATURES = {
                             C.c_void_p, u64p, u64p, u64p]),
     "sbg_enum_fetch": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, u64p]),
     "sbg_enum_pick": (C.c_int, [C.c_void_p, u64p, C.c_uint64, C.c_void_p]),
+    "sbg_enum_block_sums": (C.c_int, [C.c_void_p, C.c_void_p, u64p]),
+    "sbg_enum_set_global": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, u64p, C.c_int, u64p]),
 }
 
 _lib = None
