@@ -228,6 +228,8 @@ struct sbg_handle {
   int opt_group_chunks = 6; // SBG_GROUP_CHUNKS: chunks of 32 pairs per weighted phase-1 ticket (0 = whole prefixes)
   int opt_group_chunks_conc = 0;  // SBG_GROUP_CHUNKS_CONC: the same while several chains share the device
   int opt_packed = 1;       // SBG_PACKED: phase 1 keeps two parts per register where <= 15 last gates remain
+  int opt_sieve = 1;        // SBG_SIEVE: phase 1 (shifted windows) rules out last gates with the pair sieve
+                            // first: 0 never, 1 above kSieveMinPositions masked positions, 2 always
   int opt_decomp_filter = 1;  // SBG_DECOMP_FILTER: lane-parallel stage-1 filter of phase 2 (0 = ballot form only)
   int opt_batch_conc = 2;   // SBG_BATCH_CONC: phase-1 prefixes per ticket while several chains share
                             // the device (sbg_search_batch)
@@ -351,6 +353,11 @@ constexpr int kSinglePrefixMaxGates = 72;
 // aligned two-word windows under a full mask, by less as n grows (scripts/sweep_shift.sh compares
 // the two).
 constexpr int kShiftMaxGates = 60;
+// Phase 1's pair sieve (shifted windows) above this many masked positions (SBG_SIEVE=0|1|2
+// overrides).  On one H100 at n = 40 it took the launches under 256 / 128 / 64 positions from
+// 0.393 / 0.277 / 0.231 ms to 0.264 / 0.231 / 0.212 ms; under 32 positions the cell loop visits
+// about 10 positions per chunk, no more than the sieve's per-prefix set-up saves (0.220 -> 0.223 ms).
+constexpr int kSieveMinPositions = 32;
 uint64_t pick_batch(const sbg_handle *h, uint64_t tickets, int n, int P) {
   const uint64_t warps = kNominalWarps;
   if (h->opt_batch > 0) {
@@ -632,11 +639,12 @@ int enqueue_search5(sbg_handle *h, sbg_lane &L, int part, int nparts, bool two) 
 }
 
 template <int NW, int P>
-size_t filter_pm_smem(int n, int m, bool shifted = false) {
+size_t filter_pm_smem(int n, int m, bool shifted = false, bool sieve = false) {
   const int npad = (n + 3) & ~3;
   const int ngw = (((n + 31) >> 5) + 1) & ~1;
   return sizeof(uint32_t) * (size_t)(NW * npad + ((m * ngw + 3) & ~3)
-      + kWarpsPerCta * ((1 << P) * NW + ngw * 32) + (shifted ? std::max(n - 6, 1) * m : 0));
+      + kWarpsPerCta * ((1 << P) * NW + ngw * 32 + (sieve ? kSieveWords : 0))
+      + (shifted ? std::max(n - 6, 1) * m : 0));
 }
 
 // Position-major phase 1 (k_filter7_pm): work items are 4- or 5-gate prefixes.  The 5-gate form does
@@ -758,14 +766,14 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
   const ChunkPlan &pl = fp.pl;
   cudaError_t e = cudaSuccess;
   int rc = SBG_OK;
-#define SBG_LAUNCH_PM(NWV, WV, FSV, SHV)                                                       \
+#define SBG_LAUNCH_PM_S(NWV, WV, FSV, SHV, SVV)                                                \
   {                                                                                            \
-    const size_t smem = filter_pm_smem<NWV, P>(n, m, SHV);                                     \
-    if ((rc = ensure_smem(h, k_filter7_pm<NWV, WV, P, FSV, SHV>, smem)) != SBG_OK) return rc;  \
-    int grid = grid_for(h, k_filter7_pm<NWV, WV, P, FSV, SHV>, smem,                           \
+    const size_t smem = filter_pm_smem<NWV, P>(n, m, SHV, SVV);                                \
+    if ((rc = ensure_smem(h, k_filter7_pm<NWV, WV, P, FSV, SHV, SVV>, smem)) != SBG_OK) return rc; \
+    int grid = grid_for(h, k_filter7_pm<NWV, WV, P, FSV, SHV, SVV>, smem,                      \
         fp.tickets + fp.chunk_tickets);                                                        \
     if (fp.max_warps > 0) grid = std::min(grid, (fp.max_warps + kWarpsPerCta - 1) / kWarpsPerCta); \
-    e = launch(h, k_filter7_pm<NWV, WV, P, FSV, SHV>, grid, kThreads, smem, L.stream,          \
+    e = launch(h, k_filter7_pm<NWV, WV, P, FSV, SHV, SVV>, grid, kThreads, smem, L.stream,     \
         !h->timing, h->d_slots + L.slot, L.d_ctl, L.d_hits, L.d_aux, L.d_tcount, L.d_gcount,   \
         (unsigned long long)L.hits_cap, (unsigned long long)fp.tickets_cap, part, nparts,      \
         list_cap, (int)fp.batch, fp.max_warps,                                                 \
@@ -773,10 +781,21 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
         (unsigned long long)fp.chunk_tickets, (unsigned long long)fp.seg_base,                 \
         h->opt_packed ? 15 : 0, fp.wt);                                                        \
   }
+#define SBG_LAUNCH_PM(NWV, WV, FSV, SHV) SBG_LAUNCH_PM_S(NWV, WV, FSV, SHV, false)
   const bool shifted = P == 4 && (h->opt_shift >= 0 ? h->opt_shift != 0 && n <= 63
                                                      : n <= kShiftMaxGates);
   if constexpr (P == 4) {
-    if (shifted) {         // one word of 31 candidate gates from the first possible g on
+    // the pair sieve where it pays: it costs a fixed set-up per prefix, and under the smallest masks
+    // the cell loop it replaces visits too few positions per chunk (SBG_SIEVE=2: always)
+    const bool sieve = h->opt_sieve == 2 || (h->opt_sieve == 1 && m > kSieveMinPositions);
+    if (shifted && sieve) {
+      switch (hp.nw) {
+        case 1: SBG_LAUNCH_PM_S(1, 1, true, true, true) break;
+        case 2: SBG_LAUNCH_PM_S(2, 1, true, true, true) break;
+        case 4: SBG_LAUNCH_PM_S(4, 1, true, true, true) break;
+        default: SBG_LAUNCH_PM_S(8, 1, true, true, true) break;
+      }
+    } else if (shifted) {  // one word of 31 candidate gates from the first possible g on
       switch (hp.nw) {
         case 1: SBG_LAUNCH_PM(1, 1, true, true) break;
         case 2: SBG_LAUNCH_PM(2, 1, true, true) break;
@@ -809,6 +828,7 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
     }
   }
 #undef SBG_LAUNCH_PM
+#undef SBG_LAUNCH_PM_S
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_filter7_pm: %s", cudaGetErrorString(e));
   return SBG_OK;
 }
@@ -1807,6 +1827,7 @@ int sbg_create(sbg_handle **out, int device) {
   }
   if (getenv("SBG_PACKED") != nullptr) h->opt_packed = atoi(getenv("SBG_PACKED")) != 0;
   if (getenv("SBG_SHIFT") != nullptr) h->opt_shift = atoi(getenv("SBG_SHIFT")) != 0;
+  if (getenv("SBG_SIEVE") != nullptr) h->opt_sieve = std::max(0, std::min(2, atoi(getenv("SBG_SIEVE"))));
   if (getenv("SBG_HEAD_WAVES") != nullptr) h->opt_head_waves = atoi(getenv("SBG_HEAD_WAVES"));
   if (getenv("SBG_PDL") != nullptr) h->opt_pdl = atoi(getenv("SBG_PDL")) != 0;
   if (getenv("SBG_DECOMP_FILTER") != nullptr) {   // 0 off, 1 by list length, 2..32 forced block size

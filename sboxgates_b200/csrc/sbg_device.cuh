@@ -847,7 +847,20 @@ __device__ __forceinline__ void unrank_weighted_warp(uint32_t t, int np,
 #define SBG_FILTER_MIN_CTAS (SH ? 3 : 2)
 #endif
 constexpr int kQuadGates = 7;   // QUAD windows: 7 candidate gates + the target bit per byte
-template <int NW, int W, int P, bool FS, bool SH = false>
+// SIEVE (SH only): a 7-tuple is feasible iff every masked (target 1, target 0) pair of positions is
+// told apart by one of its gates.  Within a mixed cell of the prefix a, b, c and d agree on every
+// such pair, so (e,f,g) must separate all of the cell's pairs; the gates that separate pair
+// (p,q) are S = ~(xr[p] ^ xr[q]) over the gate bits.  Per prefix the warp takes up to 64 such pairs
+// (each position of a mixed cell with the first position of the other target in its cell) and
+// keeps, per warp, S[u] for each pair u and
+// sep[x] = the pairs gate x separates.  A lane with pair (e,f) then only has to intersect its
+// candidate g with S[u] for the pairs u neither e nor f separates -- a necessary condition, usually
+// empty after a few pairs.  Lanes and chunks that keep candidates go through the exact cell loop,
+// seeded with what the sieve left.
+constexpr int kSievePairs = 64;
+constexpr int kSieveWords = 4 * kSievePairs;   // per warp: S[64] and sep[64], 64-bit words
+// SV: the sieve is compiled in (SH only); without it the shifted form is the plain cell loop.
+template <int NW, int W, int P, bool FS, bool SH = false, bool SV = false>
 __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(const DevProblem *__restrict__ prob,
     DevCtl *__restrict__ ctl, uint64_t *__restrict__ hits, uint64_t *__restrict__ aux,
     uint32_t *__restrict__ tcount, uint32_t *__restrict__ gcount, unsigned long long hits_cap,
@@ -889,10 +902,15 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
   uint32_t *cells = s_xr + ((m * ngw + 3) & ~3) + warp * (NC * NW);
   // per warp: the surviving-g vectors of one chunk, word-major (vs[word * 32 + lane])
   uint32_t *vs = s_xr + ((m * ngw + 3) & ~3) + kWarpsPerCta * (NC * NW) + warp * (ngw * 32);
+  // SV only: the warp's sieve tables, S[u] at s_sieve[u] and sep[x] at s_sieve[kSievePairs + x]
+  uint64_t *s_sieve = reinterpret_cast<uint64_t *>(s_xr + ((m * ngw + 3) & ~3)
+      + kWarpsPerCta * (NC * NW + ngw * 32) + warp * kSieveWords);
   // SH only: the shifted rows for EVERY window base 6 .. n-1 (a prefix's first window starts at its
   // last gate + 3 >= 6), sxt[(base - 6) * m + p]; built once per CTA, read by all its warps
-  uint32_t *sxt = s_xr + ((m * ngw + 3) & ~3) + kWarpsPerCta * (NC * NW + ngw * 32);
+  uint32_t *sxt = s_xr + ((m * ngw + 3) & ~3)
+      + kWarpsPerCta * (NC * NW + ngw * 32 + (SV ? kSieveWords : 0));
   static_assert(!SH || (W == 1 && P == 4 && FS), "shifted windows: one word, 4-gate prefixes, n <= 63");
+  static_assert(!SV || SH, "the sieve is part of the shifted-window form");
   const uint32_t sxt_top = (uint32_t)__cvta_generic_to_shared(sxt + 31);   // row 31 of base 6
   const uint32_t xr_base = (uint32_t)__cvta_generic_to_shared(s_xr);
   const uint32_t neg_row_bytes = 0u - (uint32_t)ngw * 4u;   // one multiply-add per address
@@ -1122,9 +1140,68 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
       const int mc = __popc(mixed_ballot);
 #ifdef SBG_COUNT_FILTER
       unsigned long long dbg_chunks = 0, dbg_windows = 0, dbg_cells = 0, dbg_pos = 0, dbg_packed = 0;
-      unsigned long long dbg_quad = 0;
+      unsigned long long dbg_quad = 0, dbg_sieve = 0, dbg_exact = 0;
       unsigned long long dbg_mc = (unsigned long long)mc;
 #endif
+      if constexpr (SV) {
+        {
+          // the sieve's pairs, all mixed cells at once: every masked position p of a mixed cell is
+          // paired with the first position of the other target in its cell (lane j < mc holds those
+          // of mixed cell j), except the first target-0 position, whose pair the first target-1
+          // position already has; positions in order, word by word, up to 64 pairs.  No loop over
+          // cells and no dependent shared-memory round trips per cell.
+          const uint64_t gmask = (1ull << n) - 1u;   // gate bits: no target bit, no padding
+          int rep1 = 0, rep0 = 0;
+          if (lane < mc) {
+            bool f1 = false, f0 = false;
+#pragma unroll
+            for (int w = 0; w < NW; w++) {
+              const uint32_t c = cells[lane * NW + w];
+              const uint32_t a = c & T[w], bq = c & ~T[w];
+              if (!f1 && a != 0) rep1 = w * 32 + __ffs(a) - 1;
+              if (!f0 && bq != 0) rep0 = w * 32 + __ffs(bq) - 1;
+              f1 |= a != 0;
+              f0 |= bq != 0;
+            }
+          }
+          int npairs = 0;
+#pragma unroll
+          for (int w = 0; w < NW; w++) {
+            if (npairs < kSievePairs) {   // warp-uniform
+              const int p = w * 32 + lane;
+              uint32_t cell = 0;
+#pragma unroll
+              for (int i = 0; i < P; i++) cell = (cell << 1) | ((s_tabs[w * npad + pre[i]] >> lane) & 1u);
+              const bool t1 = ((T[w] >> lane) & 1u) != 0;
+              const int slot = __popc(mixed_ballot & ((1u << cell) - 1u));
+              const int r1 = __shfl_sync(kFull, rep1, slot), r0 = __shfl_sync(kFull, rep0, slot);
+              const int q = t1 ? r0 : r1;
+              const bool paired = ((M[w] >> lane) & 1u) != 0 && ((mixed_ballot >> cell) & 1u) != 0
+                  && (t1 || p != r0);
+              const uint32_t bal = __ballot_sync(kFull, paired);
+              const int u = npairs + __popc(bal & lanemask_lt());
+              if (paired && u < kSievePairs) {
+                const uint64_t xp = *reinterpret_cast<const uint64_t *>(s_xr + p * ngw);
+                const uint64_t xq = *reinterpret_cast<const uint64_t *>(s_xr + q * ngw);
+                s_sieve[u] = ~(xp ^ xq) & gmask;
+              }
+              npairs = min(kSievePairs, npairs + __popc(bal));
+            }
+          }
+          __syncwarp();
+          // entries past npairs are stale; their bits are masked below and never read
+          const uint64_t s_lo = s_sieve[lane], s_hi = s_sieve[lane + 32];
+          // sep[x] for the gates that can be e or f; pairs past npairs count as separated, so that
+          // a prefix without mixed cells (npairs = 0) passes everything
+          const uint64_t unused = npairs >= kSievePairs ? 0ull : ~0ull << npairs;
+          for (int x = last + 1; x <= n - 2; x++) {
+            const uint32_t lo = __ballot_sync(kFull, ((s_lo >> x) & 1u) != 0);
+            const uint32_t hi = npairs > 32 ? __ballot_sync(kFull, ((s_hi >> x) & 1u) != 0) : 0u;
+            if (lane == 0) s_sieve[kSievePairs + x] = (((uint64_t)hi << 32) | lo) | unused;
+          }
+          __syncwarp();
+        }
+      }
 
       unsigned long long emitted = 0;
       bool prefix_done = false;
@@ -1163,7 +1240,41 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         // windows of 32*W candidate gates g, from the first that can hold the smallest possible g
         // (SH: windows of 31 gates starting AT the chunk's smallest candidate g, wb counts them)
         int first_g = last + (K - P);
-        if constexpr (SH) {
+        uint64_t cand = 0;   // SV: the lane's candidate g, gf < g < n, excluded gates out, sieved
+        if constexpr (SV) {
+          if (lane_ok) cand = ((1ull << n) - 1u) & (~0ull << (gf + 1)) & ~(uint64_t)(inmask & 0xffu);
+          {
+            const uint64_t sepd = s_sieve[kSievePairs + ge] | s_sieve[kSievePairs + gf];
+            // the pairs neither e nor f separates, in two halves taken a pair each per step: two
+            // independent load chains instead of one
+            uint32_t u_lo = ~(uint32_t)sepd, u_hi = ~(uint32_t)(sepd >> 32);
+#ifdef SBG_COUNT_FILTER
+            uint32_t its = 0;
+#endif
+            while ((u_lo | u_hi) != 0 && cand != 0) {
+              const uint64_t s_a = u_lo != 0 ? s_sieve[__ffs(u_lo) - 1] : ~0ull;
+              const uint64_t s_b = u_hi != 0 ? s_sieve[31 + __ffs(u_hi)] : ~0ull;
+              cand &= s_a & s_b;
+              u_lo &= u_lo - 1;
+              u_hi &= u_hi - 1;
+#ifdef SBG_COUNT_FILTER
+              its++;
+#endif
+            }
+#ifdef SBG_COUNT_FILTER
+            dbg_sieve += __reduce_max_sync(kFull, its);
+#endif
+          }
+          // a lane needs only its candidates: the chunk's windows start at the lowest of its lanes
+          // (often well above the prefix's last + 3), so that more of them take the packed forms
+          const uint32_t lo = __reduce_min_sync(kFull, cand != 0 ? (uint32_t)(__ffsll((long long)cand) - 1)
+                                                                 : (uint32_t)n);
+          if (lo >= (uint32_t)n) continue;   // no candidate left in any lane: nothing to test or emit
+          first_g = (int)lo;
+#ifdef SBG_COUNT_FILTER
+          dbg_exact++;
+#endif
+        } else if constexpr (SH) {
           // a lane needs only g > f: the chunk's windows start at the lowest gf + 1 of its live lanes
           // (often well above the prefix's last + 3), so that more of them take the packed forms
           const uint32_t lo = __reduce_min_sync(kFull, lane_ok ? (uint32_t)(gf + 1) : (uint32_t)n);
@@ -1183,7 +1294,9 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
           const bool quad = packed && n - base <= kQuadGates;
           const uint32_t sx_top = sxt_top + (uint32_t)((base - 6) * m) * 4u;
           uint32_t V[W];
-          if constexpr (SH) {
+          if constexpr (SV) {
+            V[0] = (uint32_t)(cand >> base) & 0x7fffffffu;   // gates base .. base+30
+          } else if constexpr (SH) {
             uint32_t v = 0x7fffffffu;                // gates base .. base+30: keep gf < g < n
             if (n - base < 31) v = 0x7fffffffu >> (31 - (n - base));
             if (gf + 1 - base >= 31) v = 0u;
@@ -1441,6 +1554,8 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         atomicAdd(&ctl->pad1[5], dbg_packed);
         atomicAdd(&ctl->pad1[6], dbg_mc);
         atomicAdd(&ctl->pad1[7], dbg_quad);
+        atomicAdd(&ctl->pad1[8], dbg_sieve);
+        atomicAdd(&ctl->pad1[9], dbg_exact);
       }
 #endif
     }
@@ -1477,11 +1592,12 @@ __global__ void __launch_bounds__(256) k_offsets(DevCtl *__restrict__ ctl,
         + min(volatile_load(&ctl->hit_count), (unsigned long long)0xffffffffu);
     ctl->list_count = (unsigned int)min(total, (unsigned long long)list_cap);
 #ifdef SBG_COUNT_FILTER
-    // windows = single (31 gates) + packed (two parts of 15) + quad (four parts of 7)
-    printf("F1 prefixes %llu chunks %llu windows %llu cells %llu positions %llu packed %llu mixed %llu hits %llu quad %llu\n",
+    // windows = single (31 gates) + packed (two parts of 15) + quad (four parts of 7); sieve = the
+    // slowest lane's sieve iterations summed over chunks, exact = chunks the cell loop still ran on
+    printf("F1 prefixes %llu chunks %llu windows %llu cells %llu positions %llu packed %llu mixed %llu hits %llu quad %llu sieve %llu exact %llu\n",
         ctl->pad1[0], ctl->pad1[1], ctl->pad1[2], ctl->pad1[3], ctl->pad1[4], ctl->pad1[5],
-        ctl->pad1[6], ctl->hit_count, ctl->pad1[7]);
-    for (int i = 0; i < 8; i++) ctl->pad1[i] = 0;
+        ctl->pad1[6], ctl->hit_count, ctl->pad1[7], ctl->pad1[8], ctl->pad1[9]);
+    for (int i = 0; i < 10; i++) ctl->pad1[i] = 0;
 #endif
   }
   if (first >= handed) return;

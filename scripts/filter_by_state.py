@@ -1,5 +1,8 @@
 """Per-state kernel times of one bench step (n gates, the 8 states of step seed 1003): which of
-the four families dominates at each mask depth, and how long the lists are."""
+the four families dominates at each mask depth, and how long the lists are.  With a
+-DSBG_COUNT_FILTER build (SBG_LIB=...) every phase-1 launch also prints its F1 line: work units, and
+the pair sieve's `sieve` (slowest lane's iterations, summed over chunks) next to `positions`, and
+`exact` (chunks the sieve left to the cell loop) next to `chunks`."""
 import os
 import sys
 
