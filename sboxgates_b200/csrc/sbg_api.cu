@@ -11,6 +11,7 @@
 #include <cstring>
 #include <ctime>
 #include <map>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -142,13 +143,13 @@ struct sbg_lane {
   uint32_t *d_ecount = nullptr;             // matches per ticket
   unsigned long long *d_eoffset = nullptr;  // their exclusive prefix sum
   DevMatch *d_ematch = nullptr;             // the emitted records
-  uint64_t ecount_cap = 0, ematch_cap = 0;
+  uint64_t ecount_cap = 0, eoffset_cap = 0, ematch_cap = 0;
   // fetch and pick on an enumeration cursor (allocated on the first call)
   unsigned long long *d_pranks = nullptr;   // requested ranks, ascending
   unsigned int *d_pslots = nullptr;         // their output slots
   unsigned long long *d_ptickets = nullptr; // ticket of each rank, then the distinct tickets
   unsigned int *d_pfirst = nullptr;         // each distinct ticket's first rank in d_pranks
-  uint64_t pick_cap = 0;
+  uint64_t pranks_cap = 0, pslots_cap = 0, ptickets_cap = 0, pfirst_cap = 0;
   // global ranks (sbg_enum_block_sums / sbg_enum_set_global; allocated on the first call)
   unsigned long long *d_bsums = nullptr;    // the share's block sums
   unsigned long long *d_delta = nullptr;    // what k_enum_rebase adds to each of its blocks
@@ -336,6 +337,18 @@ cudaError_t launch(sbg_handle *h, void (*kernel)(KArgs...), int grid, int block,
   cfg.numAttrs = (pdl && h->opt_pdl != 0) ? 1 : 0;
   h->launches++;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+// f(nw_c) with the problem's table width in 32-bit words (1, 2, 4 or 8) as the compile-time
+// constant decltype(nw_c)::value, for the kernels templated on it.
+template <class F>
+auto with_nw(int nw, F &&f) {
+  switch (nw) {
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 4: return f(std::integral_constant<int, 4>());
+    default: return f(std::integral_constant<int, 8>());
+  }
 }
 
 // Prefixes per ticket batch.  One batch costs one global atomic; batches should hold enough pairs
@@ -607,29 +620,21 @@ int enqueue_search5(sbg_handle *h, sbg_lane &L, int part, int nparts, bool two) 
   const uint64_t tickets = pl.all ? 0 : (total - pl.t_offset + nparts - 1) / nparts;
   const uint64_t chunk_tickets = (pl.items + kDeal * nparts - 1) / (kDeal * nparts) * kDeal;
   if (h->timing) cudaEventRecord(L.ev[6], L.stream);
-  cudaError_t e = cudaSuccess;
-#define SBG_LAUNCH_SWEEP(NWV)                                                                  \
-  {                                                                                            \
-    const size_t smem = sweep_smem<NWV>(n);                                                    \
-    const int grid = grid_for(h, k_sweep<NWV>, smem, tickets + chunk_tickets);                 \
-    const uint64_t bsz = pick_batch(h, tickets, n, P);                                         \
-    e = launch(h, k_sweep<NWV>, grid, kThreads, smem, L.stream, !h->timing, h->d_slots + L.slot, \
-        L.d_ctl, L.d_out, L.d_pos5, L.d_hits, (unsigned long long)L.hits_cap, part, nparts,    \
-        (int)bsz, two, h->d_tab, pl.all ? (unsigned long long)total : pl.t_offset, pl.items,   \
-        std::max(1, pl.chunks), (unsigned long long)chunk_tickets);                            \
-    if (e == cudaSuccess && two) {                                                             \
-      const size_t smem2 = decomp_smem<NWV>(n);                                                \
-      e = launch(h, k_decomp5<NWV>, 2 * h->sm_count, kThreads, smem2, L.stream, true,          \
-          h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_pos5, L.d_hits, h->d_tab);                \
-    }                                                                                          \
-  }
-  switch (hp.nw) {
-    case 1: SBG_LAUNCH_SWEEP(1) break;
-    case 2: SBG_LAUNCH_SWEEP(2) break;
-    case 4: SBG_LAUNCH_SWEEP(4) break;
-    default: SBG_LAUNCH_SWEEP(8) break;
-  }
-#undef SBG_LAUNCH_SWEEP
+  const cudaError_t e = with_nw(hp.nw, [&](auto nw_c) {
+    constexpr int NW = decltype(nw_c)::value;
+    const size_t smem = sweep_smem<NW>(n);
+    const int grid = grid_for(h, k_sweep<NW>, smem, tickets + chunk_tickets);
+    const uint64_t bsz = pick_batch(h, tickets, n, P);
+    cudaError_t e = launch(h, k_sweep<NW>, grid, kThreads, smem, L.stream, !h->timing,
+        h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_pos5, L.d_hits, (unsigned long long)L.hits_cap,
+        part, nparts, (int)bsz, two, h->d_tab, pl.all ? (unsigned long long)total : pl.t_offset,
+        pl.items, std::max(1, pl.chunks), (unsigned long long)chunk_tickets);
+    if (e == cudaSuccess && two) {
+      e = launch(h, k_decomp5<NW>, 2 * h->sm_count, kThreads, decomp_smem<NW>(n), L.stream, true,
+          h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_pos5, L.d_hits, h->d_tab);
+    }
+    return e;
+  });
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "search5 launch: %s", cudaGetErrorString(e));
   if (h->timing) {
     cudaEventRecord(L.ev[7], L.stream);
@@ -764,73 +769,41 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
   const int n = hp.n;
   const int m = hp.m;
   const ChunkPlan &pl = fp.pl;
-  cudaError_t e = cudaSuccess;
-  int rc = SBG_OK;
-#define SBG_LAUNCH_PM_S(NWV, WV, FSV, SHV, SVV)                                                \
-  {                                                                                            \
-    const size_t smem = filter_pm_smem<NWV, P>(n, m, SHV, SVV);                                \
-    if ((rc = ensure_smem(h, k_filter7_pm<NWV, WV, P, FSV, SHV, SVV>, smem)) != SBG_OK) return rc; \
-    int grid = grid_for(h, k_filter7_pm<NWV, WV, P, FSV, SHV, SVV>, smem,                      \
-        fp.tickets + fp.chunk_tickets);                                                        \
-    if (fp.max_warps > 0) grid = std::min(grid, (fp.max_warps + kWarpsPerCta - 1) / kWarpsPerCta); \
-    e = launch(h, k_filter7_pm<NWV, WV, P, FSV, SHV, SVV>, grid, kThreads, smem, L.stream,     \
-        !h->timing, h->d_slots + L.slot, L.d_ctl, L.d_hits, L.d_aux, L.d_tcount, L.d_gcount,   \
-        (unsigned long long)L.hits_cap, (unsigned long long)fp.tickets_cap, part, nparts,      \
-        list_cap, (int)fp.batch, fp.max_warps,                                                 \
-        pl.all ? (unsigned long long)fp.total : pl.t_offset, pl.items, std::max(1, pl.chunks), \
-        (unsigned long long)fp.chunk_tickets, (unsigned long long)fp.seg_base,                 \
-        h->opt_packed ? 15 : 0, fp.wt);                                                        \
-  }
-#define SBG_LAUNCH_PM(NWV, WV, FSV, SHV) SBG_LAUNCH_PM_S(NWV, WV, FSV, SHV, false)
   const bool shifted = P == 4 && (h->opt_shift >= 0 ? h->opt_shift != 0 && n <= 63
                                                      : n <= kShiftMaxGates);
-  if constexpr (P == 4) {
-    // the pair sieve where it pays: it costs a fixed set-up per prefix, and under the smallest masks
-    // the cell loop it replaces visits too few positions per chunk (SBG_SIEVE=2: always)
-    const bool sieve = h->opt_sieve == 2 || (h->opt_sieve == 1 && m > kSieveMinPositions);
-    if (shifted && sieve) {
-      switch (hp.nw) {
-        case 1: SBG_LAUNCH_PM_S(1, 1, true, true, true) break;
-        case 2: SBG_LAUNCH_PM_S(2, 1, true, true, true) break;
-        case 4: SBG_LAUNCH_PM_S(4, 1, true, true, true) break;
-        default: SBG_LAUNCH_PM_S(8, 1, true, true, true) break;
-      }
-    } else if (shifted) {  // one word of 31 candidate gates from the first possible g on
-      switch (hp.nw) {
-        case 1: SBG_LAUNCH_PM(1, 1, true, true) break;
-        case 2: SBG_LAUNCH_PM(2, 1, true, true) break;
-        case 4: SBG_LAUNCH_PM(4, 1, true, true) break;
-        default: SBG_LAUNCH_PM(8, 1, true, true) break;
-      }
+  // the pair sieve where it pays: it costs a fixed set-up per prefix, and under the smallest masks
+  // the cell loop it replaces visits too few positions per chunk (SBG_SIEVE=2: always)
+  const bool sieve = h->opt_sieve == 2 || (h->opt_sieve == 1 && m > kSieveMinPositions);
+  return with_nw(hp.nw, [&](auto nw_c) {
+    constexpr int NW = decltype(nw_c)::value;
+    // one form of the kernel: the shifted / sieve flags also size its shared memory
+    auto run = [&](auto kernel, bool sh, bool sv) {
+      const size_t smem = filter_pm_smem<NW, P>(n, m, sh, sv);
+      int rc;
+      if ((rc = ensure_smem(h, kernel, smem)) != SBG_OK) return rc;
+      int grid = grid_for(h, kernel, smem, fp.tickets + fp.chunk_tickets);
+      if (fp.max_warps > 0) grid = std::min(grid, (fp.max_warps + kWarpsPerCta - 1) / kWarpsPerCta);
+      const cudaError_t e = launch(h, kernel, grid, kThreads, smem, L.stream, !h->timing,
+          h->d_slots + L.slot, L.d_ctl, L.d_hits, L.d_aux, L.d_tcount, L.d_gcount,
+          (unsigned long long)L.hits_cap, (unsigned long long)fp.tickets_cap, part, nparts,
+          list_cap, (int)fp.batch, fp.max_warps,
+          pl.all ? (unsigned long long)fp.total : pl.t_offset, pl.items, std::max(1, pl.chunks),
+          (unsigned long long)fp.chunk_tickets, (unsigned long long)fp.seg_base,
+          h->opt_packed ? 15 : 0, fp.wt);
+      if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_filter7_pm: %s", cudaGetErrorString(e));
+      return SBG_OK;
+    };
+    if constexpr (P == 4) {
+      if (shifted && sieve) return run(k_filter7_pm<NW, 1, P, true, true, true>, true, true);
+      // one word of 31 candidate gates from the first possible g on
+      if (shifted) return run(k_filter7_pm<NW, 1, P, true, true, false>, true, false);
     }
-  }
-  if (shifted) {
-  } else if (n <= 31) {  // one word of candidate gates per pass, its top bit free
-    switch (hp.nw) {
-      case 1: SBG_LAUNCH_PM(1, 1, true, false) break;
-      case 2: SBG_LAUNCH_PM(2, 1, true, false) break;
-      case 4: SBG_LAUNCH_PM(4, 1, true, false) break;
-      default: SBG_LAUNCH_PM(8, 1, true, false) break;
-    }
-  } else if (n <= 63) {  // two words, one pass, top bit free
-    switch (hp.nw) {
-      case 1: SBG_LAUNCH_PM(1, 2, true, false) break;
-      case 2: SBG_LAUNCH_PM(2, 2, true, false) break;
-      case 4: SBG_LAUNCH_PM(4, 2, true, false) break;
-      default: SBG_LAUNCH_PM(8, 2, true, false) break;
-    }
-  } else {
-    switch (hp.nw) {
-      case 1: SBG_LAUNCH_PM(1, 2, false, false) break;
-      case 2: SBG_LAUNCH_PM(2, 2, false, false) break;
-      case 4: SBG_LAUNCH_PM(4, 2, false, false) break;
-      default: SBG_LAUNCH_PM(8, 2, false, false) break;
-    }
-  }
-#undef SBG_LAUNCH_PM
-#undef SBG_LAUNCH_PM_S
-  if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_filter7_pm: %s", cudaGetErrorString(e));
-  return SBG_OK;
+    // one word of candidate gates per pass, its top bit free
+    if (n <= 31) return run(k_filter7_pm<NW, 1, P, true, false, false>, false, false);
+    // two words, one pass, top bit free
+    if (n <= 63) return run(k_filter7_pm<NW, 2, P, true, false, false>, false, false);
+    return run(k_filter7_pm<NW, 2, P, false, false, false>, false, false);
+  });
 }
 
 // Phase 1 on lane L: the filter, then the ordered, capped list in L.d_sorted (ctl->list_count).
@@ -864,22 +837,14 @@ int enqueue_filter7(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int part, 
 int enqueue_decomp7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint64_t items_hint) {
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const int n = hp.n;
-  cudaError_t e = cudaSuccess;
-#define SBG_LAUNCH_DECOMP(NWV)                                                                 \
-  {                                                                                            \
-    const size_t smem = decomp_smem<NWV>(n);                                                   \
-    const int grid = grid_for(h, k_decomp7<NWV>, smem, items_hint);                            \
-    e = launch(h, k_decomp7<NWV>, grid, kThreads, smem, L.stream, !h->timing,                  \
-        h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_par7, L.d_sorted, part, nparts, h->d_tab,   \
-        h->opt_decomp_filter);                                                                 \
-  }
-  switch (hp.nw) {
-    case 1: SBG_LAUNCH_DECOMP(1) break;
-    case 2: SBG_LAUNCH_DECOMP(2) break;
-    case 4: SBG_LAUNCH_DECOMP(4) break;
-    default: SBG_LAUNCH_DECOMP(8) break;
-  }
-#undef SBG_LAUNCH_DECOMP
+  const cudaError_t e = with_nw(hp.nw, [&](auto nw_c) {
+    constexpr int NW = decltype(nw_c)::value;
+    const size_t smem = decomp_smem<NW>(n);
+    const int grid = grid_for(h, k_decomp7<NW>, smem, items_hint);
+    return launch(h, k_decomp7<NW>, grid, kThreads, smem, L.stream, !h->timing,
+        h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_par7, L.d_sorted, part, nparts, h->d_tab,
+        h->opt_decomp_filter);
+  });
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_decomp7: %s", cudaGetErrorString(e));
   if (h->timing) cudaEventRecord(L.ev[3], L.stream);
   return SBG_OK;
@@ -1419,27 +1384,26 @@ constexpr uint64_t kEnumWindow3 = kNominalWarps;
 constexpr uint64_t kEnumWindow5 = kNominalWarps;
 constexpr uint64_t kEnumWindow7 = kNominalWarps / 4;
 
-int ensure_enum(sbg_handle *h, sbg_lane &L, uint64_t tickets, uint64_t matches) {
-  if (L.d_ectl == nullptr) SBG_CUDA(h, cudaMalloc(&L.d_ectl, sizeof(EnumCtl)));
-  if (L.ecount_cap < tickets) {
-    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-    cudaFree(L.d_ecount);
-    cudaFree(L.d_eoffset);
-    L.d_ecount = nullptr;
-    L.d_eoffset = nullptr;
-    L.ecount_cap = 0;
-    SBG_CUDA(h, cudaMalloc(&L.d_ecount, tickets * sizeof(uint32_t)));
-    SBG_CUDA(h, cudaMalloc(&L.d_eoffset, tickets * sizeof(unsigned long long)));
-    L.ecount_cap = tickets;
-  }
-  if (L.ematch_cap < matches) {
-    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-    cudaFree(L.d_ematch);
-    L.d_ematch = nullptr;
-    L.ematch_cap = 0;
-    SBG_CUDA(h, cudaMalloc(&L.d_ematch, matches * sizeof(DevMatch)));
-    L.ematch_cap = matches;
-  }
+// Grows the lane's device buffer p (cap elements now) to `need` elements.  The lane's queued work
+// may still read the old buffer, so growing waits for it; the contents are not kept.
+template <class T>
+int grow(sbg_handle *h, sbg_lane &L, T *&p, uint64_t &cap, uint64_t need) {
+  if (cap >= need) return SBG_OK;
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  cudaFree(p);
+  p = nullptr;
+  cap = 0;
+  SBG_CUDA(h, cudaMalloc(&p, need * sizeof(T)));
+  cap = need;
+  return SBG_OK;
+}
+
+// The first n emitted records to the caller's out.
+int copy_matches(sbg_handle *h, sbg_lane &L, sbg_match *out, uint64_t n) {
+  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, n * sizeof(sbg_match), cudaMemcpyDeviceToHost,
+      L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  h->d2h_bytes += n * sizeof(sbg_match);
   return SBG_OK;
 }
 
@@ -1451,63 +1415,78 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
   static_assert(WIDTH == 3 || WIDTH == 5 || WIDTH == 7, "enumeration widths are 3, 5 and 7");
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const int n = hp.n;
-  const EnumOrders &ord = in.ord;
-  cudaError_t e = cudaSuccess;
-  int rc = SBG_OK;
-#define SBG_LAUNCH_ENUM(NWV)                                                                   \
-  {                                                                                            \
-    if (WIDTH == 3) {                                                                          \
-      const size_t smem = decomp_smem<NWV>(n);                                                 \
-      auto kern = k_enum3<NWV, MODE>;                                                          \
-      if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
-      e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
-          h->d_slots + L.slot, L.d_ectl, in.gates, L.d_ecount,                                 \
-          (const unsigned long long *)L.d_eoffset, L.d_ematch, (unsigned long long)max_out,    \
-          (unsigned long long)a, (unsigned long long)b, part, nparts);                         \
-    } else if (WIDTH == 7) {                                                                   \
-      const size_t smem = decomp_smem<NWV>(n);                                                 \
-      auto kern = k_enum7<NWV, MODE>;                                                          \
-      if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
-      e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
-          h->d_slots + L.slot, L.d_ectl, ord, (const uint64_t *)L.d_sorted,                    \
-          (unsigned int)L.list_count, L.d_ecount, (const unsigned long long *)L.d_eoffset,     \
-          L.d_ematch, (unsigned long long)max_out, (unsigned long long)a,                      \
-          (unsigned long long)b, part, nparts, (const DevTables *)h->d_tab);                   \
-    } else {                                                                                   \
-      const size_t smem = sweep_smem<NWV>(n);                                                  \
-      auto kern = k_enum5<NWV, MODE>;                                                          \
-      if ((rc = ensure_smem(h, kern, smem)) != SBG_OK) return rc;                              \
-      e = launch(h, kern, grid_for(h, kern, smem, b - a), kThreads, smem, L.stream, false,     \
-          h->d_slots + L.slot, L.d_ectl, ord, L.d_ecount,                                      \
-          (const unsigned long long *)L.d_eoffset, L.d_ematch, (unsigned long long)max_out,    \
-          (unsigned long long)a, (unsigned long long)b, part, nparts,                          \
-          (const DevTables *)h->d_tab);                                                        \
-    }                                                                                          \
-  }
-  switch (hp.nw) {
-    case 1: SBG_LAUNCH_ENUM(1) break;
-    case 2: SBG_LAUNCH_ENUM(2) break;
-    case 4: SBG_LAUNCH_ENUM(4) break;
-    default: SBG_LAUNCH_ENUM(8) break;
-  }
-#undef SBG_LAUNCH_ENUM
-  if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "enumeration launch: %s", cudaGetErrorString(e));
+  const DevProblem *prob = h->d_slots + L.slot;
+  const int rc = with_nw(hp.nw, [&](auto nw_c) {
+    constexpr int NW = decltype(nw_c)::value;
+    auto run = [&](auto kernel, size_t smem, auto... args) {
+      int rc;
+      if ((rc = ensure_smem(h, kernel, smem)) != SBG_OK) return rc;
+      const cudaError_t e = launch(h, kernel, grid_for(h, kernel, smem, b - a), kThreads, smem,
+          L.stream, false, args...);
+      if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "enumeration launch: %s", cudaGetErrorString(e));
+      return SBG_OK;
+    };
+    if constexpr (WIDTH == 3) {
+      return run(k_enum3<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates, L.d_ecount,
+          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts);
+    } else if constexpr (WIDTH == 5) {
+      return run(k_enum5<NW, MODE>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
+          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab);
+    } else {
+      return run(k_enum7<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
+          L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab);
+    }
+  });
+  if (rc != SBG_OK) return rc;
   if (MODE == kEnumCount) {
-    e = launch(h, k_enum_scan, 1, 1024, 0, L.stream, false, L.d_ectl, (const uint32_t *)L.d_ecount,
-        L.d_eoffset, (unsigned long long)a, (unsigned long long)b);
+    const cudaError_t e = launch(h, k_enum_scan, 1, 1024, 0, L.stream, false, L.d_ectl,
+        (const uint32_t *)L.d_ecount, L.d_eoffset, (unsigned long long)a, (unsigned long long)b);
     if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_scan: %s", cudaGetErrorString(e));
   }
   return SBG_OK;
 }
 
-// Count pass (in windows when only the first max_matches are wanted), offsets, emit pass, copy-out.
-// The lane's problem is prepared on the device.
+// Deal blocks part q of nparts holds out of `blocks` (blocks q, q + nparts, ...).
+uint64_t deal_share(uint64_t blocks, int q, int nparts) {
+  return blocks > (uint64_t)q ? (blocks - q + nparts - 1) / nparts : 0;
+}
+
+// Tickets per deal block of an enumeration of `width`: kDeal position pairs or 3-gate prefixes, or
+// one 7-LUT list entry.
+unsigned int enum_block_size(int width) { return width == 7 ? 1u : (unsigned)kDeal; }
+
+// sbg_enum3 / sbg_enum5 / sbg_enum7 once their arguments are checked.  Lane 0 takes the current
+// problem slot, and k_begin (flags, begin_in) brings its problem block up to date; a 7-LUT
+// enumeration without an installed list runs phase 1 instead, which does that and installs the
+// list.  Then the part's tickets are counted (in windows when only the first max_matches are
+// wanted), their offsets taken, and the first max_matches emitted and copied out.
 template <int WIDTH>
-int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int nparts,
-    uint64_t blocks, uint64_t tickets, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
+int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const EnumInputs &in,
+    int part, int nparts, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
     uint64_t *feasible) {
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
   int rc;
-  if ((rc = ensure_enum(h, L, std::max<uint64_t>(tickets, 1), 0)) != SBG_OK) return rc;
+  if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
+  if (WIDTH == 7 && !L.list_ready) {
+    uint32_t count = 0;
+    if ((rc = run_filter7(h, L, 0, 1, &count)) != SBG_OK) return rc;
+    L.list_count = count;
+    L.list_ready = true;
+  } else {
+    L.seq++;
+    if ((rc = enqueue_begin(h, L, flags, begin_in, 0)) != SBG_OK) return rc;
+  }
+  // this part's tickets: its deal blocks (the last one may be cut short)
+  const int n = h->slots[L.slot].n;
+  const uint64_t B = enum_block_size(WIDTH);
+  const uint64_t items = WIDTH == 3 ? h_binom[n][2] : WIDTH == 5 ? h_binom[n - 2][3] : L.list_count;
+  const uint64_t blocks = (items + B - 1) / B;
+  const uint64_t tickets = deal_share(blocks, part, nparts) * B;
+  if (L.d_ectl == nullptr) SBG_CUDA(h, cudaMalloc(&L.d_ectl, sizeof(EnumCtl)));
+  const uint64_t room = std::max<uint64_t>(tickets, 1);
+  if ((rc = grow(h, L, L.d_ecount, L.ecount_cap, room)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_eoffset, L.eoffset_cap, room)) != SBG_OK) return rc;
   SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
   const bool count_all = total != nullptr;
   uint64_t window = count_all ? tickets
@@ -1531,12 +1510,9 @@ int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int npa
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   const uint64_t emit = std::min<uint64_t>(max_matches, ec.carry);
   if (emit > 0) {
-    if ((rc = ensure_enum(h, L, 0, emit)) != SBG_OK) return rc;
+    if ((rc = grow(h, L, L.d_ematch, L.ematch_cap, emit)) != SBG_OK) return rc;
     if ((rc = launch_enum<WIDTH, kEnumFirst>(h, L, in, part, nparts, emit, 0, done)) != SBG_OK) return rc;
-    SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, emit * sizeof(sbg_match), cudaMemcpyDeviceToHost,
-        L.stream));
-    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-    h->d2h_bytes += emit * sizeof(sbg_match);
+    if ((rc = copy_matches(h, L, out, emit)) != SBG_OK) return rc;
   }
   *n_out = emit;
   if (count_all) {
@@ -1556,12 +1532,19 @@ int run_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int npa
     c.global = false;
   }
   if (total != nullptr) *total = ec.carry;
-  if (feasible != nullptr) *feasible = WIDTH == 7 ? (uint64_t)L.list_count : ec.feasible;
+  if (feasible != nullptr) {
+    // width 3: every feasible triple is a match
+    *feasible = WIDTH == 7 ? (uint64_t)L.list_count : WIDTH == 3 ? ec.total : ec.feasible;
+  }
   return SBG_OK;
 }
 
+// The checks every sbg_enum3 / sbg_enum5 / sbg_enum7 call starts with.  The call ends the
+// enumeration cursor, whether it succeeds or not.
 int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, sbg_match *out,
     uint64_t *n_out) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;
   if (n_out == nullptr || (max_matches > 0 && out == nullptr)) return fail(h, SBG_ERR_ARG, "null output");
   if (max_matches > SBG_ENUM_MAX_MATCHES) {
     return fail(h, SBG_ERR_ARG, "max_matches %llu above %u", (unsigned long long)max_matches,
@@ -1573,26 +1556,6 @@ int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, s
 }
 
 // ---- fetch and pick on the enumeration cursor (sbg_enum_fetch / sbg_enum_pick) ---------------------
-
-int ensure_pick(sbg_handle *h, sbg_lane &L, uint64_t nranks) {
-  if (L.pick_cap >= nranks) return SBG_OK;
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  cudaFree(L.d_pranks);
-  cudaFree(L.d_pslots);
-  cudaFree(L.d_ptickets);
-  cudaFree(L.d_pfirst);
-  L.d_pranks = nullptr;
-  L.d_pslots = nullptr;
-  L.d_ptickets = nullptr;
-  L.d_pfirst = nullptr;
-  L.pick_cap = 0;
-  SBG_CUDA(h, cudaMalloc(&L.d_pranks, nranks * sizeof(unsigned long long)));
-  SBG_CUDA(h, cudaMalloc(&L.d_pslots, nranks * sizeof(unsigned int)));
-  SBG_CUDA(h, cudaMalloc(&L.d_ptickets, nranks * sizeof(unsigned long long)));
-  SBG_CUDA(h, cudaMalloc(&L.d_pfirst, (nranks + 1) * sizeof(unsigned int)));
-  L.pick_cap = nranks;
-  return SBG_OK;
-}
 
 // The cursor, if it is still valid (nothing has run on the handle since the count that made it).
 int check_cursor(sbg_handle *h) {
@@ -1623,34 +1586,15 @@ int locate_tickets(sbg_handle *h, sbg_lane &L, uint64_t nranks, bool owned = fal
 
 // ---- global ranks across shares (sbg_enum_block_sums / sbg_enum_set_global) ---------------------
 
-// Deal blocks part q of nparts holds out of `blocks` (blocks q, q + nparts, ...).
-uint64_t deal_share(uint64_t blocks, int q, int nparts) {
-  return blocks > (uint64_t)q ? (blocks - q + nparts - 1) / nparts : 0;
-}
-
-// Tickets per deal block of the cursor's width.
-unsigned int cursor_block_size(const EnumCursor &c) { return c.width == 7 ? 1u : (unsigned)kDeal; }
-
-int grow_u64(sbg_handle *h, sbg_lane &L, unsigned long long *&p, uint64_t &cap, uint64_t need) {
-  if (cap >= need) return SBG_OK;
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  cudaFree(p);
-  p = nullptr;
-  cap = 0;
-  SBG_CUDA(h, cudaMalloc(&p, need * sizeof(unsigned long long)));
-  cap = need;
-  return SBG_OK;
-}
-
 // The cursor's block sums into L.d_bsums (and room for as many deltas in L.d_delta).
 int block_sums(sbg_handle *h, sbg_lane &L, uint64_t nblocks) {
   int rc;
-  if ((rc = grow_u64(h, L, L.d_bsums, L.bsums_cap, nblocks)) != SBG_OK) return rc;
-  if ((rc = grow_u64(h, L, L.d_delta, L.delta_cap, nblocks)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_bsums, L.bsums_cap, nblocks)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_delta, L.delta_cap, nblocks)) != SBG_OK) return rc;
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nblocks + 255) / 256,
       (uint64_t)h->sm_count * 8));
   const cudaError_t e = launch(h, k_enum_block_sums, grid, 256, 0, L.stream, false,
-      (const uint32_t *)L.d_ecount, (unsigned long long)nblocks, cursor_block_size(h->cursor),
+      (const uint32_t *)L.d_ecount, (unsigned long long)nblocks, enum_block_size(h->cursor.width),
       L.d_bsums);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_block_sums: %s", cudaGetErrorString(e));
   return SBG_OK;
@@ -2513,67 +2457,38 @@ int sbg_search7(sbg_handle *h, const uint8_t *outer_order, const uint8_t *middle
 
 int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, uint64_t max_matches,
     sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible) {
-  if (h == nullptr) return SBG_ERR_ARG;
-  h->api_seq++;   // ends the enumeration cursor
   int rc;
   if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
-  const sbg_handle::HostProblem &hp = cur(h);
-  if (hp.n < 5) return fail(h, SBG_ERR_ARG, "search_5lut needs n >= 5 (lut.c:119)");
+  if (cur(h).n < 5) return fail(h, SBG_ERR_ARG, "search_5lut needs n >= 5 (lut.c:119)");
   if (!valid_order(func_order)) return fail(h, SBG_ERR_ARG, "func_order is not a permutation");
-  SBG_CUDA(h, cudaSetDevice(h->device));
-  sbg_lane &L = h->lane[0];
-  if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
-  L.seq++;
   CallInputs in;
   in.order5 = func_order;
-  if ((rc = enqueue_begin(h, L, kBeginSearch5, in, 0)) != SBG_OK) return rc;
-  // this part's tickets: its deal blocks of kDeal prefixes (the last one may be cut short)
-  const uint64_t blocks = (h_binom[hp.n - 2][3] + kDeal - 1) / kDeal;
-  const uint64_t mine = blocks > (uint64_t)part ? (blocks - part + nparts - 1) / nparts : 0;
   EnumInputs in5;
   memcpy(in5.ord.order[0], func_order, 256);
   memset(in5.ord.order[1], 0, 256);
-  return run_enum<5>(h, L, in5, part, nparts, blocks, mine * kDeal, max_matches, out, n_out, total,
+  return run_enum<5>(h, kBeginSearch5, in, in5, part, nparts, max_matches, out, n_out, total,
       feasible);
 }
 
 int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
     uint64_t *total, uint64_t *feasible) {
-  if (h == nullptr) return SBG_ERR_ARG;
-  h->api_seq++;   // ends the enumeration cursor
   int rc;
   if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
   if (cur(h).n < 7) return fail(h, SBG_ERR_ARG, "search_7lut needs n >= 7 (lut.c:259)");
   if (!valid_order(outer_order) || !valid_order(middle_order)) {
     return fail(h, SBG_ERR_ARG, "function order is not a permutation");
   }
-  SBG_CUDA(h, cudaSetDevice(h->device));
-  sbg_lane &L = h->lane[0];
-  if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
-  if (L.list_ready) {
-    // the installed list: only bring the problem block up to date
-    L.seq++;
-    CallInputs none;
-    if ((rc = enqueue_begin(h, L, kBeginKeepCtl, none, 0)) != SBG_OK) return rc;
-  } else {
-    uint32_t count = 0;
-    if ((rc = run_filter7(h, L, 0, 1, &count)) != SBG_OK) return rc;
-    L.list_count = count;
-    L.list_ready = true;
-  }
-  const uint64_t count = L.list_count;
-  const uint64_t mine = count > (uint64_t)part ? (count - part + nparts - 1) / nparts : 0;
   EnumInputs in7;
   memcpy(in7.ord.order[0], outer_order, 256);
   memcpy(in7.ord.order[1], middle_order, 256);
-  return run_enum<7>(h, L, in7, part, nparts, count, mine, max_matches, out, n_out, total, feasible);
+  // the installed list: only bring the problem block up to date
+  return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
+      total, feasible);
 }
 
 int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
     uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible) {
-  if (h == nullptr) return SBG_ERR_ARG;
-  h->api_seq++;   // ends the enumeration cursor
   int rc;
   if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
   const int n = cur(h).n;
@@ -2587,21 +2502,12 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
     }
     seen[gate_order[i]] = true;
   }
-  SBG_CUDA(h, cudaSetDevice(h->device));
-  sbg_lane &L = h->lane[0];
-  if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
-  // only bring the problem block up to date: the control words of an installed 7-LUT list stay
-  L.seq++;
-  CallInputs none;
-  if ((rc = enqueue_begin(h, L, kBeginKeepCtl, none, 0)) != SBG_OK) return rc;
-  // this part's tickets: its deal blocks of kDeal position pairs (the last one may be cut short)
-  const uint64_t blocks = (h_binom[n][2] + kDeal - 1) / kDeal;
-  const uint64_t mine = blocks > (uint64_t)part ? (blocks - part + nparts - 1) / nparts : 0;
   EnumInputs in3;
   memset(&in3, 0, sizeof(in3));
   memcpy(in3.gates.order, gate_order, sizeof(uint16_t) * (size_t)n);
-  return run_enum<3>(h, L, in3, part, nparts, blocks, mine * kDeal, max_matches, out, n_out, total,
-      feasible);
+  // only bring the problem block up to date: the control words of an installed 7-LUT list stay
+  return run_enum<3>(h, kBeginKeepCtl, CallInputs(), in3, part, nparts, max_matches, out, n_out,
+      total, feasible);
 }
 
 int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out, uint64_t *n_out) {
@@ -2619,8 +2525,9 @@ int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out
   const uint64_t n = std::min(count, c.total - first);
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
-  if ((rc = ensure_pick(h, L, 2)) != SBG_OK) return rc;
-  if ((rc = ensure_enum(h, L, 0, n)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_pranks, L.pranks_cap, 2)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_ptickets, L.ptickets_cap, 2)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_ematch, L.ematch_cap, n)) != SBG_OK) return rc;
   // global ranks: the share writes the ranks it owns, zero records elsewhere
   if (c.global) SBG_CUDA(h, cudaMemsetAsync(L.d_ematch, 0, n * sizeof(sbg_match), L.stream));
   // the tickets of the window's first and last rank; the launch covers them and those between
@@ -2637,10 +2544,7 @@ int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out
   if (c.tickets > 0 && (rc = emit_sel<kEnumRange>(h, L, first + n, tk[0], tk[1] + 1, sel)) != SBG_OK) {
     return rc;
   }
-  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, n * sizeof(sbg_match), cudaMemcpyDeviceToHost,
-      L.stream));
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  h->d2h_bytes += n * sizeof(sbg_match);
+  if ((rc = copy_matches(h, L, out, n)) != SBG_OK) return rc;
   *n_out = n;
   return SBG_OK;
 }
@@ -2674,17 +2578,15 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
   }
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
-  if ((rc = ensure_pick(h, L, nranks)) != SBG_OK) return rc;
-  if ((rc = ensure_enum(h, L, 0, nranks)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_pranks, L.pranks_cap, nranks)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_pslots, L.pslots_cap, nranks)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_ptickets, L.ptickets_cap, nranks)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_pfirst, L.pfirst_cap, nranks + 1)) != SBG_OK) return rc;
+  if ((rc = grow(h, L, L.d_ematch, L.ematch_cap, nranks)) != SBG_OK) return rc;
   // global ranks: the share writes the ranks it owns, zero records elsewhere
   if (c.global) SBG_CUDA(h, cudaMemsetAsync(L.d_ematch, 0, nranks * sizeof(sbg_match), L.stream));
-  if (c.tickets == 0) {   // a share without tickets (global ranks only) owns no rank
-    SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, nranks * sizeof(sbg_match), cudaMemcpyDeviceToHost,
-        L.stream));
-    SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-    h->d2h_bytes += nranks * sizeof(sbg_match);
-    return SBG_OK;
-  }
+  // a share without tickets (global ranks only) owns no rank
+  if (c.tickets == 0) return copy_matches(h, L, out, nranks);
   // device: the ticket of every rank; host: the distinct tickets and their slices of the ranks.
   // Global ranks another share owns are dropped here, so that no warp sweeps a ticket for a rank
   // it never meets.
@@ -2725,11 +2627,7 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
   sel.tickets = L.d_ptickets;
   sel.first = L.d_pfirst;
   if (d > 0 && (rc = emit_sel<kEnumPick>(h, L, 0, 0, d, sel)) != SBG_OK) return rc;
-  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, nranks * sizeof(sbg_match), cudaMemcpyDeviceToHost,
-      L.stream));
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  h->d2h_bytes += nranks * sizeof(sbg_match);
-  return SBG_OK;
+  return copy_matches(h, L, out, nranks);
 }
 
 int sbg_enum_block_sums(sbg_handle *h, uint64_t *out, uint64_t *nblocks) {
@@ -2738,7 +2636,7 @@ int sbg_enum_block_sums(sbg_handle *h, uint64_t *out, uint64_t *nblocks) {
   int rc;
   if ((rc = check_cursor(h)) != SBG_OK) return rc;
   const EnumCursor &c = h->cursor;
-  const uint64_t nb = c.tickets / cursor_block_size(c);
+  const uint64_t nb = c.tickets / enum_block_size(c.width);
   *nblocks = nb;
   if (out == nullptr || nb == 0) return SBG_OK;
   SBG_CUDA(h, cudaSetDevice(h->device));
@@ -2777,12 +2675,12 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
   if (sums == nullptr && widest > 0) return fail(h, SBG_ERR_ARG, "null sums");
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
-  const unsigned int B = cursor_block_size(c);
+  const unsigned int B = enum_block_size(c.width);
   const uint64_t nb = c.tickets / B;
   uint64_t whole = 0;
   if (c.blocks > 0) {
     // the rows, packed at stride `widest` on the device
-    if ((rc = grow_u64(h, L, L.d_gsums, L.gsums_cap, (uint64_t)nparts * widest)) != SBG_OK) return rc;
+    if ((rc = grow(h, L, L.d_gsums, L.gsums_cap, (uint64_t)nparts * widest)) != SBG_OK) return rc;
     for (int q = 0; q < nparts; q++) {
       if (counts[q] == 0) continue;
       SBG_CUDA(h, cudaMemcpyAsync(L.d_gsums + (uint64_t)q * widest, sums + (uint64_t)q * stride,

@@ -144,6 +144,12 @@ __device__ __forceinline__ unsigned lanemask_lt() {
   return m;
 }
 
+// Item t of one part of a sharded sweep, as an item of the whole: items are dealt to the parts in
+// blocks of kDeal consecutive items, part p owning blocks p, p + nparts, ...
+__device__ __forceinline__ uint64_t dealt_item(uint64_t t, int part, int nparts) {
+  return (t / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal + t % kDeal;
+}
+
 // Stages `rows` rows of `npad` words of the problem's tables into shared memory with cp.async.
 __device__ __forceinline__ void stage_tables(uint32_t *s_tabs, const DevProblem *prob, int rows,
     int npad) {
@@ -508,8 +514,7 @@ __global__ void __launch_bounds__(kThreads) k_sweep(const DevProblem *__restrict
     // state the tuples in front of the first match are then decomposed by many warps, not one.
     const bool chunked = b < chunk_tickets;
     const uint64_t lt = chunked ? b : (b - chunk_tickets) * (uint64_t)batch;
-    const uint64_t dealt = (lt / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal
-        + (lt % kDeal);
+    const uint64_t dealt = dealt_item(lt, part, nparts);
     uint64_t t_first, t_end;
     uint32_t q_begin = 0, q_limit = 0xffffffffu;
     int pre[P];
@@ -1022,8 +1027,7 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
     const bool weighted = P == 4 && wt.group_pairs != 0;   // every ticket = (prefix, group of pairs)
     const bool chunked = !weighted && bg < chunk_tickets;
     const uint64_t lt = (chunked || weighted) ? bg : (bg - chunk_tickets) * (uint64_t)batch;
-    const uint64_t dealt = (lt / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal
-        + (lt % kDeal);
+    const uint64_t dealt = dealt_item(lt, part, nparts);
     bool valid = true;
     if (weighted) {
       if (dealt >= (uint64_t)wt.total) {   // past the end: every later ticket is, too
@@ -2530,13 +2534,14 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
 // search_5lut / search_7lut, not only the first.  The same decisions as the searches above with
 // nothing thrown away, in two passes over the same tickets -- a position pair of the gate order, a
 // 3-gate prefix of C(n,5) (dealt to the parts as k_sweep deals them) or one list entry:
-//   count (EMIT = false): the number of matches of each ticket, and their sum;
+//   count: the number of matches of each ticket, and their sum;
 //   k_enum_scan: exclusive prefix sum of those counts = where each ticket's matches start in the
 //     ascending key order;
-//   emit (EMIT = true): the tickets whose matches start below K write them there, in key order,
-//     decoded into DevMatch records.
+//   emit: the tickets whose matches start below K write them there, in key order, decoded into
+//     DevMatch records.
 // Tickets are numbered in key order, so the order needs no sort.  Both passes run the identical
-// sweep, so a ticket emits exactly the matches it counted.
+// sweep, so a ticket emits exactly the matches it counted: each kernel holds one sweep of a ticket,
+// enum_tickets runs it for every pass, and every ballot of matches goes through emit_step.
 //
 // After a count, any rank of the share can be emitted again from counts and offsets alone
 // (sbg_enum_fetch / sbg_enum_pick): the emit pass of the same sweep, run over the tickets that hold
@@ -2558,23 +2563,38 @@ struct EnumSel {
   const unsigned int *first;              //   ticket j's ranks: ranks[first[j] .. first[j+1]-1]
 };
 
-// One step of an emit sweep: the warp's ballot covers ranks [step_end - popc(ballot), step_end), the
-// lane's own match (if hit) has rank `at`.  write(i) writes the lane's match to out[i].  Pick: the
-// requests of this step are consumed in order from req (warp-uniform), each written by the lane that
-// holds its rank.
+// Where a pass stands in the ticket a warp sweeps (warp-uniform).
+struct EnumTicket {
+  EnumSel sel;                   // range / pick: what to emit
+  unsigned long long max_out;    // first / range: the end of the wanted ranks
+  unsigned long long base;       // emit: rank of the ticket's first match
+  uint32_t count;                // matches met so far (count pass: the ticket's count)
+  unsigned int req, req_end;     // pick: the ticket's requests not yet met
+};
+
+// One ballot of a sweep: the lanes with hit hold the next matches of the ticket, in lane order.  The
+// ballot covers ranks [step_end - popc(ballot), step_end), the lane's own match has rank `at`, and
+// write(i) writes the lane's match to out[i].  Pick: the requests of this step are consumed in
+// order from req, each written by the lane that holds its rank.  Returns whether the ticket has
+// nothing more to emit (never in the count pass).
 template <int MODE, class Write>
-__device__ __forceinline__ void emit_step(bool hit, unsigned long long at, unsigned long long step_end,
-    unsigned long long max_out, const EnumSel &sel, unsigned int &req, unsigned int req_end,
-    Write write) {
+__device__ __forceinline__ bool emit_step(bool hit, EnumTicket &tk, Write write) {
+  const uint32_t bal = __ballot_sync(kFull, hit);
+  const unsigned long long at = tk.base + tk.count + __popc(bal & lanemask_lt());
+  const unsigned long long step_end = tk.base + tk.count + __popc(bal);
   if (MODE == kEnumPick) {
-    for (; req < req_end; req++) {
-      const unsigned long long r = sel.ranks[req];
+    for (; tk.req < tk.req_end; tk.req++) {
+      const unsigned long long r = tk.sel.ranks[tk.req];
       if (r >= step_end) break;
-      if (hit && at == r) write((unsigned long long)sel.slots[req]);
+      if (hit && at == r) write((unsigned long long)tk.sel.slots[tk.req]);
     }
-  } else if (hit && at < max_out && (MODE != kEnumRange || at >= sel.lo)) {
-    write(MODE == kEnumRange ? at - sel.lo : at);
+  } else if (MODE != kEnumCount && hit && at < tk.max_out
+             && (MODE != kEnumRange || at >= tk.sel.lo)) {
+    write(MODE == kEnumRange ? at - tk.sel.lo : at);
   }
+  tk.count += __popc(bal);
+  if (MODE == kEnumCount) return false;
+  return MODE == kEnumPick ? tk.req >= tk.req_end : tk.base + tk.count >= tk.max_out;
 }
 
 // The layout of sbg_match (include/sboxgates_b200.h; sbg_api.cu checks that the two agree).
@@ -2595,6 +2615,47 @@ struct EnumCtl {
   unsigned int gbad;            //   1 if the share's own row of block sums differs from its own
 };
 
+// The ticket loop of the enumeration kernels: one warp per ticket of t_begin .. t_end-1 (pick: per
+// entry j of sel.tickets, ticket sel.tickets[j]); the emit passes skip the tickets that hold no
+// wanted rank.  sweep(t, tk, feasible) sweeps ticket t, passing every ballot of matches to
+// emit_step.  In the count pass it leaves the ticket's matches in tk.count (and the 5-LUT sweep adds
+// the feasible tuples it met to feasible); the tickets' counts and both sums are written back here.
+template <int MODE, class Sweep>
+__device__ __forceinline__ void enum_tickets(EnumCtl *__restrict__ ectl,
+    uint32_t *__restrict__ counts, const unsigned long long *__restrict__ offsets,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, Sweep sweep) {
+  EnumTicket tk = {};
+  if (MODE == kEnumRange || MODE == kEnumPick) tk.sel = ectl->sel;
+  tk.max_out = max_out;
+  const int lane = threadIdx.x & 31;
+  const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
+  unsigned long long matches_local = 0, feasible_local = 0;
+  for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta
+           + (threadIdx.x >> 5);
+       j < t_end; j += nwarps) {
+    const unsigned long long t = MODE == kEnumPick ? tk.sel.tickets[j] : j;
+    if (MODE != kEnumCount) {
+      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
+      if (MODE == kEnumRange && offsets[t] + counts[t] <= tk.sel.lo) continue;
+      if (MODE == kEnumPick) {
+        tk.req = tk.sel.first[j];
+        tk.req_end = tk.sel.first[j + 1];
+      }
+      tk.base = offsets[t];
+    }
+    tk.count = 0;
+    sweep(t, tk, feasible_local);
+    if (MODE == kEnumCount) {
+      if (lane == 0) counts[t] = tk.count;
+      matches_local += tk.count;
+    }
+  }
+  if (MODE == kEnumCount && lane == 0) {
+    if (matches_local != 0) atomicAdd(&ectl->total, matches_local);
+    if (feasible_local != 0) atomicAdd(&ectl->feasible, feasible_local);
+  }
+}
+
 struct EnumOrders {
   uint8_t order[2][256];   // the shuffled function order(s): [0] outer (5-LUT: the only one), [1] middle
 };
@@ -2612,9 +2673,28 @@ __device__ __forceinline__ uint32_t lut_word(uint32_t func, uint32_t x, uint32_t
   return r;
 }
 
-// A match's record: gates in reference order (tuple positions of ordering row k), func_inner = solved bits only
-// and inner_seen = cells with a masked position (sbg_solve_inner's closed form, on the compressed
-// tables; a match has no conflicting cell).  width 5: func_middle unused.
+// A match's record of width 3, 5 or 7: the first WIDTH gates of G, zeros in the fields the width
+// does not use (func_outer at width 3, func_middle below width 7).
+template <int WIDTH>
+__device__ __forceinline__ void store_match(DevMatch *__restrict__ dst, unsigned long long key,
+    const int *G, uint32_t fo, uint32_t fm, uint32_t inner, uint32_t seen) {
+  DevMatch m;
+  m.key = key;
+#pragma unroll
+  for (int i = 0; i < 7; i++) m.gates[i] = i < WIDTH ? (uint16_t)G[i] : (uint16_t)0;
+  m.func_outer = WIDTH > 3 ? (uint8_t)fo : (uint8_t)0;
+  m.func_middle = WIDTH == 7 ? (uint8_t)fm : (uint8_t)0;
+  m.func_inner = (uint8_t)inner;
+  m.inner_seen = (uint8_t)seen;
+  m.width = (uint8_t)WIDTH;
+#pragma unroll
+  for (int i = 0; i < 5; i++) m.pad[i] = 0;
+  *dst = m;
+}
+
+// A 5- or 7-LUT match's record: gates in reference order (tuple positions of ordering row k),
+// func_inner = solved bits only and inner_seen = cells with a masked position (sbg_solve_inner's
+// closed form, on the compressed tables; a match has no conflicting cell).
 template <int NW, int WIDTH>
 __device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned long long key,
     const int *tuple, int k, uint32_t fo, uint32_t fm, const uint32_t *s_tabs, int npad,
@@ -2636,33 +2716,18 @@ __device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned
       if (in_cell) seen |= 1u << c;
     }
   }
-  DevMatch m;
-  m.key = key;
-#pragma unroll
-  for (int i = 0; i < 7; i++) m.gates[i] = i < WIDTH ? (uint16_t)G[i] : (uint16_t)0;
-  m.func_outer = (uint8_t)fo;
-  m.func_middle = WIDTH == 7 ? (uint8_t)fm : (uint8_t)0;
-  m.func_inner = (uint8_t)ones;
-  m.inner_seen = (uint8_t)seen;
-  m.width = (uint8_t)WIDTH;
-#pragma unroll
-  for (int i = 0; i < 5; i++) m.pad[i] = 0;
-  *dst = m;
+  store_match<WIDTH>(dst, key, G, fo, fm, ones, seen);
 }
 
 // The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
 // 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
-// feasible tuple and ordering the set of working outer functions from outer_ok5.  Pick: j runs over
-// sel.tickets instead.
+// feasible tuple and ordering the set of working outer functions from outer_ok5.
 template <int NW, int MODE>
 __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts, const DevTables *__restrict__ tab) {
-  constexpr bool EMIT = MODE != kEnumCount;
-  EnumSel sel = {};
-  if (MODE == kEnumRange || MODE == kEnumPick) sel = ectl->sel;
   constexpr int P = 3, K = 5, NC = 1 << P;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[256];
@@ -2683,26 +2748,10 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
   }
   const uint32_t inmask = prob->inmask;
   const uint64_t total = c_binom[n - 2][P];
-  const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
-  unsigned long long feasible_local = 0, matches_local = 0;
 
-  for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
-       j < t_end; j += nwarps) {
-    const unsigned long long t = MODE == kEnumPick ? sel.tickets[j] : j;
-    unsigned long long base = 0;
-    unsigned int req = 0, req_end = 0;
-    if (EMIT) {
-      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
-      if (MODE == kEnumRange && offsets[t] + counts[t] <= sel.lo) continue;
-      if (MODE == kEnumPick) {
-        req = sel.first[j];
-        req_end = sel.first[j + 1];
-      }
-      base = offsets[t];
-    }
-    // prefixes are dealt to the parts in blocks of kDeal, as k_sweep deals them
-    const uint64_t dealt = (t / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal + t % kDeal;
-    uint32_t count = 0;
+  enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
+      [&](unsigned long long t, EnumTicket &tk, unsigned long long &feasible) {
+    const uint64_t dealt = dealt_item(t, part, nparts);   // as k_sweep deals its prefixes
     if (dealt < total) {
       int pre[P];
       uint64_t base_rank;
@@ -2763,7 +2812,7 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
           const int src = __ffs(fb) - 1;
           int g5[5] = {pre[0], pre[1], pre[2], __shfl_sync(kFull, gf, src),
                        __shfl_sync(kFull, gg, src)};
-          feasible_local++;
+          feasible++;
           uint32_t H1, H0;
           summary5<NW>(s_tabs, npad, g5, T, M, lane, H1, H0);
           for (int k = 0; k < 10 && !done; k++) {
@@ -2776,8 +2825,8 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
               c += __popc(surv);
               if (lane == hi) surv_mine = surv;
             }
-            if (!EMIT) {
-              count += c;
+            if (MODE == kEnumCount) {
+              tk.count += c;
               continue;
             }
             if (c == 0) continue;
@@ -2788,28 +2837,15 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
               const uint32_t pos = 32u * w + lane;
               const uint32_t fo = s_ord[pos];
               const bool hit = (__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u;
-              const uint32_t bal = __ballot_sync(kFull, hit);
-              const unsigned long long at = base + count + __popc(bal & lanemask_lt());
-              emit_step<MODE>(hit, at, base + count + __popc(bal), max_out, sel, req, req_end,
-                  [&](unsigned long long i) {
-                    write_match<NW, 5>(out + i, key_hi | pos, g5, k, fo, 0, s_tabs, npad, T, M);
-                  });
-              count += __popc(bal);
+              done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
+                write_match<NW, 5>(out + i, key_hi | pos, g5, k, fo, 0, s_tabs, npad, T, M);
+              });
             }
-            done = MODE == kEnumPick ? req >= req_end : base + count >= max_out;
           }
         }
       }
     }
-    if (!EMIT) {
-      if (lane == 0) counts[t] = count;
-      matches_local += count;
-    }
-  }
-  if (!EMIT && lane == 0) {
-    if (matches_local != 0) atomicAdd(&ectl->total, matches_local);
-    if (feasible_local != 0) atomicAdd(&ectl->feasible, feasible_local);
-  }
+  });
 }
 
 // Middle functions of one cube set (see middle_cubes) as a 256-bit set over fm, word wd = fm >> 5.
@@ -2840,8 +2876,7 @@ __device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (
 // nparts + part), one warp per entry: the summary and stage-1 filter of k_decomp7 on the TRUE gate
 // tables (no stale outer cache), then per surviving outer function and ordering row the union of
 // the middle-function cubes.  Count: one lane per outer function; emit: positions in ascending
-// order, outer position in the loop, middle position across the lanes.  Pick: j runs over
-// sel.tickets instead.
+// order, outer position in the loop, middle position across the lanes.
 template <int NW, int MODE>
 __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
@@ -2850,8 +2885,6 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts, const DevTables *__restrict__ tab) {
   constexpr bool EMIT = MODE != kEnumCount;
-  EnumSel sel = {};
-  if (MODE == kEnumRange || MODE == kEnumPick) sel = ectl->sel;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
   __shared__ uint8_t s_fo[kWarpsPerCta][256];
@@ -2874,25 +2907,10 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
   }
   uint32_t *sH = s_H[warp];
   uint8_t *fo_list = s_fo[warp];
-  const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
-  unsigned long long matches_local = 0;
 
-  for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
-       j < t_end; j += nwarps) {
-    const unsigned long long t = MODE == kEnumPick ? sel.tickets[j] : j;
+  enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
+      [&](unsigned long long t, EnumTicket &tk, unsigned long long &) {
     const uint64_t idx = t * (uint64_t)nparts + (uint64_t)part;
-    unsigned long long base = 0;
-    unsigned int req = 0, req_end = 0;
-    if (EMIT) {
-      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
-      if (MODE == kEnumRange && offsets[t] + counts[t] <= sel.lo) continue;
-      if (MODE == kEnumPick) {
-        req = sel.first[j];
-        req_end = sel.first[j + 1];
-      }
-      base = offsets[t];
-    }
-    uint32_t count = 0;
     if (idx < list_count) {
       const uint64_t cur = list[idx];
       int g[7];
@@ -2943,7 +2961,7 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
 #pragma unroll
               for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd]);
             }
-            count += __reduce_add_sync(kFull, have ? c : 0u);
+            tk.count += __reduce_add_sync(kFull, have ? c : 0u);
           }
         }
 #pragma unroll 1
@@ -2975,25 +2993,15 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
                       && (fm & S) == (hv[0][c0] | hv[1][c1]);
                 }
               }
-              const uint32_t bal = __ballot_sync(kFull, hit);
-              const unsigned long long at = base + count + __popc(bal & lanemask_lt());
-              emit_step<MODE>(hit, at, base + count + __popc(bal), max_out, sel, req, req_end,
-                  [&](unsigned long long i) {
-                    write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
-                  });
-              count += __popc(bal);
+              done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
+                write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
+              });
             }
-            done = MODE == kEnumPick ? req >= req_end : base + count >= max_out;
           }
         }
       }
     }
-    if (!EMIT) {
-      if (lane == 0) counts[t] = count;
-      matches_local += count;
-    }
-  }
-  if (!EMIT && lane == 0 && matches_local != 0) atomicAdd(&ectl->total, matches_local);
+  });
 }
 
 
@@ -3009,20 +3017,16 @@ struct EnumGateOrder {
 // of the target (scan3_blocks' test, here on the compressed tables).  Key i << 18 | k << 9 | m, so a
 // ticket's matches are consecutive keys in the order of its lanes.  A match's record: the gates in
 // position order, func_inner = cells holding a masked 1, inner_seen = cells holding a masked
-// position (sbg_solve_inner's closed form).  Pick: j runs over sel.tickets instead.
+// position (sbg_solve_inner's closed form).
 template <int NW, int MODE>
 __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts) {
-  constexpr bool EMIT = MODE != kEnumCount;
-  EnumSel sel = {};
-  if (MODE == kEnumRange || MODE == kEnumPick) sel = ectl->sel;
   extern __shared__ uint32_t smem[];
   __shared__ uint16_t s_order[kMaxGatesPad];
   const int lane = threadIdx.x & 31;
-  const int warp = threadIdx.x >> 5;
   const int n = prob->n;
   const int npad = (n + 3) & ~3;
   uint32_t *s_tabs = smem;
@@ -3036,25 +3040,10 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
     Z[w] = prob->M[w] & ~prob->T[w];
   }
   const uint64_t pairs = (uint64_t)(n * (n - 1) / 2);
-  const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
-  unsigned long long matches_local = 0;
 
-  for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta + warp;
-       j < t_end; j += nwarps) {
-    const unsigned long long t = MODE == kEnumPick ? sel.tickets[j] : j;
-    unsigned long long base = 0;
-    unsigned int req = 0, req_end = 0;
-    if (EMIT) {
-      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
-      if (MODE == kEnumRange && offsets[t] + counts[t] <= sel.lo) continue;
-      if (MODE == kEnumPick) {
-        req = sel.first[j];
-        req_end = sel.first[j + 1];
-      }
-      base = offsets[t];
-    }
-    const uint64_t dealt = (t / kDeal) * kDeal * (uint64_t)nparts + (uint64_t)part * kDeal + t % kDeal;
-    uint32_t count = 0;
+  enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
+      [&](unsigned long long t, EnumTicket &tk, unsigned long long &) {
+    const uint64_t dealt = dealt_item(t, part, nparts);
     if (dealt < pairs) {
       int pi, pk;
       unrank_pair((uint32_t)dealt, n, pi, pk);
@@ -3085,42 +3074,14 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
           if (one[c] != 0) ones |= 1u << c;
           if ((one[c] | zero[c]) != 0) seen |= 1u << c;
         }
-        const uint32_t bal = __ballot_sync(kFull, ok);
-        if (EMIT) {
-          const unsigned long long at = base + count + __popc(bal & lanemask_lt());
-          emit_step<MODE>(ok, at, base + count + __popc(bal), max_out, sel, req, req_end,
-              [&](unsigned long long dst) {
-                DevMatch m;
-                m.key = ((unsigned long long)pi << 18) | ((unsigned long long)pk << 9) | (unsigned)pm;
-                m.gates[0] = s_order[pi];
-                m.gates[1] = s_order[pk];
-                m.gates[2] = s_order[pm];
-#pragma unroll
-                for (int i = 3; i < 7; i++) m.gates[i] = 0;
-                m.func_outer = 0;
-                m.func_middle = 0;
-                m.func_inner = (uint8_t)ones;
-                m.inner_seen = (uint8_t)seen;
-                m.width = 3;
-#pragma unroll
-                for (int i = 0; i < 5; i++) m.pad[i] = 0;
-                out[dst] = m;
-              });
-        }
-        count += __popc(bal);
-        done = EMIT && (MODE == kEnumPick ? req >= req_end : base + count >= max_out);
+        done = emit_step<MODE>(ok, tk, [&](unsigned long long i) {
+          const int G[3] = {s_order[pi], s_order[pk], s_order[pm]};
+          store_match<3>(out + i, ((unsigned long long)pi << 18) | ((unsigned long long)pk << 9)
+              | (unsigned)pm, G, 0, 0, ones, seen);
+        });
       }
     }
-    if (!EMIT) {
-      if (lane == 0) counts[t] = count;
-      matches_local += count;
-    }
-  }
-  // every feasible triple is a match: the two sums are the same number
-  if (!EMIT && lane == 0 && matches_local != 0) {
-    atomicAdd(&ectl->total, matches_local);
-    atomicAdd(&ectl->feasible, matches_local);
-  }
+  });
 }
 
 
@@ -3172,20 +3133,43 @@ __global__ void __launch_bounds__(256) k_enum_block_sums(const uint32_t *__restr
   }
 }
 
+// One tile of an exclusive prefix sum over the CTA's threads (blockDim.x a multiple of 32, at most
+// 1,024), one value c per thread, every thread taking part: returns carry plus the sum of the tile's
+// values in front of this thread's, and advances carry by the tile's sum.
+__device__ __forceinline__ unsigned long long tile_scan(unsigned long long c,
+    unsigned long long &carry) {
+  __shared__ unsigned long long s_warp[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long incl = c;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const unsigned long long up = __shfl_up_sync(kFull, incl, d);
+    if (lane >= d) incl += up;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  unsigned long long before = 0;
+  for (int i = 0; i < warp; i++) before += s_warp[i];
+  unsigned long long tile = 0;
+  for (int i = 0; i < (int)(blockDim.x >> 5); i++) tile += s_warp[i];
+  __syncthreads();   // s_warp is free for the next tile
+  const unsigned long long excl = carry + before + incl - c;
+  carry += tile;
+  return excl;
+}
+
 // Exclusive prefix sum over the whole's deal blocks g = 0 .. nblocks-1, block g being part
 // q = g % nparts's local block g / nparts with sums[q * stride + g / nparts] matches.  For this
 // share's blocks (q == part): delta[j] = (global start of block j) - offsets[j * B], the amount
 // k_enum_rebase adds to the block's local offsets; ectl->gbad = 1 if the share's row of sums differs
 // from its own block sums `own` (a gather in the wrong part order), ectl->gtotal = the whole's total.
-// One CTA of 1,024 threads, a tile of 1,024 blocks at a time, as k_enum_scan.
+// One CTA of 1,024 threads, a tile of 1,024 blocks at a time.
 __global__ void __launch_bounds__(1024) k_enum_globalize(EnumCtl *__restrict__ ectl,
     const unsigned long long *__restrict__ sums, unsigned long long stride,
     unsigned long long nblocks, int part, int nparts, const unsigned long long *__restrict__ own,
     const unsigned long long *__restrict__ offsets, unsigned int B,
     unsigned long long *__restrict__ delta) {
-  __shared__ unsigned long long s_warp[32];
   __shared__ unsigned int s_bad;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (threadIdx.x == 0) s_bad = 0;
   unsigned long long carry = 0;
   for (unsigned long long g0 = 0; g0 < nblocks; g0 += blockDim.x) {
@@ -3193,25 +3177,13 @@ __global__ void __launch_bounds__(1024) k_enum_globalize(EnumCtl *__restrict__ e
     const unsigned long long j = g / (unsigned long long)nparts;
     const int q = (int)(g % (unsigned long long)nparts);
     const unsigned long long c = g < nblocks ? sums[(unsigned long long)q * stride + j] : 0ull;
-    unsigned long long incl = c;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const unsigned long long up = __shfl_up_sync(kFull, incl, d);
-      if (lane >= d) incl += up;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    unsigned long long before = 0;
-    for (int i = 0; i < warp; i++) before += s_warp[i];
-    unsigned long long tile = 0;
-    for (int i = 0; i < (int)(blockDim.x >> 5); i++) tile += s_warp[i];
+    const unsigned long long start = tile_scan(c, carry);
     if (g < nblocks && q == part) {
-      delta[j] = carry + before + incl - c - offsets[j * B];
+      delta[j] = start - offsets[j * B];
       if (c != own[j]) s_bad = 1;
     }
-    carry += tile;
-    __syncthreads();
   }
+  __syncthreads();
   if (threadIdx.x == 0) {
     ectl->gtotal = carry;
     ectl->gbad = s_bad;
@@ -3234,27 +3206,11 @@ __global__ void __launch_bounds__(256) k_enum_rebase(unsigned long long *__restr
 __global__ void __launch_bounds__(1024) k_enum_scan(EnumCtl *__restrict__ ectl,
     const uint32_t *__restrict__ counts, unsigned long long *__restrict__ offsets,
     unsigned long long t_begin, unsigned long long t_end) {
-  __shared__ unsigned long long s_warp[32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   unsigned long long carry = ectl->carry;
   for (unsigned long long t0 = t_begin; t0 < t_end; t0 += blockDim.x) {
     const unsigned long long t = t0 + threadIdx.x;
-    const unsigned long long c = t < t_end ? counts[t] : 0ull;
-    unsigned long long incl = c;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const unsigned long long up = __shfl_up_sync(kFull, incl, d);
-      if (lane >= d) incl += up;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    unsigned long long before = 0;
-    for (int i = 0; i < warp; i++) before += s_warp[i];
-    unsigned long long tile = 0;
-    for (int i = 0; i < (int)(blockDim.x >> 5); i++) tile += s_warp[i];
-    if (t < t_end) offsets[t] = carry + before + incl - c;
-    carry += tile;
-    __syncthreads();
+    const unsigned long long start = tile_scan(t < t_end ? counts[t] : 0ull, carry);
+    if (t < t_end) offsets[t] = start;
   }
   if (threadIdx.x == 0) ectl->carry = carry;
 }

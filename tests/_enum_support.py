@@ -48,6 +48,9 @@ def enum_oracle():
     lib.orc_check7_list.argtypes = [u64p, u64p, u64p, u16p, C.c_int64, C.POINTER(C.c_int64)]
     lib.orc_scan3_key.restype = C.c_uint64
     lib.orc_scan3_key.argtypes = [u64p, C.c_int, u64p, u64p, u16p, C.c_int64, C.c_int64]
+    lib.orc_enum3_range.restype = C.c_uint64
+    lib.orc_enum3_range.argtypes = [u64p, C.c_int, u64p, u64p, u16p, C.c_int64, C.c_int64,
+                                    C.c_uint64, u64p]
     _lib = lib
     return lib
 
@@ -162,6 +165,29 @@ def scan3_key(tables, target, mask, order, lo=0, hi=None, piece=None):
                                                              go.ctypes.data_as(u16p), r[0], r[1])),
                              rs))
     return min(keys) if keys else NONE
+
+
+def enum3_range(tables, target, mask, order, max_keys, lo=0, hi=None, piece=None):
+    """(total, first max_keys keys) of the 3-LUT scan's matches among the position triples of ranks
+    [lo, hi) (default: all of C(n,3)): orc_enum3_range over pieces, totals summed, key lists
+    concatenated.  Every match is a feasible triple, so the total is also the feasible count."""
+    lib = enum_oracle()
+    _keep, args = _problem(tables, target, mask, [])
+    n = args[1]
+    go = np.ascontiguousarray(order, dtype=np.uint16)
+    if hi is None:
+        hi = n * (n - 1) * (n - 2) // 6
+
+    def run(r):
+        keys = np.zeros(max(max_keys, 1), dtype=np.uint64)
+        total = lib.orc_enum3_range(args[0], n, args[2], args[3], go.ctypes.data_as(u16p), r[0],
+                                    r[1], max_keys, keys.ctypes.data_as(u64p))
+        return int(total), [int(k) for k in keys[:min(total, max_keys)]]
+    rs = pieces(lo, hi, piece or max(1, -(-(hi - lo) // (4 * workers()))))
+    with ThreadPoolExecutor(max_workers=workers()) as pool:
+        parts = list(pool.map(run, rs))
+    keys = [k for p in parts for k in p[1]][:max_keys]
+    return sum(p[0] for p in parts), keys
 
 
 def comb_rank(n, t, comb):

@@ -1,7 +1,8 @@
 /* tests/enum_oracle.c -- TEST INFRASTRUCTURE, not product code.
  *
- * CPU enumeration of every match of search_5lut / search_7lut, the checker of sbg_enum5 /
- * sbg_enum7.  The loops are those of orc_search5_key / orc_decomp7_key (oracle/sbg_oracle.c)
+ * CPU enumeration of every match of search_5lut / search_7lut / lut_search's 3-LUT scan, the
+ * checker of sbg_enum5 / sbg_enum7 / sbg_enum3.  The loops are those of orc_search5_key /
+ * orc_decomp7_key (oracle/sbg_oracle.c) and orc_scan3_key (below)
  * without the early exit: every candidate is decided, the matches are counted, and the first
  * max_keys keys (the loops run in ascending key order) are written out.  The 7-LUT candidates are
  * decided on the true gate tables (no stale outer cache).  Built together with oracle/sbg_oracle.c
@@ -9,7 +10,8 @@
  *
  * The *_range forms walk one range [lo, hi) of lexicographic combination ranks, so that a large
  * space can be cut into pieces and checked on several threads: the phase-1 list of search_7lut,
- * search_5lut's first-match key, its enumeration, and the 3-LUT scan of lut_search.
+ * search_5lut's first-match key, its enumeration, and the 3-LUT scan of lut_search and its
+ * enumeration.
  */
 #include <stdlib.h>
 #include <string.h>
@@ -143,6 +145,25 @@ uint64_t orc_scan3_key(const uint64_t *tables, int n, const uint64_t *target, co
     }
   }
   return UINT64_MAX;
+}
+
+/* orc_scan3_key without the early exit, the checker of sbg_enum3: every position triple of ranks
+   [lo, hi) whose gates pass check_n_lut_possible(3, ...) under the mask is a match
+   (get_lut_function cannot fail then).  Returns the number of matches and writes the first
+   max_keys keys i<<18 | k<<9 | m. */
+uint64_t orc_enum3_range(const uint64_t *tables, int n, const uint64_t *target,
+    const uint64_t *mask, const uint16_t *order, int64_t lo, int64_t hi, uint64_t max_keys,
+    uint64_t *keys) {
+  uint16_t pos[3];
+  uint64_t total = 0;
+  for (int64_t r = range_start(n, 3, lo, &hi, pos); r < hi; r++, orc_next_combination(pos, 3, n)) {
+    uint64_t tt[3 * 4];
+    for (int m = 0; m < 3; m++) memcpy(tt + 4 * m, tables + 4 * order[pos[m]], 32);
+    if (orc_check_n_lut_possible(3, target, mask, tt)) {
+      note((uint64_t)pos[0] << 18 | (uint64_t)pos[1] << 9 | pos[2], &total, keys, max_keys);
+    }
+  }
+  return total;
 }
 
 /* lut.c:416-484 over the list (count entries of 7 gates each): returns the number of matches. */

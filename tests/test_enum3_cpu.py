@@ -6,7 +6,6 @@ import itertools
 import numpy as np
 import pytest
 
-import _enum3_support as E3
 import _enum_support as E
 import _support as S
 import sboxgates_b200 as sb
@@ -79,7 +78,7 @@ def test_enum3_range_first_key_is_scan3_key():
         n = len(tabs)
         for size in _cuts(n * (n - 1) * (n - 2) // 6, rs):
             want = E.scan3_key(tabs, tgt, mask, order, piece=size)
-            total, keys = E3.enum3_range(tabs, tgt, mask, order, 3, piece=size)
+            total, keys = E.enum3_range(tabs, tgt, mask, order, 3, piece=size)
             assert (keys[0] if keys else NONE) == want, (i, size)
             assert len(keys) == min(total, 3) and keys == sorted(set(keys)), (i, size)
         hits += total > 0
@@ -94,13 +93,13 @@ def test_enum3_range_totals_are_a_plain_count():
         want = _numpy_keys(tabs, tgt, mask, order)
         all_triples = n * (n - 1) * (n - 2) // 6
         for size in _cuts(all_triples, rs):
-            total, keys = E3.enum3_range(tabs, tgt, mask, order, len(want) + 1, piece=size)
+            total, keys = E.enum3_range(tabs, tgt, mask, order, len(want) + 1, piece=size)
             assert total == len(want) and keys == want, (i, size, total, len(want))
         # a slice of ranks holds the matches whose triples have those ranks
         lo, hi = sorted(int(x) for x in rs.randint(0, all_triples + 1, 2))
         ranks = {k: E.comb_rank(n, 3, [k >> 18, (k >> 9) & 0x1FF, k & 0x1FF]) for k in want}
         sub = [k for k in want if lo <= ranks[k] < hi]
-        assert E3.enum3_range(tabs, tgt, mask, order, len(sub) + 1, lo, hi) == (len(sub), sub), i
+        assert E.enum3_range(tabs, tgt, mask, order, len(sub) + 1, lo, hi) == (len(sub), sub), i
         if not int(np.bitwise_or.reduce(mask)):
             assert len(want) == all_triples   # no masked position: every triple realises the target
             zero_mask += 1

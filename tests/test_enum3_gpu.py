@@ -1,5 +1,5 @@
 """GPU: sbg_enum3 (every match of lut_search's 3-LUT scan) against the CPU oracle's
-orc_enum3_range (tests/enum3_oracle.c, checked against a plain count by test_enum3_cpu.py), against
+orc_enum3_range (tests/enum_oracle.c, checked against a plain count by test_enum3_cpu.py), against
 the scan of sbg_search_node, across shards and count-free windows, next to the 7-LUT calls on one
 slot, and enumerate_lut_search against lut_search."""
 import os
@@ -8,7 +8,6 @@ import re
 import numpy as np
 import pytest
 
-import _enum3_support as E3
 import _enum_support as E
 import _support as S
 import sboxgates_b200 as sb
@@ -89,7 +88,7 @@ def test_enum3_matches_oracle(engine):
     matched = 0
     for i, (tabs, tgt, mask, order) in enumerate(_states()):
         n = len(tabs)
-        total, keys = E3.enum3_range(tabs, tgt, mask, order, K)
+        total, keys = E.enum3_range(tabs, tgt, mask, order, K)
         if _positions(mask) == 0:
             assert total == n * (n - 1) * (n - 2) // 6, i
         e = sb.enumerate_3lut(engine, tabs, tgt, mask, [0], order, K)
@@ -120,7 +119,7 @@ def test_enum3_at_large_n(engine):
         order = [int(x) for x in rs.permutation(n - 3)] + [int(x) for x in rs.permutation(3) + n - 3]
         planted = S.lut_table(0x6B ^ i, tabs[n - 3], tabs[n - 2], tabs[n - 1])
         for tgt in (planted, S.sbox_target(S.rijndael_sbox(), i % 8)):
-            total, keys = E3.enum3_range(tabs, tgt, mask, order, K)
+            total, keys = E.enum3_range(tabs, tgt, mask, order, K)
             e = sb.enumerate_3lut(engine, tabs, tgt, mask, [], order, K)
             assert (e.total, e.feasible) == (total, total) and _keys(e) == keys, (n, spec)
             _check_records(e, tabs, tgt, mask, order)
@@ -215,7 +214,7 @@ def test_count_free_windows(engine):
     assert 0 < total <= 10**6
     every = engine.enumerate3(order, total)
     assert every.total == total and len(every.matches) == total
-    want_total, want_keys = E3.enum3_range(tabs, tgt, mask, order, 3000)
+    want_total, want_keys = E.enum3_range(tabs, tgt, mask, order, 3000)
     assert total == want_total and _keys(every)[:3000] == want_keys
     tickets = np.array([_pair_ticket(n, k) for k in _keys(every)])
     assert np.all(np.diff(tickets) >= 0)

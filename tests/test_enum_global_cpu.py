@@ -14,7 +14,6 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-import _enum3_support as E3
 import _enum_support as E
 import _support as S
 import sboxgates_b200 as sb
@@ -60,7 +59,7 @@ class GlobalOracleEngine(OracleEngine):
         return sb.Enumeration(len(self.share), feasible if part == 0 else 0, self.share[:k].copy())
 
     def enumerate3(self, order, k, count=True, part=0, nparts=1):
-        _, keys = E3.enum3_range(self.tables, self.target, self.mask, order, 1 << 20)
+        _, keys = E.enum3_range(self.tables, self.target, self.mask, order, 1 << 20)
         return self._enum(3, keys, len(keys), k, part, nparts)
 
     def enumerate5(self, order, k, count=True, part=0, nparts=1):
@@ -169,7 +168,7 @@ def _expected():
         tabs, tgt, mask, inb = _state(width, 30 + width)
         orders = _orders(40 + width, len(tabs))
         if width == 3:
-            _, keys = E3.enum3_range(tabs, tgt, mask, orders[0], 1 << 20)
+            _, keys = E.enum3_range(tabs, tgt, mask, orders[0], 1 << 20)
             feas = len(keys)
         elif width == 5:
             _, keys, feas = E.oracle_enum5(tabs, tgt, mask, inb, orders[1], 1 << 20)
