@@ -274,8 +274,9 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
        sbg_set_list7, sbg_list7_device, sbg_set_list7_device, sbg_allgather_merge7 (every handle
        given), sbg_decomp7_part, sbg_finish7 or sbg_alu_peak ends it, whatever the call returns;
      - sbg_last_error, sbg_launch_count, sbg_transfer_stats, sbg_host_seconds, sbg_last_kernel_ms,
-       sbg_set_timing, sbg_set_stream, sbg_enum_fetch, sbg_enum_pick, sbg_enum_block_sums and
-       sbg_enum_set_global keep it.
+       sbg_set_timing, sbg_set_stream, sbg_enum_fetch, sbg_enum_pick, sbg_enum_block_sums,
+       sbg_enum_set_global and sbg_enum_depth_counts keep it;
+     - sbg_enum_set_depth ends it, whatever the call returns.
    Without a cursor both calls return SBG_ERR_STATE.
    A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
    a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT) or a list
@@ -319,6 +320,36 @@ int sbg_enum_block_sums(sbg_handle *h, uint64_t *out, uint64_t *nblocks);
    global.  nparts == 1 is allowed and changes nothing observable. */
 int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
     const uint64_t *counts, int nparts, uint64_t *total);
+
+/* ---- depth filter: the realisations at or below a circuit depth ------------------------------ */
+/* The caller gives a depth for every gate of the problem, D[g] for g < n (any values up to
+   SBG_MAX_DEPTH; they need not come from a real graph, and a large D[g] excludes gate g), and a
+   bound max_depth.  A match's depth is that of the output gate it would add, from its record's
+   gates in reference order:
+     3-LUT a,b,c:     1 + max(Da, Db, Dc);
+     5-LUT a..e:      1 + max(1 + max(Da, Db, Dc), Dd, De)            (outer LUT over a,b,c);
+     7-LUT a..g:      1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df), Dg).
+   Under a filter the matches of sbg_enum3 / sbg_enum5 / sbg_enum7 are exactly the unfiltered
+   matches of depth <= max_depth: keys, key order and records are unchanged, only the set shrinks,
+   and ranks are ranks within it.  The 7-LUT list is still the phase-1 list (the first
+   SBG_LIST_CAP feasible 7-combinations whatever their depths).  *feasible of sbg_enum5 then counts
+   the feasible combinations with an ordering within the bound (sbg_enum3: the matches counted,
+   sbg_enum7: the list length, as without a filter).  The cursor keeps the filter it was counted
+   under, so fetch, pick, sbg_enum_block_sums and sbg_enum_set_global serve the filtered set.
+   Searches (sbg_search*, sbg_search_node / batch, the *_part and finish calls) never read it. */
+#define SBG_MAX_DEPTH 1020     /* largest gate depth of a filter */
+#define SBG_DEPTH_BINS 1024    /* bins of the depth histogram (a match is at most 1,022 deep) */
+/* Installs the filter (n depths, host memory) for the later sbg_enum3 / sbg_enum5 / sbg_enum7
+   calls on the handle; depth == NULL clears it.  SBG_ERR_ARG, with the filter left as it was: n
+   outside 1..SBG_MAX_GATES or a depth above SBG_MAX_DEPTH.  An sbg_enum* call whose problem does
+   not have n gates returns SBG_ERR_ARG.  The call ends the cursor. */
+int sbg_enum_set_depth(sbg_handle *h, const uint16_t *depth, int n, uint32_t max_depth);
+/* out[d] = the number of the cursor's counted matches of depth d, d < nbins <= SBG_DEPTH_BINS
+   (deeper bins are not reported).  Per share, as totals are: the shares' arrays add up to the
+   whole's.  The minimum depth: count with max_depth = SBG_DEPTH_BINS - 1, take the first non-empty
+   bin, count again with that bound.  SBG_ERR_STATE without a cursor or when it was counted without
+   a filter; SBG_ERR_ARG for nbins > SBG_DEPTH_BINS.  Keeps the cursor. */
+int sbg_enum_depth_counts(sbg_handle *h, uint64_t *out, uint32_t nbins);
 
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense

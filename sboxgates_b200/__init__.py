@@ -11,14 +11,15 @@ from .rng import Xorshift1024
 from .lut import LutEngine, SearchResult, NO_GATE, search_5lut, search_7lut, shuffled_order, \
     shuffled_orders7, ordering_row, solve_inner, lut_table, lut_search, LutSearchResult, \
     Enumeration, enumerate_3lut, enumerate_5lut, enumerate_7lut, enumerate_lut_search, \
-    match_to_ret, match_to_lut3, decode_key3, decode_key5, decode_key7, sample_matches
-from .native import load_library, NativeLibraryError, MATCH_DTYPE
+    match_to_ret, match_to_lut3, decode_key3, decode_key5, decode_key7, sample_matches, \
+    match_depth, shallowest_matches
+from .native import load_library, NativeLibraryError, MATCH_DTYPE, SBG_MAX_DEPTH, SBG_DEPTH_BINS
 
 __all__ = [
     "Xorshift1024", "LutEngine", "SearchResult", "NO_GATE", "search_5lut", "search_7lut",
     "shuffled_order", "shuffled_orders7", "ordering_row", "solve_inner", "lut_table",
     "lut_search", "LutSearchResult", "Enumeration", "enumerate_3lut", "enumerate_5lut",
     "enumerate_7lut", "enumerate_lut_search", "match_to_ret", "match_to_lut3", "decode_key3",
-    "decode_key5", "decode_key7", "sample_matches", "MATCH_DTYPE",
-    "load_library", "NativeLibraryError",
+    "decode_key5", "decode_key7", "sample_matches", "match_depth", "shallowest_matches",
+    "MATCH_DTYPE", "SBG_MAX_DEPTH", "SBG_DEPTH_BINS", "load_library", "NativeLibraryError",
 ]

@@ -143,7 +143,8 @@ struct sbg_lane {
   uint32_t *d_ecount = nullptr;             // matches per ticket
   unsigned long long *d_eoffset = nullptr;  // their exclusive prefix sum
   DevMatch *d_ematch = nullptr;             // the emitted records
-  uint64_t ecount_cap = 0, eoffset_cap = 0, ematch_cap = 0;
+  unsigned long long *d_ehist = nullptr;    // filtered count: matches per depth (kDepthBins)
+  uint64_t ecount_cap = 0, eoffset_cap = 0, ematch_cap = 0, ehist_cap = 0;
   // fetch and pick on an enumeration cursor (allocated on the first call)
   unsigned long long *d_pranks = nullptr;   // requested ranks, ascending
   unsigned int *d_pslots = nullptr;         // their output slots
@@ -158,10 +159,21 @@ struct sbg_lane {
 };
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
-// (widths 5 and 7) or the gate order (width 3).
+// (widths 5 and 7) or the gate order (width 3), and the depth filter if one was installed
+// (sbg_enum_set_depth; its histogram pointer is the lane's, set at launch).
 struct EnumInputs {
   EnumOrders ord;
   EnumGateOrder gates;
+  bool filtered;
+  EnumDepth<true> depth;
+};
+
+// The depth filter of a handle (sbg_enum_set_depth): the depths of n gates and the bound.
+struct DepthFilter {
+  bool on = false;
+  int n = 0;
+  uint32_t max_depth = 0;
+  uint16_t depth[SBG_MAX_GATES] = {};
 };
 
 // The enumeration cursor: what sbg_enum_fetch / sbg_enum_pick need of the last counted enumeration
@@ -250,6 +262,7 @@ struct sbg_handle {
   // enumeration buffers; the enumeration cursor lives as long as it does not change
   uint64_t api_seq = 0;
   EnumCursor cursor;
+  DepthFilter filter;   // read by sbg_enum3 / sbg_enum5 / sbg_enum7 only
 };
 
 namespace {
@@ -1371,6 +1384,8 @@ int finish7_slot(sbg_handle *h, const sbg_handle::HostProblem &hp, uint64_t key,
 
 // ---- enumeration (sbg_enum3 / sbg_enum5 / sbg_enum7) -------------------------------------------
 
+static_assert(kDepthBins == SBG_DEPTH_BINS && SBG_MAX_DEPTH + 2 < SBG_DEPTH_BINS,
+    "every match depth has a histogram bin");
 static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
     && offsetof(sbg_match, gates) == offsetof(DevMatch, gates)
     && offsetof(sbg_match, func_outer) == offsetof(DevMatch, func_outer)
@@ -1426,16 +1441,25 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
       if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "enumeration launch: %s", cudaGetErrorString(e));
       return SBG_OK;
     };
-    if constexpr (WIDTH == 3) {
-      return run(k_enum3<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates, L.d_ecount,
-          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts);
-    } else if constexpr (WIDTH == 5) {
-      return run(k_enum5<NW, MODE>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
-          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab);
-    } else {
-      return run(k_enum7<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
-          L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab);
-    }
+    // the unfiltered or the filtered form (DF) of the width's kernel
+    auto run_form = [&](auto df_c, const EnumDepth<decltype(df_c)::value> &dep) {
+      constexpr bool DF = decltype(df_c)::value;
+      if constexpr (WIDTH == 3) {
+        return run(k_enum3<NW, MODE, DF>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates, L.d_ecount,
+            L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, dep);
+      } else if constexpr (WIDTH == 5) {
+        return run(k_enum5<NW, MODE, DF>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
+            L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, dep);
+      } else {
+        return run(k_enum7<NW, MODE, DF>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
+            L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts,
+            h->d_tab, dep);
+      }
+    };
+    if (!in.filtered) return run_form(std::false_type(), EnumDepth<false>());
+    EnumDepth<true> dep = in.depth;
+    dep.hist = L.d_ehist;
+    return run_form(std::true_type(), dep);
   });
   if (rc != SBG_OK) return rc;
   if (MODE == kEnumCount) {
@@ -1488,6 +1512,10 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   if ((rc = grow(h, L, L.d_ecount, L.ecount_cap, room)) != SBG_OK) return rc;
   if ((rc = grow(h, L, L.d_eoffset, L.eoffset_cap, room)) != SBG_OK) return rc;
   SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
+  if (in.filtered) {
+    if ((rc = grow(h, L, L.d_ehist, L.ehist_cap, (uint64_t)kDepthBins)) != SBG_OK) return rc;
+    SBG_CUDA(h, cudaMemsetAsync(L.d_ehist, 0, kDepthBins * sizeof(unsigned long long), L.stream));
+  }
   const bool count_all = total != nullptr;
   uint64_t window = count_all ? tickets
       : (WIDTH == 3 ? kEnumWindow3 : WIDTH == 5 ? kEnumWindow5 : kEnumWindow7);
@@ -1552,6 +1580,22 @@ int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, s
   }
   if (nparts < 1 || part < 0 || part >= nparts) return fail(h, SBG_ERR_ARG, "bad part %d/%d", part, nparts);
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
+  return SBG_OK;
+}
+
+// The handle's depth filter, if any, into the inputs of an sbg_enum* call on the current problem.
+int take_filter(sbg_handle *h, EnumInputs &in) {
+  const DepthFilter &f = h->filter;
+  in.filtered = f.on;
+  if (!f.on) return SBG_OK;
+  const int n = cur(h).n;
+  if (f.n != n) {
+    return fail(h, SBG_ERR_ARG, "the depth filter holds %d gates, the problem has %d", f.n, n);
+  }
+  memset(&in.depth, 0, sizeof(in.depth));
+  memcpy(in.depth.d, f.depth, sizeof(uint16_t) * (size_t)n);
+  // no match is deeper than kDepthBins - 2, so a larger bound filters nothing more
+  in.depth.max_depth = (int)std::min<uint32_t>(f.max_depth, kDepthBins - 1);
   return SBG_OK;
 }
 
@@ -1950,7 +1994,7 @@ void sbg_destroy(sbg_handle *h) {
       cudaFree(L.d_tcount); cudaFree(L.d_toffset); cudaFree(L.d_gcount);
       cudaFree(L.d_ectl); cudaFree(L.d_ecount); cudaFree(L.d_eoffset); cudaFree(L.d_ematch);
       cudaFree(L.d_pranks); cudaFree(L.d_pslots); cudaFree(L.d_ptickets); cudaFree(L.d_pfirst);
-      cudaFree(L.d_bsums); cudaFree(L.d_delta); cudaFree(L.d_gsums);
+      cudaFree(L.d_bsums); cudaFree(L.d_delta); cudaFree(L.d_gsums); cudaFree(L.d_ehist);
       if (L.h_out != nullptr) cudaFreeHost(L.h_out);
       if (L.h_ctl != nullptr) cudaFreeHost(L.h_ctl);
       for (int k = 0; k < 8; k++) if (L.ev[k] != nullptr) cudaEventDestroy(L.ev[k]);
@@ -2466,6 +2510,7 @@ int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, ui
   EnumInputs in5;
   memcpy(in5.ord.order[0], func_order, 256);
   memset(in5.ord.order[1], 0, 256);
+  if ((rc = take_filter(h, in5)) != SBG_OK) return rc;
   return run_enum<5>(h, kBeginSearch5, in, in5, part, nparts, max_matches, out, n_out, total,
       feasible);
 }
@@ -2482,6 +2527,7 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
   EnumInputs in7;
   memcpy(in7.ord.order[0], outer_order, 256);
   memcpy(in7.ord.order[1], middle_order, 256);
+  if ((rc = take_filter(h, in7)) != SBG_OK) return rc;
   // the installed list: only bring the problem block up to date
   return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
       total, feasible);
@@ -2505,6 +2551,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
   EnumInputs in3;
   memset(&in3, 0, sizeof(in3));
   memcpy(in3.gates.order, gate_order, sizeof(uint16_t) * (size_t)n);
+  if ((rc = take_filter(h, in3)) != SBG_OK) return rc;
   // only bring the problem block up to date: the control words of an installed 7-LUT list stay
   return run_enum<3>(h, kBeginKeepCtl, CallInputs(), in3, part, nparts, max_matches, out, n_out,
       total, feasible);
@@ -2713,6 +2760,46 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
   c.global = true;
   c.total = whole;
   *total = whole;
+  return SBG_OK;
+}
+
+int sbg_enum_set_depth(sbg_handle *h, const uint16_t *depth, int n, uint32_t max_depth) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
+  if (depth == nullptr) {
+    h->filter.on = false;
+    return SBG_OK;
+  }
+  if (n < 1 || n > SBG_MAX_GATES) return fail(h, SBG_ERR_ARG, "n = %d outside 1..%d", n, SBG_MAX_GATES);
+  for (int g = 0; g < n; g++) {
+    if (depth[g] > SBG_MAX_DEPTH) {
+      return fail(h, SBG_ERR_ARG, "depth[%d] = %u above %d", g, (unsigned)depth[g], SBG_MAX_DEPTH);
+    }
+  }
+  DepthFilter &f = h->filter;
+  memcpy(f.depth, depth, sizeof(uint16_t) * (size_t)n);
+  f.n = n;
+  f.max_depth = max_depth;
+  f.on = true;
+  return SBG_OK;
+}
+
+int sbg_enum_depth_counts(sbg_handle *h, uint64_t *out, uint32_t nbins) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  if (nbins > SBG_DEPTH_BINS) return fail(h, SBG_ERR_ARG, "nbins %u above %d", nbins, SBG_DEPTH_BINS);
+  if (out == nullptr && nbins > 0) return fail(h, SBG_ERR_ARG, "null output");
+  int rc;
+  if ((rc = check_cursor(h)) != SBG_OK) return rc;
+  if (!h->cursor.in.filtered) {
+    return fail(h, SBG_ERR_STATE, "the enumeration cursor was counted without a depth filter");
+  }
+  if (nbins == 0) return SBG_OK;
+  SBG_CUDA(h, cudaSetDevice(h->device));
+  sbg_lane &L = h->lane[0];
+  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ehist, nbins * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+      L.stream));
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  h->d2h_bytes += nbins * sizeof(uint64_t);
   return SBG_OK;
 }
 

@@ -2719,15 +2719,105 @@ __device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned
   store_match<WIDTH>(dst, key, G, fo, fm, ones, seen);
 }
 
+// ---- depth filter (sbg_enum_set_depth) -----------------------------------------------------------
+// The filtered forms of k_enum3/5/7 (template flag DF) keep only the matches whose depth is at most
+// max_depth.  A match's depth is that of the output gate it would add, from the caller's gate
+// depths D: 1 + max(Da, Db, Dc) (width 3), 1 + max(1 + max(Da, Db, Dc), Dd, De) (width 5),
+// 1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df), Dg) (width 7), gates in reference order.  It
+// depends on the ticket and the lane's third position (width 3) or the ordering row (widths 5 and
+// 7) only, so the count and emit passes apply the same test and a ticket emits what it counted.
+// Pruning: a gate with D >= max_depth occurs in no match, and the shallowest ordering of a 5-tuple
+// has depth max(2 + third deepest, 1 + deepest) (any 3 of the 5 may be the outer inputs), of a
+// 7-tuple max(2 + second deepest, 1 + deepest) (any of the 7 may be the last input); tickets and
+// (d,e) pairs none of whose orderings fit are dropped before their feasibility work.  The filtered
+// count pass fills a histogram of the matches by depth, per CTA in shared memory (one atomic per
+// (tuple, ordering), per (list entry, row, 32 outer functions), or per distinct depth of a 3-LUT
+// ballot), flushed to global memory once at the end.
+constexpr int kDepthBins = 1024;   // SBG_DEPTH_BINS: every depth (at most 1,022) has a bin
+
+template <bool DF> struct EnumDepth {};   // the unfiltered forms take no filter
+template <> struct EnumDepth<true> {
+  uint16_t d[kMaxGatesPad];     // depth of each gate of the problem
+  int max_depth;                // the bound, at most kDepthBins - 1
+  unsigned long long *hist;     // count pass: matches per depth, kDepthBins bins
+};
+
+__device__ __forceinline__ uint16_t *depth_smem() {
+  __shared__ uint16_t s_depth[kMaxGatesPad];
+  return s_depth;
+}
+
+__device__ __forceinline__ unsigned long long *hist_smem() {
+  __shared__ unsigned long long s_hist[kDepthBins];
+  return s_hist;
+}
+
+// The gate depths to shared memory (and a zero histogram for the count pass); the kernel's
+// __syncthreads after its own staging covers these stores.
+template <int MODE>
+__device__ __forceinline__ const uint16_t *stage_depth(const EnumDepth<true> &dep, int n) {
+  uint16_t *s = depth_smem();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) s[i] = dep.d[i];
+  if (MODE == kEnumCount) {
+    for (int i = threadIdx.x; i < kDepthBins; i += blockDim.x) hist_smem()[i] = 0;
+  }
+  return s;
+}
+
+template <bool DF>
+__device__ __forceinline__ int depth_bound(const EnumDepth<DF> &dep) {
+  if constexpr (DF) return dep.max_depth; else return 0;
+}
+
+// c more matches of depth d in the CTA's histogram.
+__device__ __forceinline__ void hist_add(int d, unsigned long long c) {
+  atomicAdd(hist_smem() + d, c);
+}
+
+// The end of a filtered count pass: the CTA's histogram into dep.hist.
+template <int MODE, bool DF>
+__device__ __forceinline__ void flush_hist(const EnumDepth<DF> &dep) {
+  if constexpr (DF && MODE == kEnumCount) {
+    __syncthreads();
+    const unsigned long long *s = hist_smem();
+    for (int i = threadIdx.x; i < kDepthBins; i += blockDim.x) {
+      if (s[i] != 0) atomicAdd(dep.hist + i, s[i]);
+    }
+  }
+}
+
+// Depth of a 5-LUT match of ordering row k, d5 = the depths of the tuple's gates in tuple order.
+__device__ __forceinline__ int depth5(const int *d5, int k) {
+  const uint32_t outer = (1u << c_rows5[k][0]) | (1u << c_rows5[k][1]) | (1u << c_rows5[k][2]);
+  int mo = 0, mi = 0;
+#pragma unroll
+  for (int i = 0; i < 5; i++) {
+    if ((outer >> i) & 1u) mo = max(mo, d5[i]); else mi = max(mi, d5[i]);
+  }
+  return max(2 + mo, 1 + mi);
+}
+
+// Depth of a 7-LUT match of ordering row k, d7 = the depths of the entry's gates in tuple order.
+__device__ __forceinline__ int depth7(const int *d7, int k) {
+  const int gs = c_rows7[k][6];
+  int m6 = 0, dg = 0;
+#pragma unroll
+  for (int i = 0; i < 7; i++) {
+    if (i == gs) dg = d7[i]; else m6 = max(m6, d7[i]);
+  }
+  return max(2 + m6, 1 + dg);
+}
+
 // The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
 // 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
-// feasible tuple and ordering the set of working outer functions from outer_ok5.
-template <int NW, int MODE>
+// feasible tuple and ordering the set of working outer functions from outer_ok5.  DF: the depth
+// filter (see depth5); `feasible` then counts the feasible tuples with an ordering within the bound.
+template <int NW, int MODE, bool DF>
 __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab) {
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
   constexpr int P = 3, K = 5, NC = 1 << P;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[256];
@@ -2739,6 +2829,9 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
   uint32_t *cells = smem + NW * npad + warp * (NC * 2 * NW);  // per prefix cell: C1[NW], C0[NW]
   stage_tables(s_tabs, prob, NW, npad);
   for (int i = threadIdx.x; i < 256; i += blockDim.x) s_ord[i] = ord.order[0][i];
+  const uint16_t *s_dep = nullptr;
+  if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
+  const int B = depth_bound(dep);
   __syncthreads();
   uint32_t T[NW], M[NW];
 #pragma unroll
@@ -2759,6 +2852,15 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
       bool rejected = false;
 #pragma unroll
       for (int i = 0; i < P; i++) rejected |= (pre[i] < 8) && ((inmask >> pre[i]) & 1u);
+      int pre_deep = 0;   // DF: prefix gates of depth B - 1 (at most two gates of a match may have it)
+      if constexpr (DF) {
+#pragma unroll
+        for (int i = 0; i < P; i++) {
+          rejected |= s_dep[pre[i]] >= B;
+          pre_deep += s_dep[pre[i]] >= B - 1;
+        }
+        rejected |= pre_deep > 2;
+      }
       const int last = pre[P - 1];
       const int r = n - last - 1;
       const uint32_t Q = rejected ? 0u : (uint32_t)(r * (r - 1) / 2);
@@ -2794,6 +2896,12 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
         if (alive) unrank_pair(q, r, pi, pj);
         const int gf = last + 1 + pi, gg = last + 1 + pj;
         if ((gf < 8 && ((inmask >> gf) & 1u)) || (gg < 8 && ((inmask >> gg) & 1u))) alive = false;
+        if constexpr (DF) {
+          if (alive) {
+            const int df = s_dep[gf], dg = s_dep[gg];
+            alive = df < B && dg < B && pre_deep + (df >= B - 1) + (dg >= B - 1) <= 2;
+          }
+        }
         for (uint32_t mc = mixed; mc != 0 && alive; mc &= mc - 1) {
           const int cj = __ffs(mc) - 1;
           uint32_t a11 = 0, a10 = 0, a01 = 0, a00 = 0, b11 = 0, b10 = 0, b01 = 0, b00 = 0;
@@ -2815,7 +2923,17 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
           feasible++;
           uint32_t H1, H0;
           summary5<NW>(s_tabs, npad, g5, T, M, lane, H1, H0);
+          int d5[5];
+          if constexpr (DF) {
+#pragma unroll
+            for (int i = 0; i < 5; i++) d5[i] = s_dep[g5[i]];
+          }
           for (int k = 0; k < 10 && !done; k++) {
+            int kd = 0;
+            if constexpr (DF) {
+              kd = depth5(d5, k);
+              if (kd > B) continue;
+            }
             uint32_t ok[8], surv_mine = 0;
             outer_ok5(H1, H0, k, lane, tab, ok);
             uint32_t c = 0;
@@ -2827,6 +2945,7 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
             }
             if (MODE == kEnumCount) {
               tk.count += c;
+              if (DF && lane == 0 && c != 0) hist_add(kd, c);
               continue;
             }
             if (c == 0) continue;
@@ -2846,6 +2965,7 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
       }
     }
   });
+  flush_hist<MODE>(dep);
 }
 
 // Middle functions of one cube set (see middle_cubes) as a 256-bit set over fm, word wd = fm >> 5.
@@ -2876,14 +2996,15 @@ __device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (
 // nparts + part), one warp per entry: the summary and stage-1 filter of k_decomp7 on the TRUE gate
 // tables (no stale outer cache), then per surviving outer function and ordering row the union of
 // the middle-function cubes.  Count: one lane per outer function; emit: positions in ascending
-// order, outer position in the loop, middle position across the lanes.
-template <int NW, int MODE>
+// order, outer position in the loop, middle position across the lanes.  DF: the depth filter (see
+// depth7); an entry without an ordering within the bound is skipped, and so is every row above it.
+template <int NW, int MODE, bool DF>
 __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab) {
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
   constexpr bool EMIT = MODE != kEnumCount;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
@@ -2898,6 +3019,9 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
   stage_tables(s_tabs, prob, NW, npad);
   for (int i = threadIdx.x; i < 25 * 32; i += blockDim.x) s_src7[i] = tab->src7[i >> 5][i & 31];
   for (int i = threadIdx.x; i < 512; i += blockDim.x) s_ord[i >> 8][i & 255] = ord.order[i >> 8][i & 255];
+  const uint16_t *s_dep = nullptr;
+  if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
+  const int B = depth_bound(dep);
   __syncthreads();
   uint32_t T[NW], M[NW];
 #pragma unroll
@@ -2916,11 +3040,29 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
       int g[7];
 #pragma unroll
       for (int i = 0; i < 7; i++) g[i] = (int)((cur >> (9 * (6 - i))) & 0x1ffu);
+      int d7[7];
+      if constexpr (DF) {
+        // no gate of depth >= B, and at most one of depth B - 1 (it must be the last input)
+        int deep = 0;
+        bool over = false;
+#pragma unroll
+        for (int i = 0; i < 7; i++) {
+          d7[i] = s_dep[g[i]];
+          over |= d7[i] >= B;
+          deep += d7[i] >= B - 1;
+        }
+        if (over || deep > 1) return;
+      }
       tuple_summary<NW>(s_tabs, npad, g, T, M, lane, sH);
       const uint32_t pass_j = triples_with_colourings(sH, lane);
       bool done = false;
       for (int j = 0; j < 25 && !done; j++) {
         if (((pass_j >> j) & 1u) == 0) continue;
+        if constexpr (DF) {
+          bool fits = false;
+          for (int row = 0; row < c_j_rows[j]; row++) fits |= depth7(d7, c_j_first_k[j] + row) <= B;
+          if (!fits) continue;
+        }
         uint32_t W[8], ok[8];
         outer_ok7(sH, s_src7[j * 32 + lane], lane, W, ok);
         uint32_t any = 0, surv_mine = 0;
@@ -2954,12 +3096,23 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
             uint32_t c = 0;
 #pragma unroll 1
             for (int row = 0; row < nrows; row++) {
+              int rd = 0;
+              if constexpr (DF) {
+                rd = depth7(d7, k0 + row);
+                if (rd > B) continue;
+              }
+              const uint32_t c_before = c;
               uint32_t hv[2][4], S, ov, bits[8];
               bool hok[2][4];
               middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
               cube_union(hv, hok, S, ov, bits);
 #pragma unroll
               for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd]);
+              if constexpr (DF) {
+                // rows differ in depth: each row's matches go to its own bin
+                const uint32_t s = __reduce_add_sync(kFull, have ? c - c_before : 0u);
+                if (lane == 0 && s != 0) hist_add(rd, s);
+              }
             }
             tk.count += __reduce_add_sync(kFull, have ? c : 0u);
           }
@@ -2967,6 +3120,7 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
 #pragma unroll 1
         for (int row = 0; EMIT && row < nrows && !done; row++) {
           const int k = k0 + row;
+          if (DF && depth7(d7, k) > B) continue;
 #pragma unroll 1
           for (int po = 0; po < 256 && !done; po++) {
             const uint32_t fo = s_ord[0][po];
@@ -3002,6 +3156,7 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
       }
     }
   });
+  flush_hist<MODE>(dep);
 }
 
 
@@ -3017,13 +3172,14 @@ struct EnumGateOrder {
 // of the target (scan3_blocks' test, here on the compressed tables).  Key i << 18 | k << 9 | m, so a
 // ticket's matches are consecutive keys in the order of its lanes.  A match's record: the gates in
 // position order, func_inner = cells holding a masked 1, inner_seen = cells holding a masked
-// position (sbg_solve_inner's closed form).
-template <int NW, int MODE>
+// position (sbg_solve_inner's closed form).  DF: the depth filter; a pair with a gate of depth
+// >= max_depth is skipped.
+template <int NW, int MODE, bool DF>
 __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts) {
+    int nparts, const EnumDepth<DF> dep) {
   extern __shared__ uint32_t smem[];
   __shared__ uint16_t s_order[kMaxGatesPad];
   const int lane = threadIdx.x & 31;
@@ -3032,6 +3188,9 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
   uint32_t *s_tabs = smem;
   stage_tables(s_tabs, prob, NW, npad);
   for (int i = threadIdx.x; i < n; i += blockDim.x) s_order[i] = go.order[i];
+  const uint16_t *s_dep = nullptr;
+  if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
+  const int B = depth_bound(dep);
   __syncthreads();
   uint32_t T[NW], Z[NW];   // masked positions with target 1 / with target 0
 #pragma unroll
@@ -3047,6 +3206,11 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
     if (dealt < pairs) {
       int pi, pk;
       unrank_pair((uint32_t)dealt, n, pi, pk);
+      int dab = 0;   // DF: the deeper of the pair's gates; a match's depth is 1 + max(dab, Dc)
+      if constexpr (DF) {
+        dab = max((int)s_dep[s_order[pi]], (int)s_dep[s_order[pk]]);
+        if (dab >= B) return;
+      }
       const uint32_t *ta = s_tabs + s_order[pi], *tb = s_tabs + s_order[pk];
       bool done = false;
       for (int m0 = pk + 1; m0 < n && !done; m0 += 32) {
@@ -3074,6 +3238,15 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
           if (one[c] != 0) ones |= 1u << c;
           if ((one[c] | zero[c]) != 0) seen |= 1u << c;
         }
+        if constexpr (DF) {
+          const int dm = 1 + max(dab, (int)s_dep[s_order[pm < n ? pm : pk]]);
+          ok &= dm <= B;
+          if (MODE == kEnumCount) {
+            // one histogram atomic per distinct depth of the ballot, by its lowest lane
+            const uint32_t peers = __match_any_sync(kFull, ok ? dm : -1);
+            if (ok && (peers & lanemask_lt()) == 0) hist_add(dm, __popc(peers));
+          }
+        }
         done = emit_step<MODE>(ok, tk, [&](unsigned long long i) {
           const int G[3] = {s_order[pi], s_order[pk], s_order[pm]};
           store_match<3>(out + i, ((unsigned long long)pi << 18) | ((unsigned long long)pk << 9)
@@ -3082,6 +3255,7 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
       }
     }
   });
+  flush_hist<MODE>(dep);
 }
 
 

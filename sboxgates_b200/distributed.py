@@ -26,8 +26,9 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .lut import (MATCH_DTYPE, SBG_KEY_NONE, SBG_LIST_CAP, Enumeration, result5_to_ret,
-                  result7_to_ret, sample_matches, shuffled_order, shuffled_orders7)
+from .lut import (MATCH_DTYPE, SBG_DEPTH_BINS, SBG_KEY_NONE, SBG_LIST_CAP, Enumeration,
+                  _trim, result5_to_ret, result7_to_ret, sample_matches, shuffled_order,
+                  shuffled_orders7)
 
 _I64_MAX = (1 << 63) - 1
 
@@ -268,3 +269,28 @@ class DistributedLutSearch:
         """k distinct matches drawn uniformly from the whole (lut.sample_matches); every rank draws
         the same ranks from the same seed."""
         return sample_matches(self, enumeration, k, seed)
+
+    # -- depth filter ----------------------------------------------------------------------------
+    def set_depth_filter(self, depth, max_depth):
+        """The engine's depth filter (LutEngine.set_depth_filter), on every rank: later
+        enumerations count, rank and fetch within the matches of depth <= max_depth."""
+        self.engine.set_depth_filter(depth, max_depth)
+
+    def clear_depth_filter(self):
+        self.engine.clear_depth_filter()
+
+    def depth_counts(self):
+        """The whole's matches per depth of the last enumerate* call (counted under a filter):
+        one all-reduce(SUM) of the ranks' histograms.  Trimmed after the last non-empty bin."""
+        local = self.engine.depth_counts()
+        if self.world == 1:
+            return local
+        t0 = time.perf_counter()
+        full = np.zeros(SBG_DEPTH_BINS, dtype=np.uint64)
+        full[:local.shape[0]] = local
+        t = torch.from_numpy(full.view(np.int64).copy()).to(self.device)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        self.collectives += 1
+        out = t.cpu().numpy().view(np.uint64)
+        self.collective_ms += 1e3 * (time.perf_counter() - t0)
+        return _trim(out)

@@ -11,6 +11,8 @@ import xml.etree.ElementTree as ET
 from dataclasses import dataclass, field
 from typing import List
 
+import numpy as np
+
 MASK256 = (1 << 256) - 1
 
 # state.h:35-56 / state.c:33-53; a two-input gate type's number is its truth table over (A, B):
@@ -140,6 +142,17 @@ def load_graph(path):
             raise GraphError("bad output element")
         g.outputs[bit] = gate
     return g
+
+
+def gate_depths(graph):
+    """The depth of every gate of a loaded graph, in gate order, as a numpy uint16 array: 0 for an
+    input, else 1 + the largest depth among the gate's inputs.  What LutEngine.set_depth_filter
+    takes for the graph's search state."""
+    depth = np.zeros(len(graph.gates), dtype=np.uint16)
+    for i, g in enumerate(graph.gates):
+        if g.type != "IN":
+            depth[i] = 1 + max((int(depth[j]) for j in g.inputs), default=0)
+    return depth
 
 
 def verify_graph(graph, sbox, require_bits=None):

@@ -15,7 +15,7 @@ import numpy as np
 from . import native
 from .native import (SbgResult, SbgJob, SbgNodeResult, NativeLibraryError, SBG_KEY_NONE,
                      SBG_LIST_CAP, SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7, MATCH_DTYPE,
-                     SBG_ENUM_MAX_MATCHES)
+                     SBG_ENUM_MAX_MATCHES, SBG_MAX_GATES, SBG_MAX_DEPTH, SBG_DEPTH_BINS)
 
 NO_GATE = 0xFFFF  # state.h:30
 
@@ -479,6 +479,86 @@ class LutEngine:
                                                  counts.ctypes.data_as(native.u64p),
                                                  int(counts.shape[0]), C.byref(total)))
         return int(total.value)
+
+    # -- depth filter: the realisations at or below a circuit depth -----------------------------
+    def set_depth_filter(self, depth, max_depth):
+        """Later enumerate3/5/7 calls keep only the matches of depth <= max_depth, `depth` giving
+        the depth of each of the problem's gates (see match_depth).  Ends the cursor.  The
+        searches never read the filter."""
+        d, max_depth = _depth_args(depth, max_depth)
+        buf = (C.c_uint16 * d.shape[0]).from_buffer_copy(d.tobytes())
+        self._check(self.lib.sbg_enum_set_depth(self._h, buf, d.shape[0], max_depth))
+
+    def clear_depth_filter(self):
+        """Removes the depth filter.  Ends the cursor."""
+        self._check(self.lib.sbg_enum_set_depth(self._h, None, 0, 0))
+
+    def depth_counts(self):
+        """The cursor's matches per depth (index = depth) as a numpy uint64 array, cut after the
+        last non-empty bin.  The cursor must have been counted under a depth filter."""
+        out = np.zeros(SBG_DEPTH_BINS, dtype=np.uint64)
+        self._check(self.lib.sbg_enum_depth_counts(self._h, out.ctypes.data_as(native.u64p),
+                                                   SBG_DEPTH_BINS))
+        return _trim(out)
+
+
+def _depth_args(depth, max_depth):
+    """A depth filter's arguments, checked: (uint16 array of the gate depths, bound)."""
+    d = np.asarray(depth)
+    if d.ndim != 1 or not 1 <= d.shape[0] <= SBG_MAX_GATES:
+        raise ValueError("depth must be a 1-D array of 1..%d gate depths" % SBG_MAX_GATES)
+    if d.dtype.kind not in "iu":
+        raise ValueError("depth must hold integers")
+    if int(d.min()) < 0 or int(d.max()) > SBG_MAX_DEPTH:
+        raise ValueError("gate depths must lie in 0..%d" % SBG_MAX_DEPTH)
+    max_depth = int(max_depth)
+    if not 0 <= max_depth < 2**32:
+        raise ValueError("max_depth must lie in 0..2**32-1")
+    return np.ascontiguousarray(d, dtype=np.uint16), max_depth
+
+
+def _trim(hist):
+    """A histogram without its trailing empty bins."""
+    nz = np.flatnonzero(hist)
+    return hist[:int(nz[-1]) + 1].copy() if nz.size else hist[:0].copy()
+
+
+def match_depth(record, depth):
+    """The depth of the gate an enumerated match (a MATCH_DTYPE record) would add, given the depth
+    of every gate of the problem: 1 + max(Da, Db, Dc) for a 3-LUT; 1 + max(1 + max(Da, Db, Dc),
+    Dd, De) for a 5-LUT (outer LUT over a, b, c); 1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df),
+    Dg) for a 7-LUT (outer over a, b, c, middle over d, e, f).  Gates in the record's order."""
+    width = int(record["width"])
+    d = [int(depth[int(g)]) for g in record["gates"][:width]]
+    if width == 3:
+        return 1 + max(d)
+    if width == 5:
+        return 1 + max(1 + max(d[:3]), d[3], d[4])
+    if width == 7:
+        return 1 + max(1 + max(d[:3]), 1 + max(d[3:6]), d[6])
+    raise ValueError("not a match record (width %d)" % width)
+
+
+def shallowest_matches(engine, width, orders, depth, max_matches):
+    """The shallowest realisations of the current problem by the width-3, 5 or 7 enumeration:
+    one count with the loosest bound gives the depth histogram, a second counts at its first
+    non-empty depth.  `orders` are the enumerate call's order arguments: (gate_order,),
+    (func_order,) or (outer, middle).  Returns (minimum depth or None, the number of matches at
+    it, the first max_matches of them in key order).  The filter stays installed at the minimum
+    depth, so the engine's cursor serves the shallowest set (fetch_matches, pick_matches).
+    `engine` is a LutEngine or a DistributedLutSearch."""
+    if width not in (3, 5, 7):
+        raise ValueError("width must be 3, 5 or 7")
+    run = getattr(engine, "enumerate%d" % width)
+    engine.set_depth_filter(depth, SBG_DEPTH_BINS - 1)
+    run(*orders, 0)
+    hist = engine.depth_counts()
+    if hist.size == 0:
+        return None, 0, np.zeros(0, dtype=MATCH_DTYPE)
+    dmin = int(np.flatnonzero(hist)[0])
+    engine.set_depth_filter(depth, dmin)
+    e = run(*orders, max_matches)
+    return dmin, int(e.total), e.matches
 
 
 def _torch_stream_done(t):

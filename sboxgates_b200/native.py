@@ -54,6 +54,9 @@ MATCH_DTYPE = np.dtype([("key", "<u8"), ("gates", "<u2", (7,)), ("func_outer", "
                         ("func_middle", "u1"), ("func_inner", "u1"), ("inner_seen", "u1"),
                         ("width", "u1"), ("pad", "u1", (5,))])
 SBG_ENUM_MAX_MATCHES = 1 << 24
+SBG_MAX_GATES = 500
+SBG_MAX_DEPTH = 1020      # largest gate depth of a depth filter
+SBG_DEPTH_BINS = 1024     # bins of the depth histogram
 
 SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7 = 1, 2, 4
 SBG_LANES = 8
@@ -108,6 +111,8 @@ SIGNATURES = {
     "sbg_enum_pick": (C.c_int, [C.c_void_p, u64p, C.c_uint64, C.c_void_p]),
     "sbg_enum_block_sums": (C.c_int, [C.c_void_p, C.c_void_p, u64p]),
     "sbg_enum_set_global": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, u64p, C.c_int, u64p]),
+    "sbg_enum_set_depth": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint16), C.c_int, C.c_uint32]),
+    "sbg_enum_depth_counts": (C.c_int, [C.c_void_p, u64p, C.c_uint32]),
 }
 
 _lib = None
