@@ -227,25 +227,19 @@ struct sbg_handle {
   uint64_t feasible = 0;
   std::map<std::pair<const void *, size_t>, int> occupancy;  // grid_for's cache
   std::map<const void *, size_t> smem_attr;                  // largest dynamic smem opted into
-  // tuning knobs, read from the environment when the handle is created (tests create handles under
-  // different settings to cross-check the alternative kernels against each other)
-  int opt_batch = 0;        // SBG_BATCH: prefixes per ticket batch (0 = automatic)
+  // Kernel-form switches, read from the environment when the handle is created.  Each forces one
+  // form of a kernel that the automatic choice would not pick for the same state, so that tests can
+  // compare the forms with each other and with the oracle.  SBG_TICKET_TABLE and SBG_HITS_CAP (below)
+  // shrink the ticket table and the hit buffer to reach the segment and overflow-retry paths.
   int opt_pm_prefix = 0;    // SBG_PM_PREFIX: 4 or 5 (0 = by n)
   int opt_search5 = 0;      // SBG_SEARCH5: 0 by size, 1 fused, 2 two kernels
   int opt_head = -1;        // SBG_HEAD: chunked phase of the 7-LUT filter, 0 none, 1 first prefixes,
                             // 2 everything (-1 = by n and mask size)
   int opt_shift = -1;       // SBG_SHIFT: phase-1 shifted single-word windows, 0 never, 1 whenever n <= 63
-  int opt_head_waves = 0;   // SBG_HEAD_WAVES: size of the chunked head in waves of warps (0 = default)
-  int opt_pdl = 1;          // SBG_PDL: programmatic dependent launch between the kernels of a chain
-  int opt_speculate = 1;    // SBG_SPECULATE: see enqueue_chain
-  int opt_group_chunks = 6; // SBG_GROUP_CHUNKS: chunks of 32 pairs per weighted phase-1 ticket (0 = whole prefixes)
-  int opt_group_chunks_conc = 0;  // SBG_GROUP_CHUNKS_CONC: the same while several chains share the device
   int opt_packed = 1;       // SBG_PACKED: phase 1 keeps two parts per register where <= 15 last gates remain
   int opt_sieve = 1;        // SBG_SIEVE: phase 1 (shifted windows) rules out last gates with the pair sieve
                             // first: 0 never, 1 above kSieveMinPositions masked positions, 2 always
   int opt_decomp_filter = 1;  // SBG_DECOMP_FILTER: lane-parallel stage-1 filter of phase 2 (0 = ballot form only)
-  int opt_batch_conc = 2;   // SBG_BATCH_CONC: phase-1 prefixes per ticket while several chains share
-                            // the device (sbg_search_batch)
   bool concurrent = false;  // set while sbg_search_batch enqueues more than one chain
   bool hits_cap_forced = false;
   size_t hits_cap_default = kDefaultHitsCap;
@@ -347,7 +341,7 @@ cudaError_t launch(sbg_handle *h, void (*kernel)(KArgs...), int grid, int block,
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = (pdl && h->opt_pdl != 0) ? 1 : 0;
+  cfg.numAttrs = pdl ? 1 : 0;
   h->launches++;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
@@ -384,23 +378,20 @@ constexpr int kShiftMaxGates = 60;
 // 0.393 / 0.277 / 0.231 ms to 0.264 / 0.231 / 0.212 ms; under 32 positions the cell loop visits
 // about 10 positions per chunk, no more than the sieve's per-prefix set-up saves (0.220 -> 0.223 ms).
 constexpr int kSieveMinPositions = 32;
+// Phase-1 prefixes per ticket (4-gate prefixes, n <= kSinglePrefixMaxGates) while several chains
+// share the device (sbg_search_batch).
+constexpr uint64_t kConcurrentBatch = 2;
 uint64_t pick_batch(const sbg_handle *h, uint64_t tickets, int n, int P) {
   const uint64_t warps = kNominalWarps;
-  if (h->opt_batch > 0) {
-    uint64_t b = std::max<uint64_t>(1, std::min<uint64_t>(16, (uint64_t)h->opt_batch));
-    while (b & (b - 1)) b &= b - 1;
-    return b;
-  }
   // work per ticket in lane-items: (d,e) pairs for the 5-LUT sweep (P = 3), (e,f) pairs for the
   // position-major kernel with 4-gate prefixes (P = 4), single f for its 5-gate form (P = 6)
   const bool pm = P == 4 || P == 6;
-  // position-major kernel, 4-gate prefixes: single prefixes up to n = 72 (scripts/sweep_head.sh /
-  // sweep_batch.sh: faster than the formula below at n = 48 and 64 under a full mask; from n = 80 on
-  // the formula's 4 is as good or better)
+  // position-major kernel, 4-gate prefixes: single prefixes up to n = 72 (faster than the formula
+  // below at n = 48 and 64 under a full mask; from n = 80 on the formula's 4 is as good or better)
   // ... when the kernel has the device to itself.  Several chains at once (sbg_search_batch) fill
   // each other's tails, and what counts is fewer trips to the ticket counter: on bench.py's step
   // (n = 40, 8 states) pairs of prefixes beat single prefixes and fours.
-  if (P == 4 && n <= kSinglePrefixMaxGates) return h->concurrent ? (uint64_t)h->opt_batch_conc : 1;
+  if (P == 4 && n <= kSinglePrefixMaxGates) return h->concurrent ? kConcurrentBatch : 1;
   const uint64_t total = pm ? h_binom[n - 1][6] : h_binom[n][P + 2];
   const uint64_t avg_pairs = std::max<uint64_t>(1, total / std::max<uint64_t>(1, tickets));
   const uint64_t qmax = P == 6 ? (uint64_t)std::max(1, n - 7) : h_binom[n - P - (P == 4 ? 1 : 0)][2];
@@ -682,8 +673,7 @@ ChunkPlan plan_chunks(const sbg_handle *h, const sbg_handle::HostProblem &hp, bo
   if (retry) mode = n >= kHeadAlwaysMinGates ? 2 : 0;
   // lane items: (e,f) pairs out of the n-5 gates that leave room for g; single f for 5-gate prefixes
   const uint64_t qmax = P == 4 ? h_binom[n - 5][2] : (uint64_t)(n - 6);
-  return plan_chunks_mode<P, 7>(n, hp.inmask, mode,
-      h->opt_head_waves > 0 ? (uint64_t)h->opt_head_waves : kHeadWaves, qmax);
+  return plan_chunks_mode<P, 7>(n, hp.inmask, mode, kHeadWaves, qmax);
 }
 
 // How one phase-1 launch is cut into tickets: everything the filter, k_offsets and k_begin must
@@ -728,6 +718,9 @@ void build_weighted(int n, uint32_t group_pairs, WeightedTickets *wt) {
   wt->total = wt->w[3][0];
 }
 
+// Chunks of 32 pairs per weighted ticket.
+constexpr uint32_t kGroupChunks = 6;
+
 template <int P>
 FilterPlan plan_filter_p(const sbg_handle *h, const sbg_lane &L, const sbg_handle::HostProblem &hp,
     int nparts, bool retry, uint64_t seg_base) {
@@ -749,11 +742,10 @@ FilterPlan plan_filter_p(const sbg_handle *h, const sbg_lane &L, const sbg_handl
   if (fp.max_warps > 0) fp.batch = 1;
   fp.wt.group_pairs = 0;
   // Weighted tickets: a chain that has the device to itself, 4-gate prefixes, no head, no retry
-  // (chains that share the device fill each other's tails and prefer fewer, larger tickets).
-  const int group_chunks = h->concurrent ? h->opt_group_chunks_conc : h->opt_group_chunks;
-  if (P == 4 && !retry && group_chunks > 0 && h->opt_batch <= 0
-      && fp.pl.items == 0 && n >= 7 && n <= kWeightedMaxGates) {
-    build_weighted(n, 32u * (uint32_t)group_chunks, &fp.wt);
+  // (chains that share the device fill each other's tails and prefer fewer, larger tickets: whole
+  // prefixes, see pick_batch).
+  if (P == 4 && !retry && !h->concurrent && fp.pl.items == 0 && n >= 7 && n <= kWeightedMaxGates) {
+    build_weighted(n, 32u * kGroupChunks, &fp.wt);
     if (fp.wt.group_pairs != 0) {
       fp.tickets = ((uint64_t)fp.wt.total + nparts - 1) / nparts;
       fp.batch = 1;
@@ -1087,11 +1079,6 @@ int stage_problem(sbg_handle *h, int slot, const uint64_t *tables, int n, const 
 
 constexpr int kDoScan3 = SBG_DO_SCAN3, kDoSearch5 = SBG_DO_SEARCH5, kDoSearch7 = SBG_DO_SEARCH7;
 
-struct ChainInfo {
-  bool two5 = false;
-  FilterPlan fp;
-};
-
 // First kernel of a chain: control words, position tables, minpos3, ticket-group counters, and
 // whatever of the problem block has to be (re)derived.
 int enqueue_begin(sbg_handle *h, sbg_lane &L, uint32_t flags, const CallInputs &in, uint32_t gcount_n) {
@@ -1131,7 +1118,7 @@ int enqueue_begin(sbg_handle *h, sbg_lane &L, uint32_t flags, const CallInputs &
 // Enqueues scan3 -> search_5lut -> search_7lut (whichever `what` asks for) of the lane's problem,
 // every stage predicated on the device on the earlier ones not having matched.  One launch chain,
 // no host synchronisation inside.
-int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in, ChainInfo &ci) {
+int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
   sbg_handle::HostProblem &hp = h->slots[L.slot];
   int rc;
   L.seq++;
@@ -1140,25 +1127,23 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in, Ch
   if ((what & kDoSearch5) && hp.n >= 5) flags |= kBeginSearch5;
   if ((what & kDoSearch7) && hp.n >= 7) flags |= kBeginSearch7 | kBeginRows;
   uint32_t gcount_n = 0;
+  FilterPlan fp;
   if (flags & kBeginSearch7) {
     if ((rc = ensure_hits(h, L, std::max(L.hits_cap, h->hits_cap_default))) != SBG_OK) return rc;
-    ci.fp = plan_filter(h, L, hp, 1, false);
-    if ((rc = ensure_tickets(h, L, ci.fp.tickets_cap)) != SBG_OK) return rc;
-    gcount_n = (uint32_t)(ci.fp.tickets_cap / kTicketGroup + 1);
+    fp = plan_filter(h, L, hp, 1, false);
+    if ((rc = ensure_tickets(h, L, fp.tickets_cap)) != SBG_OK) return rc;
+    gcount_n = (uint32_t)(fp.tickets_cap / kTicketGroup + 1);
   }
-  if (flags & kBeginSearch5) ci.two5 = search5_two_kernels(h, hp.n);
   if ((rc = enqueue_begin(h, L, flags, in, gcount_n)) != SBG_OK) return rc;
-  // How far ahead of the results to launch (SBG_SPECULATE; single calls -- a batch always launches
-  // whole chains, its lanes keep the device busy).  Half of a graph build's nodes end at the 3-LUT
-  // scan, which runs inside that first kernel, and a third at search_5lut: the kernels of the later
-  // stages would return at once, but launching and draining hundreds of empty blocks still occupies
-  // the stream for 15-20 us, which the NEXT node's chain then waits behind.  So by default the host
-  // looks at the scan's result before it launches search_5lut + search_7lut (one idle launch latency
-  // for the nodes that go on, against the drain for the ones that do not); 0 = also wait for
-  // search_5lut before launching search_7lut; 2 = launch everything at once.
+  // How far ahead of the results to launch.  A batch launches whole chains: its lanes keep the
+  // device busy.  Half of a graph build's nodes end at the 3-LUT scan, which runs inside that first
+  // kernel: the kernels of the later stages would return at once, but launching and draining
+  // hundreds of empty blocks still occupies the stream for 15-20 us, which the NEXT node's chain then
+  // waits behind.  So a single call looks at the scan's result before it launches search_5lut +
+  // search_7lut (one idle launch latency for the nodes that go on, against the drain for the ones
+  // that do not).
   const volatile HostOut *o = L.h_out;
-  const int policy = h->concurrent ? 2 : h->opt_speculate;
-  if ((flags & kBeginScan3) && policy < 2 && (flags & (kBeginSearch5 | kBeginSearch7))) {
+  if ((flags & kBeginScan3) && !h->concurrent && (flags & (kBeginSearch5 | kBeginSearch7))) {
     if ((rc = wait_stage(h, L, 0)) != SBG_OK) return rc;
   }
   auto over = [&]() {
@@ -1167,14 +1152,9 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in, Ch
         && (word & kScanKeyNone) != kScanKeyNone;
   };
   if ((flags & kBeginSearch5) && !over()
-      && (rc = enqueue_search5(h, L, 0, 1, ci.two5)) != SBG_OK) return rc;
-  bool stop = over();
-  if (!stop && policy == 0 && (flags & kBeginSearch5) && (flags & kBeginSearch7)) {
-    if ((rc = wait_stage(h, L, 1)) != SBG_OK) return rc;
-    stop = o->key[1] != SBG_KEY_NONE || o->overflow[1] != 0;
-  }
-  if ((flags & kBeginSearch7) && !stop) {
-    if ((rc = enqueue_filter7(h, L, ci.fp, 0, 1)) != SBG_OK) return rc;
+      && (rc = enqueue_search5(h, L, 0, 1, search5_two_kernels(h, hp.n))) != SBG_OK) return rc;
+  if ((flags & kBeginSearch7) && !over()) {
+    if ((rc = enqueue_filter7(h, L, fp, 0, 1)) != SBG_OK) return rc;
     if (!over() && (rc = enqueue_decomp7(h, L, 0, 1, SBG_LIST_CAP)) != SBG_OK) return rc;
   }
   record_done(h, L);
@@ -1249,8 +1229,7 @@ int redo_search7_steps(sbg_handle *h, sbg_lane &L, const uint8_t *outer, const u
 
 // Waits for the lane's chain stage by stage and fills the result.  Returns as soon as a stage
 // matched (the rest of the chain drains as no-ops).
-int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, const ChainInfo &ci,
-    sbg_node_result *res) {
+int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, sbg_node_result *res) {
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const HostOut *o = L.h_out;
   int rc;
@@ -1303,7 +1282,6 @@ int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, const ChainInf
         o->feasible[2], swept7, &res->r7)) != SBG_OK) return rc;
     if (res->r7.found) res->found_stage = 7;
   }
-  (void)ci;
   return SBG_OK;
 }
 
@@ -1787,45 +1765,18 @@ int sbg_create(sbg_handle **out, int device) {
         e != cudaSuccess ? cudaGetErrorString(e) : "device count 0");
   }
   if (device < 0 || device >= ndev) return fail(h, SBG_ERR_ARG, "device %d out of range", device);
-  const bool timing = getenv("SBG_DEBUG_TIMING") != nullptr;
-  auto stamp = [&](const char *what) {
-    static double last = 0.0;
-    if (!timing) return;
-    struct timespec ts;
-    clock_gettime(CLOCK_MONOTONIC, &ts);
-    const double t = ts.tv_sec + 1e-9 * ts.tv_nsec;
-    if (last != 0.0) fprintf(stderr, "[sbg_create] %-28s %.1f ms\n", what, 1e3 * (t - last));
-    last = t;
-  };
-  stamp("start");
   SBG_CUDA(h, cudaSetDevice(device));
   SBG_CUDA(h, cudaFree(nullptr));
-  stamp("context");
   cudaDeviceProp prop;
   SBG_CUDA(h, cudaGetDeviceProperties(&prop, device));
   h->sm_count = prop.multiProcessorCount;
-  if (getenv("SBG_BATCH") != nullptr) h->opt_batch = atoi(getenv("SBG_BATCH"));
   if (getenv("SBG_PM_PREFIX") != nullptr) h->opt_pm_prefix = atoi(getenv("SBG_PM_PREFIX"));
   if (getenv("SBG_HEAD") != nullptr) h->opt_head = std::max(0, std::min(2, atoi(getenv("SBG_HEAD"))));
-  if (getenv("SBG_GROUP_CHUNKS") != nullptr) {
-    h->opt_group_chunks = std::max(0, std::min(64, atoi(getenv("SBG_GROUP_CHUNKS"))));
-  }
-  if (getenv("SBG_GROUP_CHUNKS_CONC") != nullptr) {
-    h->opt_group_chunks_conc = std::max(0, std::min(64, atoi(getenv("SBG_GROUP_CHUNKS_CONC"))));
-  }
   if (getenv("SBG_PACKED") != nullptr) h->opt_packed = atoi(getenv("SBG_PACKED")) != 0;
   if (getenv("SBG_SHIFT") != nullptr) h->opt_shift = atoi(getenv("SBG_SHIFT")) != 0;
   if (getenv("SBG_SIEVE") != nullptr) h->opt_sieve = std::max(0, std::min(2, atoi(getenv("SBG_SIEVE"))));
-  if (getenv("SBG_HEAD_WAVES") != nullptr) h->opt_head_waves = atoi(getenv("SBG_HEAD_WAVES"));
-  if (getenv("SBG_PDL") != nullptr) h->opt_pdl = atoi(getenv("SBG_PDL")) != 0;
-  if (getenv("SBG_DECOMP_FILTER") != nullptr) {   // 0 off, 1 by list length, 2..32 forced block size
-    h->opt_decomp_filter = std::max(0, std::min(32, atoi(getenv("SBG_DECOMP_FILTER"))));
-  }
-  if (getenv("SBG_SPECULATE") != nullptr) h->opt_speculate = std::max(0, std::min(2, atoi(getenv("SBG_SPECULATE"))));
-  if (getenv("SBG_BATCH_CONC") != nullptr) {
-    int b = std::max(1, std::min(16, atoi(getenv("SBG_BATCH_CONC"))));
-    while (b & (b - 1)) b &= b - 1;
-    h->opt_batch_conc = b;
+  if (getenv("SBG_DECOMP_FILTER") != nullptr) {   // 0 ballot form only, 1 lane-parallel filter first
+    h->opt_decomp_filter = atoi(getenv("SBG_DECOMP_FILTER")) > 0;
   }
   if (getenv("SBG_TIMING") != nullptr) h->timing = atoi(getenv("SBG_TIMING")) != 0;
   if (getenv("SBG_SEARCH5") != nullptr) {
@@ -1861,10 +1812,8 @@ int sbg_create(sbg_handle **out, int device) {
     SBG_CUDA(h, cudaHostGetDevicePointer(&L.d_out, L.h_out, 0));
     SBG_CUDA(h, cudaMallocHost(&L.h_ctl, sizeof(DevCtl)));
   }
-  stamp("lanes");
 
   SBG_CUDA(h, cudaMemcpyToSymbol(c_binom, h_binom, sizeof(h_binom)));
-  stamp("first symbol (module load)");
   {
     // search5: lane = u<<2 | v2, canonical cell bit of slot s is 4-s.
     uint8_t src5[10][32];
@@ -1970,7 +1919,6 @@ int sbg_create(sbg_handle **out, int device) {
     SBG_CUDA(h, cudaMemcpyToSymbol(c_rows7, rows7, sizeof(rows7)));
   }
 
-  stamp("constant tables");
   SBG_CUDA(h, cudaMalloc(&h->d_slots, sizeof(DevProblem) * kSlots));
   h->slots = new sbg_handle::HostProblem[kSlots];
   for (int i = 0; i < kSlots; i++) {
@@ -1978,7 +1926,6 @@ int sbg_create(sbg_handle **out, int device) {
   }
   SBG_CUDA(h, cudaMallocHost(&h->h_stage, (size_t)SBG_MAX_GATES * 32));
   SBG_CUDA(h, cudaStreamSynchronize(h->lane[0].stream));
-  stamp("problem slots");
   return SBG_OK;
 }
 
@@ -2404,11 +2351,10 @@ int sbg_search_node(sbg_handle *h, const sbg_job *job, sbg_node_result *res) {
   in.outer = job->outer7;
   in.middle = job->middle7;
   in.gate_order = job->gate_order;
-  ChainInfo ci;
   L.list_ready = false;
-  if ((rc = enqueue_chain(h, L, job->flags, in, ci)) != SBG_OK) return rc;
+  if ((rc = enqueue_chain(h, L, job->flags, in)) != SBG_OK) return rc;
   const double t1 = wall_now();
-  if ((rc = collect_chain(h, L, job, ci, res)) != SBG_OK) return rc;
+  if ((rc = collect_chain(h, L, job, res)) != SBG_OK) return rc;
   h->host_s[0] += t1 - t0;
   h->host_s[1] += wall_now() - t1;
   if (h->timing) {
@@ -2437,7 +2383,6 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
   cudaStream_t main_stream = h->lane[0].stream;
   for (int base = 0; base < njobs; base += kLanes) {
     const int wave = std::min(kLanes, njobs - base);
-    ChainInfo ci[kLanes];
     h->concurrent = wave > 1;
     if (wave > 1) SBG_CUDA(h, cudaEventRecord(h->lane[0].ev_done, main_stream));
     for (int k = 0; k < wave; k++) {
@@ -2452,7 +2397,7 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
       in.middle = job.middle7;
       in.gate_order = job.gate_order;
       L.list_ready = false;
-      if ((rc = enqueue_chain(h, L, job.flags, in, ci[k])) != SBG_OK) {
+      if ((rc = enqueue_chain(h, L, job.flags, in)) != SBG_OK) {
         h->concurrent = false;
         return rc;
       }
@@ -2460,7 +2405,7 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
     h->concurrent = false;
     for (int k = 0; k < wave; k++) {
       sbg_lane &L = h->lane[k];
-      if ((rc = collect_chain(h, L, &jobs[base + k], ci[k], &results[base + k])) != SBG_OK) return rc;
+      if ((rc = collect_chain(h, L, &jobs[base + k], &results[base + k])) != SBG_OK) return rc;
     }
     // join: the caller's stream waits for every lane's chain (including chains still draining)
     for (int k = 1; k < wave; k++) {

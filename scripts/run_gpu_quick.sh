@@ -3,4 +3,3 @@
 cd /root/repo
 ( timeout 1800 python -m pytest tests/test_gpu_node.py tests/test_gpu_parity.py tests/test_gpu_stress.py -m gpu -x -q 2>&1 | tail -6 )
 bash scripts/dropin_time.sh sboxgates_gpu 2>&1 | grep -v "^\[sbg\] start-up" | cut -c1-330
-L=sboxgates_b200/libsboxgates_b200.so; bash scripts/ab_bench.sh $L:SBG_GROUP_CHUNKS=0 $L:SBG_GROUP_CHUNKS=1 $L $L:SBG_GROUP_CHUNKS=4 $L:SBG_GROUP_CHUNKS=0 $L

@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
 """Randomised differential test on the GPU (minutes, not part of pytest): for random states / masks /
 excluded bits it checks that
-  * every phase-1 form (position-major with 4- and 5-gate prefixes, with and without programmatic
-    dependent launch) and every batch size returns the same hit list, equal to the CPU oracle's where that is affordable;
+  * every phase-1 form (position-major with 4- and 5-gate prefixes, packed and unpacked, with and
+    without programmatic dependent launch) returns the same hit list, equal to the CPU oracle's where
+    that is affordable;
   * sharded phase 1 (3 parts) merges to the same list;
   * search_5lut: fused kernel == two kernels == 3 parts, and == oracle for small n;
   * search_7lut: one-call path == step-by-step path == 4 parts.
@@ -31,10 +32,9 @@ def engine(**env):
 
 cases = int(sys.argv[1]) if len(sys.argv) > 1 else 60
 rs = np.random.RandomState(int(sys.argv[2]) if len(sys.argv) > 2 else 1)
-engines = {"pm4": engine(SBG_PM_PREFIX=4), "pm5": engine(SBG_PM_PREFIX=5),
-           "plain": engine(SBG_PDL=0), "pm4_b1": engine(SBG_PM_PREFIX=4, SBG_BATCH=1),
-           "pm5_b16": engine(SBG_PM_PREFIX=5, SBG_BATCH=16),
-           "pm4_g1": engine(SBG_PM_PREFIX=4, SBG_GROUP_CHUNKS=1, SBG_PACKED=0)}
+engines = {"pm4": engine(SBG_PM_PREFIX=4), "pm5": engine(SBG_PM_PREFIX=5), "plain": engine(),
+           "pm4_unpacked": engine(SBG_PM_PREFIX=4, SBG_PACKED=0)}
+engines["plain"].set_timing(True)   # timed launches are stream-ordered, without programmatic dependent launch
 e5 = {"fused": engine(SBG_SEARCH5="fused"), "two": engine(SBG_SEARCH5="two")}
 e7_plain = engine(SBG_DECOMP_FILTER=0)   # phase 2 without the lane-parallel stage-1 filter
 sbox = S.rijndael_sbox()

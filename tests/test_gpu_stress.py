@@ -1,4 +1,4 @@
-"""GPU: randomised differential test (scripts/stress_gpu.py): all phase-1 kernels and batch sizes,
+"""GPU: randomised differential test (scripts/stress_gpu.py): all phase-1 kernel forms,
 sharded and unsharded paths, fused and two-kernel search_5lut, one-call and step-by-step
 search_7lut must agree with each other, and with the CPU oracle wherever it is affordable."""
 import os
