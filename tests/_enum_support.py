@@ -274,3 +274,57 @@ def record_fields(rec):
     width = int(rec["width"])
     return ([int(g) for g in rec["gates"][:width]], int(rec["func_outer"]), int(rec["func_middle"]),
             int(rec["func_inner"]), int(rec["inner_seen"]))
+
+
+# ------------------------------------------------------------------------------------------------
+# The depth filter on the host: what a filtered enumeration must keep, from the unfiltered records.
+
+def record_depths(recs, depth):
+    """match_depth of every record (all of one width), vectorised."""
+    if len(recs) == 0:
+        return np.zeros(0, dtype=np.int64)
+    w = int(recs["width"][0])
+    d = np.asarray(depth, dtype=np.int64)[recs["gates"][:, :w].astype(np.int64)]
+    if w == 3:
+        return 1 + d.max(axis=1)
+    if w == 5:
+        return 1 + np.maximum(1 + d[:, :3].max(axis=1), d[:, 3:].max(axis=1))
+    return 1 + np.maximum(np.maximum(1 + d[:, :3].max(axis=1), 1 + d[:, 3:6].max(axis=1)), d[:, 6])
+
+
+def bound_admits(d, bound, width):
+    """Whether a gate set of depths d ((..., width)) has an ordering of depth <= bound, by the
+    shortcut the filtered kernels prune with: no gate of depth >= bound, and at most two (width 5)
+    or one (width 7) of depth bound - 1; width 3 has one ordering, of depth 1 + the deepest gate."""
+    d = np.asarray(d, dtype=np.int64)
+    fits = np.all(d < bound, axis=-1)
+    if width == 3:
+        return fits
+    return fits & (np.sum(d >= bound - 1, axis=-1) <= {5: 2, 7: 1}[width])
+
+
+def feasible5_under_bound(tabs, target, mask, inbits, depth, bound):
+    """The feasible 5-combinations of the state with an ordering of depth <= bound, by brute force
+    over all of C(n, 5): a combination is feasible iff no masked position of target 1 and masked
+    position of target 0 share its gates' 5-bit pattern; combinations holding an excluded input
+    bit do not count."""
+    from itertools import combinations
+    n = len(tabs)
+    pos = np.arange(256)
+    bits = np.stack([(np.asarray(t, dtype=np.uint64)[pos >> 6] >> (pos & 63).astype(np.uint64))
+                     & np.uint64(1) for t in tabs]).astype(np.int64)                    # (n, 256)
+    tg = (np.asarray(target, dtype=np.uint64)[pos >> 6] >> (pos & 63).astype(np.uint64)) & np.uint64(1)
+    mk = (np.asarray(mask, dtype=np.uint64)[pos >> 6] >> (pos & 63).astype(np.uint64)) & np.uint64(1)
+    p1, p0 = np.flatnonzero((mk == 1) & (tg == 1)), np.flatnonzero((mk == 1) & (tg == 0))
+    combs = np.array(list(combinations(range(n), 5)), dtype=np.int64).reshape(-1, 5)
+    combs = combs[~np.isin(combs, list(inbits)).any(axis=1)]
+    combs = combs[bound_admits(np.asarray(depth, dtype=np.int64)[combs], bound, 5)]
+    if len(combs) == 0:
+        return 0
+    pattern = sum(bits[combs[:, i]] << i for i in range(5))                         # (C, 256)
+    rows = np.arange(len(combs))[:, None]
+    ones = np.zeros((len(combs), 32), dtype=bool)
+    zeros = np.zeros((len(combs), 32), dtype=bool)
+    ones[rows, pattern[:, p1]] = True
+    zeros[rows, pattern[:, p0]] = True
+    return int(np.sum(~np.any(ones & zeros, axis=1)))

@@ -1,6 +1,9 @@
 """CPU: the host side of the depth filter -- graph.gate_depths against the golden graphs' XML,
 match_depth on hand-worked records, shallowest_matches over a stand-in engine, the argument checks
-that need no device, and the header's constants and declarations."""
+that need no device, and the header's constants and declarations.  Also the host reference the GPU
+tests filter with (tests/_enum_support.py): record_depths against match_depth, the pruning shortcuts
+against the minimum over every ordering row, and the brute-force feasible count against the CPU
+oracle."""
 import ctypes as C
 import glob
 import os
@@ -10,6 +13,7 @@ import xml.etree.ElementTree as ET
 import numpy as np
 import pytest
 
+import _enum_support as E
 import _support as S
 import sboxgates_b200 as sb
 from sboxgates_b200 import graph, native
@@ -144,3 +148,82 @@ def test_header_declares_the_depth_filter():
     # the new entry points appear in the cursor-lifetime list
     lifetime = header[header.index("Cursor lifetime:"):header.index("Without a cursor")]
     assert "sbg_enum_depth_counts" in lifetime and "sbg_enum_set_depth" in lifetime
+
+
+def _records(width, gates):
+    recs = np.zeros(len(gates), dtype=sb.MATCH_DTYPE)
+    recs["width"] = width
+    recs["gates"][:, :width] = gates
+    return recs
+
+
+@pytest.mark.parametrize("width", [3, 5, 7])
+def test_record_depths_equal_match_depth(width):
+    rs = np.random.RandomState(width)
+    depth = rs.randint(0, native.SBG_MAX_DEPTH + 1, 40)
+    depth[:8] = rs.choice([0, 1, native.SBG_MAX_DEPTH], 8)
+    recs = _records(width, np.array([rs.choice(40, width, replace=False) for _ in range(500)]))
+    got = E.record_depths(recs, depth)
+    assert [int(x) for x in got] == [sb.match_depth(r, depth) for r in recs]
+    assert E.record_depths(recs[:0], depth).shape == (0,)
+
+
+@pytest.mark.parametrize("width", [3, 5, 7])
+def test_bound_shortcuts_equal_every_ordering(width):
+    """The kernels prune a gate set unless no gate has depth >= B and at most two (width 5) or one
+    (width 7) have depth B - 1; that must be exactly 'some ordering row has depth <= B', the
+    minimum of match_depth over the 10 rows of order5_rows / 70 rows of order7_rows."""
+    rows = {3: [[0, 1, 2]], 5: S.order5_rows(), 7: S.order7_rows()}[width]
+    assert len(rows) == {3: 1, 5: 10, 7: 70}[width]
+    recs = _records(width, np.array(rows))
+    rs = np.random.RandomState(50 + width)
+    seen = set()
+    for i in range(3000):
+        hi = 4 if i % 2 else 1022
+        d = rs.randint(0, hi + 1, width)
+        if i % 3 == 0:   # gates concentrated on the edges of a bound
+            b = int(rs.randint(2, 1023))
+            d = rs.choice([b - 2, b - 1, b], width)
+        best = int(E.record_depths(recs, d).min())
+        if width > 3:   # the closed form the pruning rests on
+            s = sorted(d, reverse=True)
+            assert best == max(2 + int(s[{5: 2, 7: 1}[width]]), 1 + int(s[0]))
+        for bound in {0, best - 2, best - 1, best, best + 1, int(rs.randint(0, 1024))}:
+            if bound < 0:
+                continue
+            ok = bool(E.bound_admits(d, bound, width))
+            assert ok == (best <= bound), (d, bound, best)
+            seen.add((ok, int(np.sum(d == bound - 1))))
+    # both sides of the count rule occur: the largest count kept and the smallest dropped
+    keep_max = {3: 3, 5: 2, 7: 1}[width]
+    assert (True, keep_max) in seen
+    if width > 3:
+        assert (False, keep_max + 1) in seen
+
+
+def _feasible_state(n, seed):
+    """A seeded state whose target is a planted 5-LUT circuit, under a mux mask of depth 1 - 3."""
+    tabs = S.synthetic_state(n, seed=seed)
+    rs = np.random.RandomState(seed)
+    fixed = [(int(b), int(rs.randint(0, 2))) for b in rs.choice(8, 1 + seed % 3, replace=False)]
+    inb = [b for b, _ in fixed]
+    g = [int(x) for x in rs.choice([x for x in range(n) if x not in inb], 5, replace=False)]
+    tgt = S.lut_table(int(rs.randint(1, 255)), S.lut_table(int(rs.randint(1, 255)), tabs[g[0]],
+                      tabs[g[1]], tabs[g[2]]), tabs[g[3]], tabs[g[4]])
+    return tabs, tgt, S.mux_mask(fixed), inb
+
+
+@pytest.mark.parametrize("n,seed", [(12, 3), (16, 4), (18, 5), (20, 6)])
+def test_feasible5_brute_force_equals_oracle(n, seed):
+    """With the loosest bound the brute force counts what search_5lut's enumeration reports as
+    feasible (the CPU oracle); tighter bounds only ever drop combinations."""
+    tabs, tgt, mask, inb = _feasible_state(n, seed)
+    order = E.orders(seed)[0]
+    _, _, feasible = E.oracle_enum5(tabs, tgt, mask, inb, order, 0)
+    depth = np.random.RandomState(seed).randint(0, native.SBG_MAX_DEPTH + 1, n)
+    assert E.feasible5_under_bound(tabs, tgt, mask, inb, depth, sb.SBG_DEPTH_BINS - 1) == feasible
+    assert feasible > 0
+    small = np.random.RandomState(seed).randint(0, 4, n)
+    got = [E.feasible5_under_bound(tabs, tgt, mask, inb, small, b) for b in range(7)]
+    assert got[0] == got[1] == 0 and got[-1] == feasible
+    assert got == sorted(got)

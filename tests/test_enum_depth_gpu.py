@@ -1,7 +1,9 @@
 """GPU: the depth filter of the enumerations (sbg_enum_set_depth / sbg_enum_depth_counts).  Under a
 filter, sbg_enum3/5/7 must enumerate exactly the unfiltered matches of depth <= max_depth, in the
 same order with the same records: checked against a full unfiltered fetch filtered on the host,
-against the CPU oracle's keys, across shares, and on planted circuits at n = 128."""
+against the CPU oracle's keys, across shares, and on planted circuits at n = 128.  CASES run every
+filtered kernel form (width 3, 5, 7 at NW = 1, 2, 4, 8 words per table); the edges of the filter
+are in test_enum_depth_edges_gpu.py."""
 import ctypes as C
 
 import numpy as np
@@ -40,12 +42,33 @@ def _state(n, mask_spec, inb, seed, width):
         outer = S.lut_table(f[0], tabs[g[0]], tabs[g[1]], tabs[g[2]])
         mid = tabs[g[3]] if width == 5 else S.lut_table(f[1], tabs[g[3]], tabs[g[4]], tabs[g[5]])
         tgt = S.lut_table(f[2], outer, mid, tabs[g[-1]])
-    return tabs, tgt, S.mux_mask(MUX[mask_spec]), inb
+    return tabs, tgt, _mask(mask_spec, seed), inb
 
 
-# (width, n, mux depth, excluded inputs, seed)
+def _mask(spec, seed):
+    """A mux mask of depth `spec` (0 - 3: 256 >> spec positions), or "r<count>": a seeded random mask
+    of that many positions, whose last 32-bit word is partly padding."""
+    if not isinstance(spec, str):
+        return S.mux_mask(MUX[spec])
+    rs = np.random.RandomState(1000 + seed)
+    mask = np.zeros(4, dtype=np.uint64)
+    for p in rs.choice(256, int(spec[1:]), replace=False):
+        mask[p >> 6] |= np.uint64(1) << np.uint64(p & 63)
+    return mask
+
+
+def _nw(mask):
+    """The library's 32-bit words per compressed table for a mask: 1, 2, 4 or 8."""
+    m = sum(bin(int(w)).count("1") for w in mask)
+    return 1 if m <= 32 else 2 if m <= 64 else 4 if m <= 128 else 8
+
+
+# (width, n, mask: mux depth or random "r<positions>", excluded inputs, seed).  Every width meets
+# every word count NW (mux depth 3, 2, 1, 0 -> NW 1, 2, 4, 8) and one padded random mask.
 CASES = [(3, 24, 2, [], 11), (3, 40, 3, [], 12), (5, 12, 2, [0], 13), (5, 16, 3, [], 14),
-         (5, 20, 1, [2], 15), (7, 10, 2, [0], 16), (7, 12, 1, [], 17), (7, 14, 2, [1], 18)]
+         (5, 20, 1, [2], 15), (7, 10, 2, [0], 16), (7, 12, 1, [], 17), (7, 14, 2, [1], 18),
+         (3, 32, 1, [], 19), (3, 20, 0, [], 20), (3, 28, "r65", [1], 21), (5, 14, 0, [], 22),
+         (5, 16, "r200", [0], 23), (7, 12, 3, [1], 36), (7, 12, 0, [0], 33), (7, 12, "r33", [], 30)]
 
 
 def _load(engine, case):
@@ -66,19 +89,6 @@ def _run(engine, width, orders, k, count=True):
     return fn(*orders, k, count)
 
 
-def _depths(recs, depth):
-    """match_depth of every record, vectorised."""
-    if len(recs) == 0:
-        return np.zeros(0, dtype=np.int64)
-    w = int(recs["width"][0])
-    d = np.asarray(depth, dtype=np.int64)[recs["gates"][:, :w].astype(np.int64)]
-    if w == 3:
-        return 1 + d.max(axis=1)
-    if w == 5:
-        return 1 + np.maximum(1 + d[:, :3].max(axis=1), d[:, 3:].max(axis=1))
-    return 1 + np.maximum(np.maximum(1 + d[:, :3].max(axis=1), 1 + d[:, 3:6].max(axis=1)), d[:, 6])
-
-
 def _all(engine, width, orders):
     e = _run(engine, width, orders, 0)
     assert e.total <= FULL_CAP
@@ -94,7 +104,17 @@ def _random_depth(n, seed):
     return np.random.RandomState(seed).randint(0, 7, n).astype(np.uint16)
 
 
-@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%d" % c[:3])
+def test_cases_cover_every_filtered_form():
+    """Each of the 12 (width, NW) forms of the filtered kernels meets the host reference in CASES,
+    and each width also runs a random mask whose last 32-bit word is partly padding."""
+    forms = {(c[0], _nw(_mask(c[2], c[4]))) for c in CASES}
+    assert forms == {(w, nw) for w in (3, 5, 7) for nw in (1, 2, 4, 8)}
+    padded = {c[0] for c in CASES if isinstance(c[2], str)
+              and sum(bin(int(x)).count("1") for x in _mask(c[2], c[4])) % 32 != 0}
+    assert padded == {3, 5, 7}
+
+
+@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%s" % c[:3])
 def test_filter_equals_post_filter(engine, case):
     width = case[0]
     _, orders = _load(engine, case)
@@ -102,7 +122,7 @@ def test_filter_equals_post_filter(engine, case):
     full = _all(engine, width, orders)
     assert len(full) > 0
     depth = _random_depth(case[1], case[4])
-    dep = _depths(full, depth)
+    dep = E.record_depths(full, depth)
     engine.set_depth_filter(depth, sb.SBG_DEPTH_BINS - 1)
     e = _run(engine, width, orders, 50)
     assert e.total == len(full)
@@ -140,7 +160,7 @@ def _key_depth(width, key, depth, n, orders, tuples):
     return 1 + max(1 + max(d[:3]), 1 + max(d[3:6]), d[6])
 
 
-@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%d" % c[:3])
+@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%s" % c[:3])
 def test_filtered_keys_match_oracle(engine, case):
     width, n = case[0], case[1]
     (tabs, tgt, mask, inb), orders = _load(engine, case)
@@ -163,7 +183,7 @@ def test_filtered_keys_match_oracle(engine, case):
         assert [int(k) for k in got["key"]] == [k for k, d in zip(keys, kd) if d <= bound]
 
 
-@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%d" % c[:3])
+@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%s" % c[:3])
 def test_neutral_filter_changes_nothing(engine, case):
     width, n = case[0], case[1]
     _, orders = _load(engine, case)
@@ -186,7 +206,7 @@ def test_neutral_filter_changes_nothing(engine, case):
         assert engine.search7(*orders).key == key
 
 
-@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%d" % c[:3])
+@pytest.mark.parametrize("case", CASES, ids=lambda c: "w%d-n%d-m%s" % c[:3])
 def test_excluded_gate_and_count_free(engine, case):
     width, n = case[0], case[1]
     _, orders = _load(engine, case)
