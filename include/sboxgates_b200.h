@@ -191,7 +191,9 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
    installed list.  *total = its length.  The in-process counterpart of the all-gather
    (lut.c:329-349). */
 int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total);
-/* 7-LUT phase 2 over list indices congruent to part modulo nparts. */
+/* 7-LUT phase 2 over list indices congruent to part modulo nparts.  sbg_finish7 decodes any part's
+   key against the installed list; it reuses the entries sbg_decomp7_part returned with its key only
+   while that list is still installed. */
 int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t *key);
 int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,

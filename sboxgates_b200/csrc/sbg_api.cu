@@ -1161,6 +1161,15 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
   return SBG_OK;
 }
 
+// Every install or drop of a lane's 7-LUT list goes through here.  The key and list entries the last
+// sbg_decomp7_part left behind belong to the list it searched, so any change of the list forgets them
+// (sbg_finish7 would otherwise decode an equal key of the new list with the old list's entries).
+void set_list(sbg_lane &L, uint32_t count, bool ready) {
+  L.list_count = count;
+  L.list_ready = ready;
+  L.last_key = SBG_KEY_NONE;
+}
+
 int check_job(sbg_handle *h, const sbg_job *job) {
   if (job->slot < 0 || job->slot >= kSlots || !h->slots[job->slot].ready) {
     return fail(h, SBG_ERR_STATE, "slot %d holds no problem", job->slot);
@@ -1213,8 +1222,7 @@ int redo_search7_steps(sbg_handle *h, sbg_lane &L, const uint8_t *outer, const u
   int rc;
   uint32_t keep = 0;
   if ((rc = run_filter7(h, L, 0, 1, &keep, hit_buffer_overflowed)) != SBG_OK) return rc;
-  L.list_count = keep;
-  L.list_ready = true;
+  set_list(L, keep, true);
   L.seq++;
   CallInputs in;
   in.outer = outer;
@@ -1276,8 +1284,7 @@ int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, sbg_node_resul
           o->overflow[2] == 1)) != SBG_OK) return rc;
       swept7 = h->swept;
     }
-    L.list_count = (uint32_t)o->feasible[2];
-    L.list_ready = true;
+    set_list(L, (uint32_t)o->feasible[2], true);
     if ((rc = finish7_slot(h, hp, o->key[2], job->outer7, job->middle7, o->tuple, o->tuple_prev,
         o->feasible[2], swept7, &res->r7)) != SBG_OK) return rc;
     if (res->r7.found) res->found_stage = 7;
@@ -1473,8 +1480,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   if (WIDTH == 7 && !L.list_ready) {
     uint32_t count = 0;
     if ((rc = run_filter7(h, L, 0, 1, &count)) != SBG_OK) return rc;
-    L.list_count = count;
-    L.list_ready = true;
+    set_list(L, count, true);
   } else {
     L.seq++;
     if ((rc = enqueue_begin(h, L, flags, begin_in, 0)) != SBG_OK) return rc;
@@ -2036,8 +2042,7 @@ int sbg_use_problem(sbg_handle *h, int slot) {
   if (!h->slots[slot].ready) return fail(h, SBG_ERR_STATE, "slot %d holds no problem", slot);
   h->cur_slot = slot;
   h->problem_ready = true;
-  h->lane[0].list_ready = false;
-  h->lane[0].list_count = 0;
+  set_list(h->lane[0], 0, false);
   return SBG_OK;
 }
 
@@ -2121,7 +2126,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
   uint32_t keep = 0;
-  L.list_ready = false;
+  set_list(L, L.list_count, false);
   if ((rc = run_filter7(h, L, part, nparts, &keep)) != SBG_OK) return rc;
   for (int i = 0; i < 4; i++) h->last_ms[i] = L.ms[i];
   *count = (int)keep;
@@ -2133,8 +2138,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   }
   // The part's own ordered list stays on the device; when it is the whole space (nparts == 1) it
   // IS the list, and phase 2 may follow without sbg_set_list7().
-  L.list_count = keep;
-  L.list_ready = nparts == 1;
+  set_list(L, keep, nparts == 1);
   return SBG_OK;
 }
 
@@ -2169,8 +2173,7 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
   const cudaError_t e = launch(h, k_merge_runs, grid, 256, 0, L.stream, false, runs,
       (unsigned long long)stride, rcnt, nruns, L.d_sorted, (unsigned int)SBG_LIST_CAP, L.d_ctl);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_merge_runs: %s", cudaGetErrorString(e));
-  L.list_count = (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP);
-  L.list_ready = true;
+  set_list(L, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP), true);
   return SBG_OK;
 }
 
@@ -2351,7 +2354,7 @@ int sbg_search_node(sbg_handle *h, const sbg_job *job, sbg_node_result *res) {
   in.outer = job->outer7;
   in.middle = job->middle7;
   in.gate_order = job->gate_order;
-  L.list_ready = false;
+  set_list(L, L.list_count, false);
   if ((rc = enqueue_chain(h, L, job->flags, in)) != SBG_OK) return rc;
   const double t1 = wall_now();
   if ((rc = collect_chain(h, L, job, res)) != SBG_OK) return rc;
@@ -2396,7 +2399,7 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
       in.outer = job.outer7;
       in.middle = job.middle7;
       in.gate_order = job.gate_order;
-      L.list_ready = false;
+      set_list(L, L.list_count, false);
       if ((rc = enqueue_chain(h, L, job.flags, in)) != SBG_OK) {
         h->concurrent = false;
         return rc;

@@ -190,6 +190,143 @@ def enum3_range(tables, target, mask, order, max_keys, lo=0, hi=None, piece=None
     return sum(p[0] for p in parts), keys
 
 
+# ------------------------------------------------------------------------------------------------
+# search_7lut's phase 2 on the host: orc_decomp7_key over pieces of a list, per entry and per part,
+# and the sbg_result fields a key must come with.
+
+class _List7:
+    """The pointers orc_decomp7_key takes for one (state, list, orders), marshalled once."""
+
+    def __init__(self, tables, target, mask, tuples, outer, middle):
+        self.tables, self.tp = S._u64(tables)
+        self.target, self.gp = S._u64(target)
+        self.mask, self.mp = S._u64(mask)
+        self.lst = np.ascontiguousarray(tuples, dtype=np.uint16).reshape(-1, 7)
+        self.outer, self.middle = S._order(outer), S._order(middle)
+
+    def key(self, part, nparts, lo=0, hi=None):
+        """orc_decomp7_key(part, nparts) of entries [lo, hi) (hi <= the list's length), full-list
+        indices.  The list handed over starts at entry lo - 1, whose row 69 leaves the outer cache
+        that entry lo begins with; entry lo - 1 itself is not decided."""
+        hi = self.lst.shape[0] if hi is None else hi
+        base = max(lo - 1, 0)
+        sub = self.lst[base:hi]
+        first = lo - base + (part - lo) % nparts   # the first entry >= lo of index part (mod nparts)
+        key = int(S.oracle_lib().orc_decomp7_key(self.tp, self.gp, self.mp,
+                                                 sub.ctypes.data_as(u16p), sub.shape[0],
+                                                 self.outer, self.middle, first, nparts))
+        return key if key == NONE else key + (base << 23)
+
+
+def decomp7_range(tables, target, mask, tuples, outer, middle, lo, hi):
+    """The oracle's first key over list entries [lo, hi) with full-list indices (orc_decomp7_key of
+    the whole list restricted to those entries; the outer cache on entry to lo comes from lo - 1)."""
+    lst = _List7(tables, target, mask, tuples, outer, middle)
+    hi = min(hi, lst.lst.shape[0])
+    return NONE if lo >= hi else lst.key(0, 1, lo, hi)
+
+
+def decomp7_key(tables, target, mask, tuples, outer, middle, piece=8):
+    """orc_decomp7_key of the whole list: slices of `piece` entries, a batch (one per worker) at a
+    time in list order, stopping after the first batch that holds a match."""
+    lst = _List7(tables, target, mask, tuples, outer, middle)
+    rs = pieces(0, lst.lst.shape[0], piece)
+    w = workers()
+    with ThreadPoolExecutor(max_workers=w) as pool:
+        for b in range(0, len(rs), w):
+            keys = list(pool.map(lambda r: lst.key(0, 1, r[0], r[1]), rs[b:b + w]))
+            if min(keys) != NONE:
+                return min(keys)
+    return NONE
+
+
+def decomp7_entry_keys(tables, target, mask, tuples, outer, middle):
+    """Every entry's own first key: orc_decomp7_key(part=p, nparts=len(list)) for each p (the
+    entry's predecessor still sets its outer cache), on the pool."""
+    lst = _List7(tables, target, mask, tuples, outer, middle)
+    count = lst.lst.shape[0]
+    with ThreadPoolExecutor(max_workers=workers()) as pool:
+        return list(pool.map(lambda p: lst.key(p, count), range(count)))
+
+
+def part_keys(entry_keys, nparts):
+    """Part p's key of decomp7_part(p, nparts) from the entries' own keys: the minimum over the
+    entries of index p (mod nparts) (NONE for an empty part)."""
+    return [min(entry_keys[p::nparts], default=NONE) for p in range(nparts)]
+
+
+def planted7(tables, gates, k, fo, fm, fi, stale_gate=None):
+    """Target fi(fo(outer), fm(middle), last) on ordering row k of the 7 gates; the outer LUT reads
+    stale_gate in place of its first input when given (what a stale-cache row computes)."""
+    row = S.order7_rows()[k]
+    g = [int(gates[row[i]]) for i in range(7)]
+    a = g[0] if stale_gate is None else stale_gate
+    return S.lut_table(int(fi), S.lut_table(int(fo), tables[a], tables[g[1]], tables[g[2]]),
+                       S.lut_table(int(fm), tables[g[3]], tables[g[4]], tables[g[5]]), tables[g[6]])
+
+
+def stale_pairs(rs, n, count, lo=1):
+    """count pairs (0, a1..a4, t1, t2) < (0, t1, t2, ...) that follow each other in list order, the
+    a's of each pair above the t1 of the pair before and the first a at least lo: the second entry
+    of a pair runs rows 0-3 on the outer tables the first one's row 69 left (gates a1, t1, t2)."""
+    out, floor = [], lo
+    for j in range(count):
+        room = (n - 6 - floor - 4) // (count - j)   # values left for this pair's a's and t1
+        assert room >= 1, (n, count, lo)
+        t1 = floor + 4 + int(rs.randint(room))
+        head = sorted(int(x) for x in rs.choice(np.arange(floor, t1), 4, replace=False))
+        rest = sorted(int(x) for x in rs.choice(np.arange(t1 + 2, n), 4, replace=False))
+        out += [[0] + head + [t1, t1 + 1], [0, t1, t1 + 1] + rest]
+        floor = t1 + 1
+    return out
+
+
+def stale_source(tuples, idx, k):
+    """The gate the reference's outer cache holds in place of row k's first gate at entry idx, or
+    None: rows 0-3 (outer = first three gates) of an entry whose first gate is 0 keep the outer
+    tables of the previous entry's row 69 (outer = its gates 1, 5, 6) when that entry ends in this
+    one's gates 1 and 2 (the cache key drops the first gate)."""
+    if idx == 0 or k >= 4:
+        return None
+    t, prev = tuples[idx], tuples[idx - 1]
+    if t[0] == 0 and prev[5] == t[1] and prev[6] == t[2]:
+        return int(prev[1])
+    return None
+
+
+def expected_result7(key, tuples, tables, target, mask, outer, middle):
+    """The sbg_result fields (a dict) the 7-LUT key `key` over the list `tuples` must come with, from
+    the oracle's ordering rows and inner solver; None for SBG_KEY_NONE or a key that does not
+    decompose."""
+    if key == NONE:
+        return None
+    idx, k, po, pm = key >> 23, (key >> 16) & 0x7F, (key >> 8) & 0xFF, key & 0xFF
+    lst = np.asarray(tuples, dtype=np.uint16).reshape(-1, 7)
+    row = S.order7_rows()[k]
+    gates = [int(lst[idx][row[i]]) for i in range(7)]
+    fo, fm = int(outer[po]), int(middle[pm])
+    sub = stale_source(lst, idx, k)
+    a = gates[0] if sub is None else sub
+    t1 = S.lut_table(fo, tables[a], tables[gates[1]], tables[gates[2]])
+    t2 = S.lut_table(fm, tables[gates[3]], tables[gates[4]], tables[gates[5]])
+    arrs = [S._u64(x) for x in (t1, t2, tables[gates[6]], target, mask)]
+    fi, seen = C.c_uint8(), C.c_uint8()
+    if not S.oracle_lib().orc_solve_inner(*[x[1] for x in arrs], C.byref(fi), C.byref(seen)):
+        return None
+    return dict(found=1, key=key, index=idx, ordering=k, pos_outer=po, pos_middle=pm,
+                func_outer=fo, func_middle=fm, func_inner=int(fi.value),
+                inner_seen=int(seen.value), gates=gates, stale_outer=int(sub is not None))
+
+
+def result7_fields(res):
+    """The fields of an sbg_result (SbgResult) that expected_result7 gives, as a dict."""
+    out = {f: int(getattr(res, f)) for f in ("found", "key", "index", "ordering", "pos_outer",
+                                              "pos_middle", "func_outer", "func_middle",
+                                              "func_inner", "inner_seen", "stale_outer")}
+    out["gates"] = [int(g) for g in res.gates[:7]]
+    return out
+
+
 def comb_rank(n, t, comb):
     """Lexicographic rank of a t-subset of {0..n-1} (orc_combination_rank)."""
     c = (C.c_uint16 * t)(*[int(x) for x in comb])
