@@ -125,6 +125,8 @@ struct sbg_lane {
   uint32_t *d_tcount = nullptr;  // hits per ticket
   uint32_t *d_toffset = nullptr; // their exclusive prefix sum
   uint32_t *d_gcount = nullptr;  // hits per group of 1,024 tickets
+  uint64_t *d_sieve3 = nullptr;  // phase 1's pair sieve per 3-gate prefix (k_sieve3)
+  uint64_t sieve3_entries = 0;
   size_t hits_cap = 0;
   size_t tickets_alloc = 0;
   cudaEvent_t ev[8] = {};        // timing (only with sbg_set_timing)
@@ -375,8 +377,9 @@ constexpr int kSinglePrefixMaxGates = 72;
 constexpr int kShiftMaxGates = 60;
 // Phase 1's pair sieve (shifted windows) above this many masked positions (SBG_SIEVE=0|1|2
 // overrides).  On one H100 at n = 40 it took the launches under 256 / 128 / 64 positions from
-// 0.393 / 0.277 / 0.231 ms to 0.264 / 0.231 / 0.212 ms; under 32 positions the cell loop visits
-// about 10 positions per chunk, no more than the sieve's per-prefix set-up saves (0.220 -> 0.223 ms).
+// 0.393 / 0.277 / 0.231 ms to 0.264 / 0.231 / 0.212 ms (0.212 / 0.199 / 0.212 ms with its pairs
+// built once per 3-gate prefix, k_sieve3); under 32 positions the cell loop visits about 10
+// positions per chunk, fewer than the sieve and its table cost (0.220 -> 0.249 ms forced on).
 constexpr int kSieveMinPositions = 32;
 // Phase-1 prefixes per ticket (4-gate prefixes, n <= kSinglePrefixMaxGates) while several chains
 // share the device (sbg_search_batch).
@@ -511,6 +514,20 @@ int ensure_tickets(sbg_handle *h, sbg_lane &L, uint64_t tickets) {
   SBG_CUDA(h, cudaMalloc(&L.d_toffset, want * sizeof(uint32_t)));
   SBG_CUDA(h, cudaMalloc(&L.d_gcount, (want / kTicketGroup + 2) * sizeof(uint32_t)));
   L.tickets_alloc = want;
+  return SBG_OK;
+}
+
+// The k_sieve3 table for n gates: C(n - 4, 3) entries of kSieve3Words words, 7.3 MB at n = 40,
+// 28.4 MB at n = 60 (the shifted windows' limit).  Entry ranks do not depend on n, so a table
+// allocated for a larger n serves every smaller one.
+int ensure_sieve3(sbg_handle *h, sbg_lane &L, int n) {
+  const uint64_t entries = h_binom[n - 4][3];
+  if (L.d_sieve3 != nullptr && L.sieve3_entries >= entries) return SBG_OK;
+  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
+  cudaFree(L.d_sieve3);
+  L.d_sieve3 = nullptr;
+  SBG_CUDA(h, cudaMalloc(&L.d_sieve3, entries * kSieve3Words * sizeof(uint64_t)));
+  L.sieve3_entries = entries;
   return SBG_OK;
 }
 
@@ -767,9 +784,11 @@ FilterPlan plan_filter(const sbg_handle *h, const sbg_lane &L, const sbg_handle:
                                    : plan_filter_p<4>(h, L, hp, nparts, retry, seg_base);
 }
 
+// build_sieve3: the sieve's form first fills the lane's k_sieve3 table; a later launch of the same
+// search (the next segment, the overflow retry) finds it filled.
 template <int P>
 int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int part, int nparts,
-    unsigned long long list_cap) {
+    unsigned long long list_cap, bool build_sieve3) {
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const int n = hp.n;
   const int m = hp.m;
@@ -794,12 +813,22 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
           list_cap, (int)fp.batch, fp.max_warps,
           pl.all ? (unsigned long long)fp.total : pl.t_offset, pl.items, std::max(1, pl.chunks),
           (unsigned long long)fp.chunk_tickets, (unsigned long long)fp.seg_base,
-          h->opt_packed ? 15 : 0, fp.wt);
+          h->opt_packed ? 15 : 0, fp.wt, (const uint64_t *)L.d_sieve3);
       if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_filter7_pm: %s", cudaGetErrorString(e));
       return SBG_OK;
     };
     if constexpr (P == 4) {
-      if (shifted && sieve) return run(k_filter7_pm<NW, 1, P, true, true, true>, true, true);
+      if (shifted && sieve) {
+        if (build_sieve3) {
+          int rc;
+          if ((rc = ensure_sieve3(h, L, n)) != SBG_OK) return rc;
+          const int grid = (int)((h_binom[n - 4][3] + kWarpsPerCta - 1) / kWarpsPerCta);
+          const cudaError_t e = launch(h, k_sieve3<NW>, grid, kThreads, 0, L.stream, !h->timing,
+              h->d_slots + L.slot, (const DevCtl *)L.d_ctl, L.d_sieve3);
+          if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_sieve3: %s", cudaGetErrorString(e));
+        }
+        return run(k_filter7_pm<NW, 1, P, true, true, true>, true, true);
+      }
       // one word of 31 candidate gates from the first possible g on
       if (shifted) return run(k_filter7_pm<NW, 1, P, true, true, false>, true, false);
     }
@@ -813,12 +842,13 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
 
 // Phase 1 on lane L: the filter, then the ordered, capped list in L.d_sorted (ctl->list_count).
 // The caller has enqueued k_begin (which cleared fp.tickets_cap / kTicketGroup + 1 group counters).
-int enqueue_filter7(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int part, int nparts) {
+int enqueue_filter7(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int part, int nparts,
+    bool build_sieve3) {
   int rc;
   if (h->timing) cudaEventRecord(L.ev[0], L.stream);
   const unsigned long long room = (unsigned long long)SBG_LIST_CAP - fp.list_base;
-  rc = fp.five ? launch_filter7_pm_p<5>(h, L, fp, part, nparts, room)
-               : launch_filter7_pm_p<4>(h, L, fp, part, nparts, room);
+  rc = fp.five ? launch_filter7_pm_p<5>(h, L, fp, part, nparts, room, build_sieve3)
+               : launch_filter7_pm_p<4>(h, L, fp, part, nparts, room, build_sieve3);
   if (rc != SBG_OK) return rc;
   if (h->timing) cudaEventRecord(L.ev[1], L.stream);
   const uint64_t groups = (fp.tickets_cap + kTicketGroup - 1) / kTicketGroup;
@@ -912,7 +942,9 @@ int run_filter7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint32_t *coun
     CallInputs none;
     if ((rc = enqueue_begin(h, L, kBeginSearch7 | kBeginRows, none,
         (uint32_t)(fp.tickets_cap / kTicketGroup + 1))) != SBG_OK) return rc;
-    if ((rc = enqueue_filter7(h, L, fp, part, nparts)) != SBG_OK) return rc;
+    // the sieve's table once per search; the fused chain that overflowed has built it already
+    const bool first_launch = seg_base == 0 && overflows == 0 && !overflowed_already;
+    if ((rc = enqueue_filter7(h, L, fp, part, nparts, first_launch)) != SBG_OK) return rc;
     if ((rc = fetch_ctl(h, L)) != SBG_OK) return rc;
     if (h->timing) {
       ms_filter += elapsed(L.ev[0], L.ev[1]);
@@ -1154,7 +1186,7 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
   if ((flags & kBeginSearch5) && !over()
       && (rc = enqueue_search5(h, L, 0, 1, search5_two_kernels(h, hp.n))) != SBG_OK) return rc;
   if ((flags & kBeginSearch7) && !over()) {
-    if ((rc = enqueue_filter7(h, L, fp, 0, 1)) != SBG_OK) return rc;
+    if ((rc = enqueue_filter7(h, L, fp, 0, 1, true)) != SBG_OK) return rc;
     if (!over() && (rc = enqueue_decomp7(h, L, 0, 1, SBG_LIST_CAP)) != SBG_OK) return rc;
   }
   record_done(h, L);
@@ -1944,7 +1976,7 @@ void sbg_destroy(sbg_handle *h) {
       sbg_lane &L = h->lane[i];
       cudaFree(L.d_ctl); cudaFree(L.d_par7); cudaFree(L.d_pos5); cudaFree(L.d_order3);
       cudaFree(L.d_hits); cudaFree(L.d_aux); cudaFree(L.d_sorted);
-      cudaFree(L.d_tcount); cudaFree(L.d_toffset); cudaFree(L.d_gcount);
+      cudaFree(L.d_tcount); cudaFree(L.d_toffset); cudaFree(L.d_gcount); cudaFree(L.d_sieve3);
       cudaFree(L.d_ectl); cudaFree(L.d_ecount); cudaFree(L.d_eoffset); cudaFree(L.d_ematch);
       cudaFree(L.d_pranks); cudaFree(L.d_pslots); cudaFree(L.d_ptickets); cudaFree(L.d_pfirst);
       cudaFree(L.d_bsums); cudaFree(L.d_delta); cudaFree(L.d_gsums); cudaFree(L.d_ehist);

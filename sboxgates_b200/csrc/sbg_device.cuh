@@ -17,8 +17,11 @@
 // per-launch DRAM traffic is the 16.5 KB problem block plus the hit list.
 #pragma once
 
-#if defined(SBG_COUNT_STAGE1) || defined(SBG_COUNT_FILTER)
+#if defined(SBG_COUNT_STAGE1) || defined(SBG_COUNT_FILTER) || defined(SBG_TIME_FILTER)
 #include <cstdio>
+#endif
+#if defined(SBG_COUNT_FILTER) && defined(SBG_TIME_FILTER)
+#error "SBG_COUNT_FILTER and SBG_TIME_FILTER share the control block's spare words"
 #endif
 #include <cuda_pipeline.h>
 #include <cuda_runtime.h>
@@ -855,15 +858,135 @@ constexpr int kQuadGates = 7;   // QUAD windows: 7 candidate gates + the target 
 // SIEVE (SH only): a 7-tuple is feasible iff every masked (target 1, target 0) pair of positions is
 // told apart by one of its gates.  Within a mixed cell of the prefix a, b, c and d agree on every
 // such pair, so (e,f,g) must separate all of the cell's pairs; the gates that separate pair
-// (p,q) are S = ~(xr[p] ^ xr[q]) over the gate bits.  Per prefix the warp takes up to 64 such pairs
-// (each position of a mixed cell with the first position of the other target in its cell) and
-// keeps, per warp, S[u] for each pair u and
-// sep[x] = the pairs gate x separates.  A lane with pair (e,f) then only has to intersect its
-// candidate g with S[u] for the pairs u neither e nor f separates -- a necessary condition, usually
-// empty after a few pairs.  Lanes and chunks that keep candidates go through the exact cell loop,
+// (p,q) are S = ~(xr[p] ^ xr[q]) over the gate bits.  Per prefix the warp copies the entry of its
+// first three gates from the k_sieve3 table (below): up to 64 pairs inside the cells of (a, b, c),
+// S[u] for each pair u and sep[x] = the pairs gate x separates.  A lane with pair (e,f) then only
+// has to intersect its candidate g with S[u] for the pairs u none of d, e and f separates -- a
+// necessary condition, usually empty after a few pairs.  Lanes and chunks that keep candidates go through the exact cell loop,
 // seeded with what the sieve left.
 constexpr int kSievePairs = 64;
 constexpr int kSieveWords = 4 * kSievePairs;   // per warp: S[64] and sep[64], 64-bit words
+
+// The sieve's pairs per 3-gate prefix a < b < c <= n - 5, built once per search by k_sieve3 (one
+// warp per prefix) into a table of entries laid out like a warp's s_sieve: S[u] for up to
+// kSievePairs pairs, sep[x] for c < x <= n - 2 (pairs past the last one count as separated, every
+// other sep[x] is all-ones).  Entry C(c,3) + C(b,2) + a (the colex rank, the same for every n).  A
+// pair is a masked position p of a mixed cell of (a, b, c) and the first position of the other
+// target in that cell -- positions in order, the cell's first target-0 position left out (the first
+// target-1 position has that pair) -- so a, b and c agree on it.  A 4-gate prefix (a, b, c, d) copies
+// its entry and drops the pairs d separates: what is left lies inside its own cells, where a, b, c
+// and d agree, and the filter's test per pair is unchanged.  Every 4-gate prefix with the same first
+// three gates used to find the same cells and pairs again.
+constexpr int kSieve3Words = 2 * kSievePairs;   // 64-bit words per entry
+template <int NW>
+__global__ void __launch_bounds__(kThreads) k_sieve3(const DevProblem *__restrict__ prob,
+    const DevCtl *__restrict__ ctl, uint64_t *__restrict__ table) {
+  __shared__ uint64_t s_pairs[kWarpsPerCta][kSievePairs];
+  __shared__ uint64_t s_rows[256];         // position-major rows, gate bits 0..63
+  __shared__ uint32_t s_tabs[NW][64];      // gate-major tables (the sieve's form has n <= 63)
+  __shared__ uint32_t s_T[NW], s_M[NW];
+  wait_for_predecessor();   // the chain's first kernel derives the problem block and its rows
+  if (chain_is_over(ctl) || volatile_load32(&ctl->skip7) != 0) return;
+  const int n = prob->n;
+  const int m = prob->m;
+  const uint32_t inmask = prob->inmask;
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  for (int i = threadIdx.x; i < m; i += kThreads) {
+    s_rows[i] = *reinterpret_cast<const uint64_t *>(&prob->xr[i][0]);
+  }
+  for (int i = threadIdx.x; i < NW * 64; i += kThreads) {
+    s_tabs[i >> 6][i & 63] = (i & 63) < n ? prob->tabs[i >> 6][i & 63] : 0u;
+  }
+  if (threadIdx.x < NW) {
+    s_T[threadIdx.x] = prob->T[threadIdx.x];
+    s_M[threadIdx.x] = prob->M[threadIdx.x];
+  }
+  const uint64_t gmask = (1ull << n) - 1u;   // gate bits: no target bit, no padding
+  const uint64_t total = c_binom[n - 4][3];
+  __syncthreads();
+  for (uint64_t t = (uint64_t)blockIdx.x * kWarpsPerCta + warp; t < total;
+       t += (uint64_t)gridDim.x * kWarpsPerCta) {
+    // colex unranking, one ballot per element and 32 candidates: c = the largest x with C(x,3) <= t,
+    // then b = the largest x with C(x,2) <= t - C(c,3), a = the rest (c <= n - 5 < 66)
+    int pre[3];
+    {
+      const uint64_t x0 = (uint64_t)lane + 3, x1 = x0 + 32;
+      const int c = 2 + __popc(__ballot_sync(kFull, x0 * (x0 - 1) * (x0 - 2) / 6 <= t))
+          + __popc(__ballot_sync(kFull, x1 * (x1 - 1) * (x1 - 2) / 6 <= t));
+      const uint64_t r = t - c_binom[c][3];
+      const uint64_t y0 = (uint64_t)lane + 2, y1 = y0 + 32;
+      const int b = 1 + __popc(__ballot_sync(kFull, y0 * (y0 - 1) / 2 <= r))
+          + __popc(__ballot_sync(kFull, y1 * (y1 - 1) / 2 <= r));
+      pre[0] = (int)(r - c_binom[b][2]);
+      pre[1] = b;
+      pre[2] = c;
+    }
+    bool rejected = false;
+#pragma unroll
+    for (int i = 0; i < 3; i++) rejected |= (pre[i] < 8) && ((inmask >> pre[i]) & 1u);
+    if (rejected) continue;   // no 4-gate prefix the filter works on starts with these gates
+    // lane < 8: cell `lane` (a most significant), its first target-1 and target-0 position
+    bool f1 = false, f0 = false;
+    int rep1 = 0, rep0 = 0;
+#pragma unroll
+    for (int w = 0; w < NW; w++) {
+      uint32_t cw = s_M[w];
+#pragma unroll
+      for (int i = 0; i < 3; i++) {
+        const uint32_t tv = s_tabs[w][pre[i]];
+        cw &= ((lane >> (2 - i)) & 1) ? tv : ~tv;
+      }
+      const uint32_t ones = cw & s_T[w], zeros = cw & ~s_T[w];
+      if (!f1 && ones != 0) rep1 = w * 32 + __ffs(ones) - 1;
+      if (!f0 && zeros != 0) rep0 = w * 32 + __ffs(zeros) - 1;
+      f1 |= ones != 0;
+      f0 |= zeros != 0;
+    }
+    const uint32_t mixed = __ballot_sync(kFull, lane < 8 && f1 && f0);
+    int npairs = 0;
+#pragma unroll
+    for (int w = 0; w < NW; w++) {
+      if (npairs < kSievePairs) {   // warp-uniform
+        const int p = w * 32 + lane;
+        uint32_t cell = 0;
+#pragma unroll
+        for (int i = 0; i < 3; i++) cell = (cell << 1) | ((s_tabs[w][pre[i]] >> lane) & 1u);
+        const bool t1 = ((s_T[w] >> lane) & 1u) != 0;
+        const int r1 = __shfl_sync(kFull, rep1, (int)cell), r0 = __shfl_sync(kFull, rep0, (int)cell);
+        const int q = t1 ? r0 : r1;
+        const bool paired = ((s_M[w] >> lane) & 1u) != 0 && ((mixed >> cell) & 1u) != 0 && (t1 || p != r0);
+        const uint32_t bal = __ballot_sync(kFull, paired);
+        const int u = npairs + __popc(bal & lanemask_lt());
+        if (paired && u < kSievePairs) {
+          s_pairs[warp][u] = ~(s_rows[p] ^ s_rows[q]) & gmask;
+        }
+        npairs = min(kSievePairs, npairs + __popc(bal));
+      }
+    }
+    __syncwarp();
+    const uint64_t s_lo = lane < npairs ? s_pairs[warp][lane] : ~0ull;
+    const uint64_t s_hi = lane + 32 < npairs ? s_pairs[warp][lane + 32] : ~0ull;
+    __syncwarp();
+    // sep[x] for the gates that can be d, e or f, lane x mod 32 keeps it
+    const uint64_t unused = npairs >= kSievePairs ? 0ull : ~0ull << npairs;
+    uint64_t sep_lo = ~0ull, sep_hi = ~0ull;
+    for (int x = pre[2] + 1; x <= n - 2; x++) {
+      const uint32_t lo = __ballot_sync(kFull, ((s_lo >> x) & 1u) != 0);
+      const uint32_t hi = npairs > 32 ? __ballot_sync(kFull, ((s_hi >> x) & 1u) != 0) : 0u;
+      const uint64_t v = (((uint64_t)hi << 32) | lo) | unused;
+      if (lane == (x & 31)) {
+        if (x < 32) sep_lo = v;
+        else sep_hi = v;
+      }
+    }
+    uint64_t *e = table + t * kSieve3Words;
+    e[lane] = s_lo;
+    e[lane + 32] = s_hi;
+    e[kSievePairs + lane] = sep_lo;
+    e[kSievePairs + lane + 32] = sep_hi;
+  }
+}
 // SV: the sieve is compiled in (SH only); without it the shifted form is the plain cell loop.
 template <int NW, int W, int P, bool FS, bool SH = false, bool SV = false>
 __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(const DevProblem *__restrict__ prob,
@@ -872,7 +995,7 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
     unsigned long long tickets_cap, int part, int nparts, unsigned long long list_cap, int batch,
     int max_warps, unsigned long long t_offset, unsigned long long chunk_items,
     int chunks_per_prefix, unsigned long long chunk_tickets, unsigned long long seg_base,
-    int packed_gates, const WeightedTickets wt) {
+    int packed_gates, const WeightedTickets wt, const uint64_t *__restrict__ sieve3) {
   constexpr int K = 7, NC = 1 << P, NP = P == 4 ? 4 : 2;
   extern __shared__ uint32_t smem[];
   __shared__ uint32_t s_wt[4][kWeightedRow];
@@ -907,7 +1030,8 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
   uint32_t *cells = s_xr + ((m * ngw + 3) & ~3) + warp * (NC * NW);
   // per warp: the surviving-g vectors of one chunk, word-major (vs[word * 32 + lane])
   uint32_t *vs = s_xr + ((m * ngw + 3) & ~3) + kWarpsPerCta * (NC * NW) + warp * (ngw * 32);
-  // SV only: the warp's sieve tables, S[u] at s_sieve[u] and sep[x] at s_sieve[kSievePairs + x]
+  // SV only: the warp's copy of its 3-gate prefix's entry of the k_sieve3 table, S[u] at s_sieve[u]
+  // and sep[x] at s_sieve[kSievePairs + x]
   uint64_t *s_sieve = reinterpret_cast<uint64_t *>(s_xr + ((m * ngw + 3) & ~3)
       + kWarpsPerCta * (NC * NW + ngw * 32) + warp * kSieveWords);
   // SH only: the shifted rows for EVERY window base 6 .. n-1 (a prefix's first window starts at its
@@ -993,6 +1117,23 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
   // would be worked on even if the cap was reached meanwhile, doubling the hits in flight.
   const bool ahead = max_warps == 0;
   const int n_allowed = n - __popc(inmask & 0xffu);
+  int sieve_abc = -1;   // SV: the 3-gate prefix whose entry s_sieve holds (9 bits per gate)
+#ifdef SBG_TIME_FILTER
+  // SM clocks per section, summed over the warp's tickets: 0 ticket, unranking and prefix stepping,
+  // 1 mixed cells, 2 sieve pairs, 3 sieve transpose, 4 chunk stepping and sieve, 5 cell loop, 6 emission
+  unsigned long long tf_acc[7] = {0, 0, 0, 0, 0, 0, 0};
+  long long tf_prev = clock64();
+#define SBG_TF_MARK(k)                      \
+  do {                                      \
+    const long long tf_now_ = clock64();    \
+    tf_acc[k] += tf_now_ - tf_prev;         \
+    tf_prev = tf_now_;                      \
+  } while (0)
+#else
+#define SBG_TF_MARK(k) \
+  do {                 \
+  } while (0)
+#endif
   if (ahead) {
 #pragma unroll
     for (int i = 0; i < kDepth; i++) {
@@ -1102,11 +1243,12 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         if (q_begin == 0 && lane == 0) swept_lane += c_binom[n - last - 1][K - P];
         continue;
       }
+      SBG_TF_MARK(0);
 
       // mixed cells of the prefix (cell = lane mod NC, first gate most significant).  With 16 cells
-      // and several table words the two half-warps take half the words each.
-      uint32_t mixed_ballot;
-      {
+      // and several table words the two half-warps take half the words each.  The sieve's form
+      // needs them only for the chunks its pairs leave a candidate in, and finds them there.
+      auto find_mixed_cells = [&]() {
         constexpr bool kSplit = NC == 16 && NW >= 2;
         constexpr int NWH = kSplit ? NW / 2 : NW;
         const bool upper = kSplit && lane >= 16;
@@ -1116,8 +1258,11 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         uint32_t ones = 0, zeros = 0;
 #pragma unroll
         for (int k = 0; k < NWH; k++) {
-          uint32_t tt = upper ? M[kSplit ? k + NWH : k] : M[k];
-          const uint32_t tw = upper ? T[kSplit ? k + NWH : k] : T[k];
+          // SV reads the mask and target words again here: held in registers they would stay live
+          // across the chunk loop
+          const int wk = upper ? k + NWH : k;
+          uint32_t tt = SV ? prob->M[wk] : upper ? M[kSplit ? k + NWH : k] : M[k];
+          const uint32_t tw = SV ? prob->T[wk] : upper ? T[kSplit ? k + NWH : k] : T[k];
 #pragma unroll
           for (int i = 0; i < P; i++) {
             const uint32_t tv = tabs_h[k * npad + pre[i]];
@@ -1132,7 +1277,8 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
           zeros |= __shfl_xor_sync(kFull, zeros, 16);
         }
         const bool mixed = ones != 0 && zeros != 0;   // both halves of a split warp agree
-        mixed_ballot = __ballot_sync(kFull, mixed) & (NC == 32 ? 0xffffffffu : ((1u << (NC & 31)) - 1u));
+        const uint32_t mixed_ballot = __ballot_sync(kFull, mixed)
+            & (NC == 32 ? 0xffffffffu : ((1u << (NC & 31)) - 1u));
         __syncwarp();
         if (mixed) {
           const int slot = __popc(mixed_ballot & ((1u << cell) - 1u));
@@ -1140,71 +1286,31 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
           for (int k = 0; k < NWH; k++) cells[slot * NW + (upper ? NWH : 0) + k] = c[k];
         }
         __syncwarp();
-      }
-      const int mc = __popc(mixed_ballot);
+        return __popc(mixed_ballot);
+      };
+      int mc = SV ? -1 : find_mixed_cells();   // SV: not yet found
+      SBG_TF_MARK(1);
 #ifdef SBG_COUNT_FILTER
       unsigned long long dbg_chunks = 0, dbg_windows = 0, dbg_cells = 0, dbg_pos = 0, dbg_packed = 0;
       unsigned long long dbg_quad = 0, dbg_sieve = 0, dbg_exact = 0;
-      unsigned long long dbg_mc = (unsigned long long)mc;
+      unsigned long long dbg_mc = SV ? 0ull : (unsigned long long)mc;
 #endif
       if constexpr (SV) {
-        {
-          // the sieve's pairs, all mixed cells at once: every masked position p of a mixed cell is
-          // paired with the first position of the other target in its cell (lane j < mc holds those
-          // of mixed cell j), except the first target-0 position, whose pair the first target-1
-          // position already has; positions in order, word by word, up to 64 pairs.  No loop over
-          // cells and no dependent shared-memory round trips per cell.
-          const uint64_t gmask = (1ull << n) - 1u;   // gate bits: no target bit, no padding
-          int rep1 = 0, rep0 = 0;
-          if (lane < mc) {
-            bool f1 = false, f0 = false;
-#pragma unroll
-            for (int w = 0; w < NW; w++) {
-              const uint32_t c = cells[lane * NW + w];
-              const uint32_t a = c & T[w], bq = c & ~T[w];
-              if (!f1 && a != 0) rep1 = w * 32 + __ffs(a) - 1;
-              if (!f0 && bq != 0) rep0 = w * 32 + __ffs(bq) - 1;
-              f1 |= a != 0;
-              f0 |= bq != 0;
-            }
-          }
-          int npairs = 0;
-#pragma unroll
-          for (int w = 0; w < NW; w++) {
-            if (npairs < kSievePairs) {   // warp-uniform
-              const int p = w * 32 + lane;
-              uint32_t cell = 0;
-#pragma unroll
-              for (int i = 0; i < P; i++) cell = (cell << 1) | ((s_tabs[w * npad + pre[i]] >> lane) & 1u);
-              const bool t1 = ((T[w] >> lane) & 1u) != 0;
-              const int slot = __popc(mixed_ballot & ((1u << cell) - 1u));
-              const int r1 = __shfl_sync(kFull, rep1, slot), r0 = __shfl_sync(kFull, rep0, slot);
-              const int q = t1 ? r0 : r1;
-              const bool paired = ((M[w] >> lane) & 1u) != 0 && ((mixed_ballot >> cell) & 1u) != 0
-                  && (t1 || p != r0);
-              const uint32_t bal = __ballot_sync(kFull, paired);
-              const int u = npairs + __popc(bal & lanemask_lt());
-              if (paired && u < kSievePairs) {
-                const uint64_t xp = *reinterpret_cast<const uint64_t *>(s_xr + p * ngw);
-                const uint64_t xq = *reinterpret_cast<const uint64_t *>(s_xr + q * ngw);
-                s_sieve[u] = ~(xp ^ xq) & gmask;
-              }
-              npairs = min(kSievePairs, npairs + __popc(bal));
-            }
-          }
-          __syncwarp();
-          // entries past npairs are stale; their bits are masked below and never read
-          const uint64_t s_lo = s_sieve[lane], s_hi = s_sieve[lane + 32];
-          // sep[x] for the gates that can be e or f; pairs past npairs count as separated, so that
-          // a prefix without mixed cells (npairs = 0) passes everything
-          const uint64_t unused = npairs >= kSievePairs ? 0ull : ~0ull << npairs;
-          for (int x = last + 1; x <= n - 2; x++) {
-            const uint32_t lo = __ballot_sync(kFull, ((s_lo >> x) & 1u) != 0);
-            const uint32_t hi = npairs > 32 ? __ballot_sync(kFull, ((s_hi >> x) & 1u) != 0) : 0u;
-            if (lane == 0) s_sieve[kSievePairs + x] = (((uint64_t)hi << 32) | lo) | unused;
-          }
+        // the 3-gate prefix's entry of the k_sieve3 table, unless s_sieve holds it already (the
+        // two prefixes of a ticket of concurrent chains, consecutive whole prefixes)
+        const int abc = (pre[0] << 18) | (pre[1] << 9) | pre[2];
+        if (abc != sieve_abc) {
+          sieve_abc = abc;
+          const uint64_t rank3 = c_binom[pre[2]][3] + c_binom[pre[1]][2] + (uint64_t)pre[0];
+          const uint4 *src = reinterpret_cast<const uint4 *>(sieve3 + rank3 * kSieve3Words);
+          uint4 *dst = reinterpret_cast<uint4 *>(s_sieve);
+          const uint4 v0 = src[lane], v1 = src[lane + 32];
+          __syncwarp();   // every lane is done with the previous entry
+          dst[lane] = v0;
+          dst[lane + 32] = v1;
           __syncwarp();
         }
+        SBG_TF_MARK(2);
       }
 
       unsigned long long emitted = 0;
@@ -1248,8 +1354,10 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         if constexpr (SV) {
           if (lane_ok) cand = ((1ull << n) - 1u) & (~0ull << (gf + 1)) & ~(uint64_t)(inmask & 0xffu);
           {
-            const uint64_t sepd = s_sieve[kSievePairs + ge] | s_sieve[kSievePairs + gf];
-            // the pairs neither e nor f separates, in two halves taken a pair each per step: two
+            // the pairs d separates are out for the whole prefix
+            const uint64_t sepd = s_sieve[kSievePairs + pre[3]] | s_sieve[kSievePairs + ge]
+                | s_sieve[kSievePairs + gf];
+            // the pairs none of d, e and f separates, in two halves taken a pair each per step: two
             // independent load chains instead of one
             uint32_t u_lo = ~(uint32_t)sepd, u_hi = ~(uint32_t)(sepd >> 32);
 #ifdef SBG_COUNT_FILTER
@@ -1273,8 +1381,16 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
           // (often well above the prefix's last + 3), so that more of them take the packed forms
           const uint32_t lo = __reduce_min_sync(kFull, cand != 0 ? (uint32_t)(__ffsll((long long)cand) - 1)
                                                                  : (uint32_t)n);
+          SBG_TF_MARK(4);
           if (lo >= (uint32_t)n) continue;   // no candidate left in any lane: nothing to test or emit
           first_g = (int)lo;
+          if (mc < 0) {
+            mc = find_mixed_cells();
+            SBG_TF_MARK(1);
+#ifdef SBG_COUNT_FILTER
+            dbg_mc = (unsigned long long)mc;
+#endif
+          }
 #ifdef SBG_COUNT_FILTER
           dbg_exact++;
 #endif
@@ -1501,6 +1617,7 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
           for (int jw = 0; jw < W; jw++) vs[(nvw + jw) * 32 + lane] = V[jw];
           nvw += W;
         }
+        SBG_TF_MARK(5);
         // emit the chunk: lane-major (= (e,f) order), then g ascending
         if (!chunk_live) continue;   // the common case: nothing survived
         int cnt = 0;
@@ -1547,6 +1664,7 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
         // One prefix never needs to contribute more than the list cap (lut.c:316-318); checked only
         // between chunks, when every pair up to here has all its g emitted.
         if (emitted >= list_cap) prefix_done = true;
+        SBG_TF_MARK(6);
       }
 #ifdef SBG_COUNT_FILTER
       if (lane == 0) {
@@ -1572,6 +1690,12 @@ __global__ void __launch_bounds__(kThreads, SBG_FILTER_MIN_CTAS) k_filter7_pm(co
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) swept_lane += __shfl_xor_sync(kFull, swept_lane, d);
   if (lane == 0 && swept_lane != 0) atomicAdd(&ctl->swept, swept_lane);
+#ifdef SBG_TIME_FILTER
+  if (lane == 0) {
+    for (int k = 0; k < 7; k++) atomicAdd(&ctl->pad1[k], tf_acc[k]);
+  }
+#endif
+#undef SBG_TF_MARK
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1602,6 +1726,13 @@ __global__ void __launch_bounds__(256) k_offsets(DevCtl *__restrict__ ctl,
         ctl->pad1[0], ctl->pad1[1], ctl->pad1[2], ctl->pad1[3], ctl->pad1[4], ctl->pad1[5],
         ctl->pad1[6], ctl->hit_count, ctl->pad1[7], ctl->pad1[8], ctl->pad1[9]);
     for (int i = 0; i < 10; i++) ctl->pad1[i] = 0;
+#endif
+#ifdef SBG_TIME_FILTER
+    // SM clocks of phase 1's warps per section (see k_filter7_pm), summed over the launch
+    printf("T1 ticket %llu mixed %llu pairs %llu sep %llu sieve %llu cells %llu emit %llu\n",
+        ctl->pad1[0], ctl->pad1[1], ctl->pad1[2], ctl->pad1[3], ctl->pad1[4], ctl->pad1[5],
+        ctl->pad1[6]);
+    for (int i = 0; i < 7; i++) ctl->pad1[i] = 0;
 #endif
   }
   if (first >= handed) return;
