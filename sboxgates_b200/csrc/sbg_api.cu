@@ -624,7 +624,8 @@ bool search5_two_kernels(const sbg_handle *h, int n) {
   return h->opt_search5 != 0 ? h->opt_search5 == 2 : h_binom[n][5] <= two_kernel_max;
 }
 
-int enqueue_search5(sbg_handle *h, sbg_lane &L, int part, int nparts, bool two) {
+// head = false keeps the fused form on the prefix deal (see sbg_search5_part's fallback).
+int enqueue_search5(sbg_handle *h, sbg_lane &L, int part, int nparts, bool two, bool head = true) {
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const int n = hp.n;
   constexpr int P = 3;
@@ -635,7 +636,7 @@ int enqueue_search5(sbg_handle *h, sbg_lane &L, int part, int nparts, bool two) 
   // the feasible-but-not-decomposable tuples in front of the first match are spread over the
   // machine instead of being decomposed by the one warp that owns their prefix
   ChunkPlan pl;
-  if (!two && h->opt_head != 0 && n >= kHeadAlwaysMinGates) {
+  if (!two && head && h->opt_head != 0 && n >= kHeadAlwaysMinGates) {
     pl = plan_chunks_mode<P, P + 2>(n, hp.inmask, 1, kHeadWaves5, h_binom[n - 3][2]);
   }
   const uint64_t tickets = pl.all ? 0 : (total - pl.t_offset + nparts - 1) / nparts;
@@ -2110,13 +2111,18 @@ int sbg_search5_part(sbg_handle *h, int part, int nparts, const uint8_t *func_or
   sbg_lane &L = h->lane[0];
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
-  bool two = search5_two_kernels(h, hp.n);
+  const bool two_first = search5_two_kernels(h, hp.n);
+  bool two = two_first;
   CallInputs in;
   in.order5 = func_order;
   for (;;) {
     L.seq++;
     if ((rc = enqueue_begin(h, L, kBeginSearch5, in, 0)) != SBG_OK) return rc;
-    if ((rc = enqueue_search5(h, L, part, nparts, two)) != SBG_OK) return rc;
+    // A part that falls back from the two-kernel form keeps the prefix deal: the chunk head deals
+    // its items differently, and the other parts, which may not have overflowed, cut their shares
+    // by the prefix deal.  With the head this part's share would overlap theirs and leave ranks out.
+    // A whole search (one part) shares with nobody and keeps the head.
+    if ((rc = enqueue_search5(h, L, part, nparts, two, !two_first || nparts == 1)) != SBG_OK) return rc;
     if ((rc = wait_stage(h, L, 1)) != SBG_OK) return rc;
     if (two && L.h_out->overflow[1] != 0) {
       two = false;   // more feasible tuples than the buffer holds: let the fused kernel do it

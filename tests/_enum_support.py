@@ -41,6 +41,8 @@ def enum_oracle():
                                     C.c_uint64, u64p, u64p]
     lib.orc_search5_range.restype = C.c_uint64
     lib.orc_search5_range.argtypes = [u64p, C.c_int, u64p, u64p, i8p, u8p, C.c_int64, C.c_int64]
+    lib.orc_feasible5_range.restype = C.c_uint64
+    lib.orc_feasible5_range.argtypes = [u64p, C.c_int, u64p, u64p, i8p, C.c_int64, C.c_int64]
     lib.orc_filter7_range.restype = C.c_int64
     lib.orc_filter7_range.argtypes = [u64p, C.c_int, u64p, u64p, i8p, C.c_int64, C.c_int64, u16p,
                                       C.c_int64]
@@ -325,6 +327,196 @@ def result7_fields(res):
                                               "func_inner", "inner_seen", "stale_outer")}
     out["gates"] = [int(g) for g in res.gates[:7]]
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# search_5lut on the host: one combination's key, the keys of the library's shares of a sharded
+# search, the feasible count and the sbg_result fields a 5-LUT key must come with.
+
+def search5_tuple_key(tables, target, mask, inbits, order, rank):
+    """The key of combination `rank` alone (orc_search5_range over [rank, rank + 1)), or NONE."""
+    lib = enum_oracle()
+    _keep, args = _problem(tables, target, mask, inbits)
+    return int(lib.orc_search5_range(*args, S._order(order), rank, rank + 1))
+
+
+def feasible5(tables, target, mask, inbits, lo=0, hi=None, piece=None):
+    """The feasible 5-combinations (inbits applied) of ranks [lo, hi) (default: all of C(n,5)):
+    orc_feasible5_range over pieces on the pool, summed."""
+    lib = enum_oracle()
+    _keep, args = _problem(tables, target, mask, inbits)
+    if hi is None:
+        hi = int(S.oracle_lib().orc_n_choose_k(args[1], 5))
+    rs = pieces(lo, hi, piece or max(1, -(-(hi - lo) // (4 * workers()))))
+    with ThreadPoolExecutor(max_workers=workers()) as pool:
+        return sum(pool.map(lambda r: int(lib.orc_feasible5_range(*args, r[0], r[1])), rs))
+
+
+def planted5(tabs, gates, k, fo, fi):
+    """Target fi(fo(outer triple), inner pair) on ordering row k of the 5 gates (in the order of
+    `gates`, which is the combination's when they ascend)."""
+    row = S.order5_rows()[k]
+    g = [int(gates[row[i]]) for i in range(5)]
+    return S.lut_table(int(fi), S.lut_table(int(fo), tabs[g[0]], tabs[g[1]], tabs[g[2]]),
+                       tabs[g[3]], tabs[g[4]])
+
+
+def expected_result5(key, tables, target, mask, order):
+    """The sbg_result fields (a dict) the 5-LUT key `key` must come with, from the oracle's ordering
+    rows and inner solver; None for SBG_KEY_NONE or a key that does not decompose."""
+    if key == NONE:
+        return None
+    rank, k, pos = key >> 12, (key >> 8) & 0xF, key & 0xFF
+    comb = nth_comb(len(tables), 5, rank)
+    row = S.order5_rows()[k]
+    gates = [comb[row[i]] for i in range(5)]
+    fo = int(order[pos])
+    t1 = S.lut_table(fo, tables[gates[0]], tables[gates[1]], tables[gates[2]])
+    arrs = [S._u64(x) for x in (t1, tables[gates[3]], tables[gates[4]], target, mask)]
+    fi, seen = C.c_uint8(), C.c_uint8()
+    if not S.oracle_lib().orc_solve_inner(*[x[1] for x in arrs], C.byref(fi), C.byref(seen)):
+        return None
+    return dict(found=1, key=key, index=rank, ordering=k, pos_outer=pos, pos_middle=0,
+                func_outer=fo, func_middle=0, func_inner=int(fi.value), inner_seen=int(seen.value),
+                gates=gates, stale_outer=0)
+
+
+def result5_fields(res):
+    """The fields of an sbg_result that expected_result5 gives, as a dict."""
+    out = result7_fields(res)
+    out["gates"] = out["gates"][:5]
+    return out
+
+
+def source_constant(name, filename):
+    """A `constexpr uint64_t name = <int>;` of the library's source (sboxgates_b200/csrc)."""
+    import re
+    text = open(os.path.join(S.ROOT, "sboxgates_b200", "csrc", filename)).read()
+    m = re.search(r"constexpr uint64_t %s = (\d+);" % name, text)
+    assert m is not None, "cannot read %s from %s: update source_constant" % (name, filename)
+    return int(m.group(1))
+
+
+class Deal5:
+    """How search_5lut's sweep (k_sweep) cuts C(n,5) into items and deals them to the parts of a
+    sharded search, as rank ranges.
+
+    An item is a 3-gate prefix (a 3-subset of {0..n-3}, lexicographic), whose 5-combinations form
+    one contiguous rank range.  With the fused head (fused form, n >= 128) the first items are
+    (allowed-gate prefix, chunk of 32 (d,e) pairs) items over the first prefixes made of allowed
+    gates only, and the prefix items start at the first allowed prefix the head does not cover
+    (t_offset); sbg_plan_tickets gives the head's items, its chunks per prefix and t_offset.  The
+    head items and the prefix items are each dealt in blocks of kDeal consecutive items, block j to
+    part j mod P.  Every head item lies below t_offset, so a part's blocks in the order head blocks,
+    prefix blocks are in ascending rank order."""
+
+    def __init__(self, n, inbits, head):
+        from sboxgates_b200 import native
+        self.n = n
+        self.kdeal = source_constant("kDeal", "sbg_device.cuh")
+        self.total = int(S.oracle_lib().orc_n_choose_k(n - 2, 3))
+        excl = sorted({int(b) for b in inbits if 0 <= b < 8})
+        self.items, self.chunks, self.t_offset = 0, 1, 0
+        if head:
+            out = (C.c_uint64 * 4)()
+            rc = native.load_library().sbg_plan_tickets(
+                5, 3, n, sum(1 << b for b in excl), 1, source_constant("kHeadWaves5", "sbg_api.cu"),
+                out)
+            assert rc == 0, (n, excl)
+            self.items, self.chunks, self.t_offset = int(out[0]), int(out[1]), int(out[2])
+        self.allowed = [g for g in range(n) if g not in excl]
+        self.head_blocks = -(-self.items // self.kdeal)
+        self.prefix_blocks = -(-(self.total - self.t_offset) // self.kdeal)
+
+    def _base(self, pre):
+        """(rank of the prefix's first combination, its number of combinations)."""
+        r = self.n - pre[2] - 1
+        return comb_rank(self.n, 5, list(pre) + [pre[2] + 1, pre[2] + 2]), r * (r - 1) // 2
+
+    def block_ranges(self, j):
+        """The rank ranges [lo, hi) of block j of the dealt order (head blocks first), ascending."""
+        out = []
+        if j < self.head_blocks:
+            for i in range(j * self.kdeal, min((j + 1) * self.kdeal, self.items)):
+                t, c = divmod(i, self.chunks)
+                idx = nth_comb(len(self.allowed) - 2, 3, t)
+                base, q = self._base([self.allowed[x] for x in idx])
+                lo, hi = base + 32 * c, base + min(32 * c + 32, q)
+                if lo >= hi:
+                    continue
+                if out and out[-1][1] == lo:
+                    out[-1] = (out[-1][0], hi)
+                else:
+                    out.append((lo, hi))
+            return out
+        j -= self.head_blocks
+        first = self.t_offset + j * self.kdeal
+        last = min(first + self.kdeal, self.total) - 1
+        lo, _ = self._base(nth_comb(self.n - 2, 3, first))
+        base, q = self._base(nth_comb(self.n - 2, 3, last))
+        return [(lo, base + q)]
+
+    def blocks(self):
+        return self.head_blocks + self.prefix_blocks
+
+    def part_blocks(self, part, nparts, skip_excluded=True):
+        """The blocks of part `part` of `nparts`, in ascending rank order.  Prefix blocks that end
+        before the first prefix of allowed gates hold no allowed combination; skip_excluded leaves
+        them out (with input bits 0-7 excluded at n = 500 they are 68,000 blocks)."""
+        first = 0
+        if skip_excluded and len(self.allowed) >= 5:
+            lead = comb_rank(self.n - 2, 3, self.allowed[:3])
+            first = max(0, (lead - self.t_offset) // self.kdeal)
+        start = first + (part - first) % nparts
+        return ([j for j in range(part, self.head_blocks, nparts)]
+                + [self.head_blocks + j for j in range(start, self.prefix_blocks, nparts)])
+
+
+class Search5Oracle:
+    """The oracle's first keys of one search_5lut problem per dealt block, computed on demand and
+    kept, so that the keys of several shardings come from one walk."""
+
+    def __init__(self, tables, target, mask, inbits, order, head):
+        self.n = len(tables)
+        self.deal = Deal5(self.n, inbits, head)
+        self.keep, self.args = _problem(tables, target, mask, inbits)
+        self.order = S._order(order)
+        self.keys = {}
+        self.walked = 0   # combinations the oracle has decided or rejected
+
+    def block_key(self, j):
+        if j not in self.keys:
+            key = NONE
+            for lo, hi in self.deal.block_ranges(j):
+                key = int(enum_oracle().orc_search5_range(*self.args, self.order, lo, hi))
+                self.walked += hi - lo
+                if key != NONE:
+                    break
+            self.keys[j] = key
+        return self.keys[j]
+
+    def part_key(self, part, nparts, limit=None):
+        """The key of part `part` of `nparts`: its blocks a batch (one per worker) at a time in rank
+        order, stopping after the first batch that holds a match.  None if its blocks spanning
+        `limit` combinations held no match and more are left."""
+        blocks = self.deal.part_blocks(part, nparts)
+        w = workers()
+        spanned = 0
+        with ThreadPoolExecutor(max_workers=w) as pool:
+            for b in range(0, len(blocks), w):
+                if limit is not None and spanned >= limit:
+                    return None
+                batch = blocks[b:b + w]
+                keys = list(pool.map(self.block_key, batch))
+                if min(keys) != NONE:
+                    return min(keys)
+                spanned += sum(hi - lo for j in batch for lo, hi in self.deal.block_ranges(j))
+        return NONE
+
+
+def part_keys5(tables, target, mask, inbits, order, part, nparts, head):
+    """The key of the library's share `part` of `nparts` of a sharded search_5lut (Deal5)."""
+    return Search5Oracle(tables, target, mask, inbits, order, head).part_key(part, nparts)
 
 
 def comb_rank(n, t, comb):

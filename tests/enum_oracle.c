@@ -98,6 +98,21 @@ uint64_t orc_search5_range(const uint64_t *tables, int n, const uint64_t *target
   return key;
 }
 
+/* The feasible 5-combinations (inbits applied) of ranks [lo, hi): what enum5_range counts in
+   *feasible, without deciding any of them. */
+uint64_t orc_feasible5_range(const uint64_t *tables, int n, const uint64_t *target,
+    const uint64_t *mask, const int8_t *inbits, int64_t lo, int64_t hi) {
+  uint16_t nums[5];
+  uint64_t feasible = 0;
+  for (int64_t r = range_start(n, 5, lo, &hi, nums); r < hi; r++, orc_next_combination(nums, 5, n)) {
+    if (rejected(nums, 5, inbits)) continue;
+    uint64_t tt[5 * 4];
+    for (int m = 0; m < 5; m++) memcpy(tt + 4 * m, tables + 4 * nums[m], 32);
+    feasible += orc_check_n_lut_possible(5, target, mask, tt) ? 1 : 0;
+  }
+  return feasible;
+}
+
 /* lut.c:290-327 over the 7-combinations of ranks [lo, hi): writes the first `cap` feasible ones
    (7 x uint16 each, inbits applied) in order; returns how many there are in the range. */
 int64_t orc_filter7_range(const uint64_t *tables, int n, const uint64_t *target,
