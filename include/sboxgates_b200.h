@@ -117,7 +117,11 @@ int sbg_load_problem(sbg_handle *h, const uint64_t *tables, int n, const uint64_
 /* The same in two steps, for callers that keep several search states resident in HBM: stage a
    state into slot 0..SBG_PROBLEM_SLOTS-1 (upload), later make a staged slot the current problem
    (no transfer).  sbg_load_problem() = stage + use of slot 0.  This is the device-resident
-   replacement of the `state` array the reference re-broadcasts per call (lut.c:533-540). */
+   replacement of the `state` array the reference re-broadcasts per call (lut.c:533-540).
+   A 7-LUT list belongs to the slot and the state it was built or installed for: staging a different
+   state into that slot, the current one included, leaves the list to no problem (sbg_enum7 then
+   runs phase 1 again, sbg_decomp7_part / sbg_finish7 return SBG_ERR_STATE); staging the state the
+   slot already holds ships nothing and keeps the list.  sbg_use_problem drops the list. */
 int sbg_stage_problem(sbg_handle *h, int slot, const uint64_t *tables, int n,
     const uint64_t *target, const uint64_t *mask, const int8_t *inbits);
 int sbg_use_problem(sbg_handle *h, int slot);
@@ -154,11 +158,17 @@ typedef struct {
   sbg_result r5;               /* as sbg_search5 (found = 0 if the stage did not run) */
   sbg_result r7;               /* as sbg_search7 */
 } sbg_node_result;
-/* One node; returns as soon as a stage has matched. */
+/* One node; returns as soon as a stage has matched.  The job's slot becomes the current problem;
+   the installed 7-LUT list is dropped, and when the search_7lut stage ran, its list is installed
+   for that slot. */
 int sbg_search_node(sbg_handle *h, const sbg_job *job, sbg_node_result *result);
 /* Independent nodes (the first children of a create_circuit node, sboxgates.c:458-607; the output
    bits of generate_graph, sboxgates.c:701-788; the -i iterations): their chains run concurrently
-   on up to SBG_LANES streams, results are read once per job. */
+   on up to SBG_LANES streams, results are read once per job.  Jobs may repeat a slot (lanes that
+   share one are ordered where the slot's problem block is brought up to date).  The current
+   problem does not change.  The installed 7-LUT list is dropped; the list of the first job of the
+   last wave of SBG_LANES jobs is left installed for that job's slot when its search_7lut stage
+   ran, so list consumers use it only when that slot is the current problem. */
 int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_result *results);
 
 /* ---- sharded building blocks (one process per GPU; part = rank, nparts = world size) -------- */
@@ -179,7 +189,8 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
    which reproduces lut.c:316-349 for size == 1. */
 int sbg_set_list7(sbg_handle *h, const uint64_t *list, int count);
 /* The same without touching the host: this part's ordered list as a device pointer (valid until the
-   next search on the handle), and the merge of `nruns` ascending runs that already sit in device
+   next search on the handle; count 0 when the handle holds no list of the current problem as it is
+   staged now), and the merge of `nruns` ascending runs that already sit in device
    memory, run r at runs + r * stride with counts[r] entries (what an all-gather of the parts'
    lists into one buffer gives). */
 int sbg_list7_device(sbg_handle *h, const uint64_t **list, int *count);
@@ -193,7 +204,8 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
 int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total);
 /* 7-LUT phase 2 over list indices congruent to part modulo nparts.  sbg_finish7 decodes any part's
    key against the installed list; it reuses the entries sbg_decomp7_part returned with its key only
-   while that list is still installed. */
+   while that list is still installed.  Both return SBG_ERR_STATE unless a list is installed for the
+   current problem as it is staged now (see sbg_stage_problem, sbg_search_batch). */
 int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t *key);
 int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
@@ -238,8 +250,9 @@ typedef struct {
 int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, uint64_t max_matches,
     sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible);
 /* The 7-LUT list: the one installed for the current problem (sbg_set_list7 / sbg_set_list7_device /
-   sbg_allgather_merge7, sbg_filter7_part with nparts == 1, or an earlier sbg_search7 of it), else
-   phase 1 runs here over the whole space and its list stays installed. */
+   sbg_allgather_merge7, sbg_filter7_part with nparts == 1, or an earlier sbg_search7, sbg_search_node
+   or sbg_search_batch of it, with the problem not staged anew since), else phase 1 runs here over
+   the whole space and its list stays installed. */
 int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
     uint64_t *total, uint64_t *feasible);

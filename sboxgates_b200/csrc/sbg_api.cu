@@ -132,10 +132,19 @@ struct sbg_lane {
   cudaEvent_t ev[8] = {};        // timing (only with sbg_set_timing)
   cudaEvent_t ev_done = nullptr; // end of the lane's last chain
   bool ev_ready = false;
+  // sbg_search_batch, one slot on several lanes of a wave: the lane's last k_begin brought the
+  // slot's problem block or rows up to date (prepared); ev_begun follows it when mark_begun is set
+  bool prepared = false;
+  bool mark_begun = false;
+  cudaEvent_t ev_begun = nullptr;
   uint64_t seq = 0;
   int slot = -1;                 // problem the lane's chain works on
   uint32_t list_count = 0;
   bool list_ready = false;
+  // the problem the list in d_sorted (installed, or a part's from sbg_filter7_part) was built for:
+  // a slot and that slot's version at the time (-1: none)
+  int list_slot = -1;
+  uint64_t list_version = 0;
   bool timed5 = false, timed7 = false;
   float ms[4] = {0, 0, 0, 0};
   uint64_t last_key = SBG_KEY_NONE;   // sbg_decomp7_part's result and the two list entries behind it
@@ -220,6 +229,7 @@ struct sbg_handle {
     int dev_n = 0;
     int comp_n = 0;
     bool header_valid = false;
+    uint64_t version = 0;        // bumped by every staged change (not by an identical restage)
   };
   HostProblem *slots = nullptr;  // kSlots entries
   int cur_slot = 0;
@@ -1081,6 +1091,7 @@ int stage_problem(sbg_handle *h, int slot, const uint64_t *tables, int n, const 
     SBG_CUDA(h, cudaStreamWaitEvent(h->lane[0].stream, h->lane[hp.busy_lane].ev_done, 0));
   }
   memcpy(hp.tables[lcp], tables + 4 * lcp, (size_t)(n - lcp) * 32);
+  hp.version++;   // a list built for the slot's previous state no longer belongs to it
   memcpy(hp.target, target, 32);
   memcpy(hp.mask, mask, 32);
   hp.dev_n = std::min(hp.dev_n, lcp);
@@ -1145,6 +1156,8 @@ int enqueue_begin(sbg_handle *h, sbg_lane &L, uint32_t flags, const CallInputs &
   const cudaError_t e = launch(h, k_begin, 1 + prep + scan, 1024, smem, L.stream, false,
       h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_par7, L.d_pos5, L.d_gcount, h->d_tab, prep, a);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_begin: %s", cudaGetErrorString(e));
+  L.prepared = (a.flags & kBeginProblem) != 0;
+  if (L.prepared && L.mark_begun) SBG_CUDA(h, cudaEventRecord(L.ev_begun, L.stream));
   return SBG_OK;
 }
 
@@ -1197,10 +1210,22 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
 // Every install or drop of a lane's 7-LUT list goes through here.  The key and list entries the last
 // sbg_decomp7_part left behind belong to the list it searched, so any change of the list forgets them
 // (sbg_finish7 would otherwise decode an equal key of the new list with the old list's entries).
-void set_list(sbg_lane &L, uint32_t count, bool ready) {
+// `slot`: the list in d_sorted was built for that slot's problem as it is staged now (-1: for none).
+void set_list(sbg_handle *h, sbg_lane &L, uint32_t count, bool ready, int slot = -1) {
   L.list_count = count;
   L.list_ready = ready;
   L.last_key = SBG_KEY_NONE;
+  L.list_slot = slot;
+  L.list_version = slot >= 0 ? h->slots[slot].version : 0;
+}
+
+// Whether lane 0's list (installed, or a part's) belongs to the current problem as staged now.  A
+// batch leaves on lane 0 the list of its last wave's first job, whatever slot that job searched, and
+// restaging a slot changes its problem under the list; the list's consumers check this.
+bool list_of_current(const sbg_handle *h) {
+  const sbg_lane &L = h->lane[0];
+  return h->problem_ready && L.list_slot == h->cur_slot
+      && L.list_version == h->slots[h->cur_slot].version;
 }
 
 int check_job(sbg_handle *h, const sbg_job *job) {
@@ -1255,7 +1280,7 @@ int redo_search7_steps(sbg_handle *h, sbg_lane &L, const uint8_t *outer, const u
   int rc;
   uint32_t keep = 0;
   if ((rc = run_filter7(h, L, 0, 1, &keep, hit_buffer_overflowed)) != SBG_OK) return rc;
-  set_list(L, keep, true);
+  set_list(h, L, keep, true, L.slot);
   L.seq++;
   CallInputs in;
   in.outer = outer;
@@ -1317,7 +1342,7 @@ int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, sbg_node_resul
           o->overflow[2] == 1)) != SBG_OK) return rc;
       swept7 = h->swept;
     }
-    set_list(L, (uint32_t)o->feasible[2], true);
+    set_list(h, L, (uint32_t)o->feasible[2], true, L.slot);
     if ((rc = finish7_slot(h, hp, o->key[2], job->outer7, job->middle7, o->tuple, o->tuple_prev,
         o->feasible[2], swept7, &res->r7)) != SBG_OK) return rc;
     if (res->r7.found) res->found_stage = 7;
@@ -1510,10 +1535,10 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   sbg_lane &L = h->lane[0];
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
-  if (WIDTH == 7 && !L.list_ready) {
+  if (WIDTH == 7 && !(L.list_ready && list_of_current(h))) {
     uint32_t count = 0;
     if ((rc = run_filter7(h, L, 0, 1, &count)) != SBG_OK) return rc;
-    set_list(L, count, true);
+    set_list(h, L, count, true, L.slot);
   } else {
     L.seq++;
     if ((rc = enqueue_begin(h, L, flags, begin_in, 0)) != SBG_OK) return rc;
@@ -1835,6 +1860,7 @@ int sbg_create(sbg_handle **out, int device) {
     L.stream = L.own_stream;
     for (int k = 0; k < 8; k++) SBG_CUDA(h, cudaEventCreate(&L.ev[k]));
     SBG_CUDA(h, cudaEventCreateWithFlags(&L.ev_done, cudaEventDisableTiming));
+    SBG_CUDA(h, cudaEventCreateWithFlags(&L.ev_begun, cudaEventDisableTiming));
     SBG_CUDA(h, cudaMalloc(&L.d_ctl, sizeof(DevCtl)));
     {
       DevCtl init;
@@ -1985,6 +2011,7 @@ void sbg_destroy(sbg_handle *h) {
       if (L.h_ctl != nullptr) cudaFreeHost(L.h_ctl);
       for (int k = 0; k < 8; k++) if (L.ev[k] != nullptr) cudaEventDestroy(L.ev[k]);
       if (L.ev_done != nullptr) cudaEventDestroy(L.ev_done);
+      if (L.ev_begun != nullptr) cudaEventDestroy(L.ev_begun);
       if (L.own_stream != nullptr) cudaStreamDestroy(L.own_stream);
     }
     cudaFree(h->d_slots);
@@ -2075,7 +2102,7 @@ int sbg_use_problem(sbg_handle *h, int slot) {
   if (!h->slots[slot].ready) return fail(h, SBG_ERR_STATE, "slot %d holds no problem", slot);
   h->cur_slot = slot;
   h->problem_ready = true;
-  set_list(h->lane[0], 0, false);
+  set_list(h, h->lane[0], 0, false);
   return SBG_OK;
 }
 
@@ -2164,7 +2191,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
   uint32_t keep = 0;
-  set_list(L, L.list_count, false);
+  set_list(h, L, L.list_count, false);
   if ((rc = run_filter7(h, L, part, nparts, &keep)) != SBG_OK) return rc;
   for (int i = 0; i < 4; i++) h->last_ms[i] = L.ms[i];
   *count = (int)keep;
@@ -2176,7 +2203,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   }
   // The part's own ordered list stays on the device; when it is the whole space (nparts == 1) it
   // IS the list, and phase 2 may follow without sbg_set_list7().
-  set_list(L, keep, nparts == 1);
+  set_list(h, L, keep, nparts == 1, h->cur_slot);
   return SBG_OK;
 }
 
@@ -2184,7 +2211,7 @@ int sbg_list7_device(sbg_handle *h, const uint64_t **list, int *count) {
   if (h == nullptr || list == nullptr || count == nullptr) return SBG_ERR_ARG;
   h->api_seq++;   // ends the enumeration cursor
   *list = h->lane[0].d_sorted;
-  *count = (int)h->lane[0].list_count;
+  *count = list_of_current(h) ? (int)h->lane[0].list_count : 0;
   return SBG_OK;
 }
 
@@ -2211,7 +2238,7 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
   const cudaError_t e = launch(h, k_merge_runs, grid, 256, 0, L.stream, false, runs,
       (unsigned long long)stride, rcnt, nruns, L.d_sorted, (unsigned int)SBG_LIST_CAP, L.d_ctl);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_merge_runs: %s", cudaGetErrorString(e));
-  set_list(L, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP), true);
+  set_list(h, L, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP), true, h->cur_slot);
   return SBG_OK;
 }
 
@@ -2314,7 +2341,9 @@ int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_o
   h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   sbg_lane &L = h->lane[0];
-  if (!L.list_ready) return fail(h, SBG_ERR_STATE, "no 7-LUT list installed");
+  if (!L.list_ready || !list_of_current(h)) {
+    return fail(h, SBG_ERR_STATE, "no 7-LUT list installed for the current problem");
+  }
   if (nparts < 1 || part < 0 || part >= nparts) return fail(h, SBG_ERR_ARG, "bad part %d/%d", part, nparts);
   if (!valid_order(outer_order) || !valid_order(middle_order)) {
     return fail(h, SBG_ERR_ARG, "function order is not a permutation");
@@ -2325,6 +2354,11 @@ int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_o
   h->last_ms[3] = 0.f;
   if (L.list_count == 0) return SBG_OK;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
+  // k_decomp7 takes the list's length from the control words, which k_begin keeps here; but the
+  // k_begin of a search_5lut or a 5-LUT enumeration since the list was installed has cleared them
+  L.h_ctl->list_count = L.list_count;
+  SBG_CUDA(h, cudaMemcpyAsync(&L.d_ctl->list_count, &L.h_ctl->list_count, sizeof(uint32_t),
+      cudaMemcpyHostToDevice, L.stream));
   L.seq++;
   CallInputs in;
   in.outer = outer_order;
@@ -2352,6 +2386,9 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
   h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   sbg_lane &L = h->lane[0];
+  if (!L.list_ready || !list_of_current(h)) {
+    return fail(h, SBG_ERR_STATE, "no 7-LUT list installed for the current problem");
+  }
   uint64_t pair[2] = {0, 0};
   if (key != SBG_KEY_NONE) {
     const uint64_t idx = key >> 23;
@@ -2392,7 +2429,7 @@ int sbg_search_node(sbg_handle *h, const sbg_job *job, sbg_node_result *res) {
   in.outer = job->outer7;
   in.middle = job->middle7;
   in.gate_order = job->gate_order;
-  set_list(L, L.list_count, false);
+  set_list(h, L, L.list_count, false);
   if ((rc = enqueue_chain(h, L, job->flags, in)) != SBG_OK) return rc;
   const double t1 = wall_now();
   if ((rc = collect_chain(h, L, job, res)) != SBG_OK) return rc;
@@ -2430,6 +2467,18 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
       sbg_lane &L = h->lane[k];
       const sbg_job &job = jobs[base + k];
       if (k > 0) SBG_CUDA(h, cudaStreamWaitEvent(L.stream, h->lane[0].ev_done, 0));
+      // A slot on several lanes: the first lane's k_begin applies the slot's pending change, and the
+      // first with search_7lut builds its rows; the later lanes skip that work and would read the
+      // problem block while it is being written.  Each starts after the last such k_begin of an
+      // earlier lane (which itself started after the one before).  Distinct slots wait on nothing.
+      for (int j = k - 1; j >= 0; j--) {
+        if (jobs[base + j].slot == job.slot && h->lane[j].prepared) {
+          SBG_CUDA(h, cudaStreamWaitEvent(L.stream, h->lane[j].ev_begun, 0));
+          break;
+        }
+      }
+      L.mark_begun = false;
+      for (int j = k + 1; j < wave; j++) L.mark_begun |= jobs[base + j].slot == job.slot;
       L.slot = job.slot;
       h->slots[job.slot].busy_lane = k;
       CallInputs in;
@@ -2437,8 +2486,10 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
       in.outer = job.outer7;
       in.middle = job.middle7;
       in.gate_order = job.gate_order;
-      set_list(L, L.list_count, false);
-      if ((rc = enqueue_chain(h, L, job.flags, in)) != SBG_OK) {
+      set_list(h, L, L.list_count, false);
+      rc = enqueue_chain(h, L, job.flags, in);
+      L.mark_begun = false;
+      if (rc != SBG_OK) {
         h->concurrent = false;
         return rc;
       }

@@ -121,7 +121,8 @@ class LutEngine:
                 self._h = C.c_void_p()
             raise NativeLibraryError("sbg_create(device=%d): %s" % (device, msg))
         self.device = device
-        self.n = 0
+        self.n = 0              # gates of the current problem (the current slot's)
+        self._cur = 0
         self._slot_n = {}
         if stream is not None:
             self.set_stream(stream)
@@ -179,6 +180,7 @@ class LutEngine:
         ib[:len(inbits)] = inbits
         self.n = tables.shape[0]
         self._slot_n[0] = self.n
+        self._cur = 0
         self._check(self.lib.sbg_load_problem(self._h, tp, self.n, gp, mp,
                                               ib.ctypes.data_as(native.i8p)))
 
@@ -191,7 +193,12 @@ class LutEngine:
         ib[:len(inbits)] = inbits
         self._check(self.lib.sbg_stage_problem(self._h, slot, tp, tables.shape[0], gp, mp,
                                                ib.ctypes.data_as(native.i8p)))
-        self._slot_n[slot] = tables.shape[0]
+        self._staged(slot, tables.shape[0])
+
+    def _staged(self, slot, n):
+        self._slot_n[slot] = n
+        if slot == self._cur:   # restaging the current slot changes the current problem
+            self.n = n
 
     def prepare_state(self, tables, target, mask, inbits):
         """Marshals a state's host buffers once (numpy -> pointers) for stage_prepared: a caller that
@@ -208,11 +215,12 @@ class LutEngine:
         """stage() on the result of prepare_state (which keeps the host buffers alive)."""
         self._check(self.lib.sbg_stage_problem(self._h, slot, prep[1], prep[8], prep[3], prep[5],
                                                prep[7]))
-        self._slot_n[slot] = prep[8]
+        self._staged(slot, prep[8])
 
     def use(self, slot):
         self._check(self.lib.sbg_use_problem(self._h, slot))
         self.n = self._slot_n[slot]
+        self._cur = slot
 
     # -- whole searches ------------------------------------------------------------------------
     def search5(self, func_order):
@@ -258,6 +266,8 @@ class LutEngine:
         job, keep = self._job(slot, order5, outer, middle, gate_order)
         res = SbgNodeResult()
         self._check(self.lib.sbg_search_node(self._h, C.byref(job), C.byref(res)))
+        self.n = self._slot_n.get(slot, self.n)   # the node's slot is now the current problem
+        self._cur = slot
         return res
 
     def search_batch(self, jobs):
