@@ -292,6 +292,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
        sbg_set_timing, sbg_set_stream, sbg_enum_fetch, sbg_enum_pick, sbg_enum_block_sums,
        sbg_enum_set_global and sbg_enum_depth_counts keep it;
      - sbg_enum_set_depth ends it, whatever the call returns.
+     - sbg_enum_set_functions ends it, whatever the call returns.
    Without a cursor both calls return SBG_ERR_STATE.
    A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
    a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT) or a list
@@ -365,6 +366,37 @@ int sbg_enum_set_depth(sbg_handle *h, const uint16_t *depth, int n, uint32_t max
    bin, count again with that bound.  SBG_ERR_STATE without a cursor or when it was counted without
    a filter; SBG_ERR_ARG for nbins > SBG_DEPTH_BINS.  Keeps the cursor. */
 int sbg_enum_depth_counts(sbg_handle *h, uint64_t *out, uint32_t nbins);
+
+/* ---- function filter: the realisations whose LUTs lie in given sets of functions ------------- */
+/* The caller gives three sets of 3-input functions, outer, middle and inner, each 4 words: bit f of
+   word f >> 6 set = function f allowed, functions numbered as for sbg_lut_table (bit index
+   in1<<2 | in2<<1 | in3).  A match is kept iff
+     7-LUT: func_outer is in outer, func_middle is in middle, and the inner LUT can be completed
+            inside inner;
+     5-LUT: func_outer is in outer, and the inner LUT can be completed inside inner (middle plays
+            no part);
+     3-LUT: the LUT can be completed inside inner (outer and middle play no part);
+   where "can be completed inside inner" means some f in inner has (f & inner_seen) == func_inner,
+   from the match's record (not from a random fill, so the result is deterministic).  Under a
+   filter the matches of sbg_enum3 / sbg_enum5 / sbg_enum7 are exactly the unfiltered matches that
+   pass it: keys, key order and records are unchanged, only the set shrinks, and ranks are ranks
+   within it.  The 7-LUT list is still the phase-1 list, and *feasible keeps its meaning (with a
+   depth filter, its depth-filtered one).  Together with a depth filter both tests apply, and
+   sbg_enum_depth_counts reports the matches that pass both.  The cursor keeps the filter it was
+   counted under, so fetch, pick, sbg_enum_block_sums and sbg_enum_set_global serve the filtered
+   set.  Searches (sbg_search*, sbg_search_node / batch, the *_part and finish calls) never read
+   it.  A filtered 7-LUT count with a restricted inner set visits every (outer, middle) pair of
+   each cube union instead of counting the union's bits, so it costs more than the others. */
+/* Installs the filter (host memory; NULL = all 256 functions) for the later sbg_enum3 /
+   sbg_enum5 / sbg_enum7 calls on the handle; all three NULL clears it.  An empty set is valid and
+   leaves no match.  The call ends the cursor. */
+int sbg_enum_set_functions(sbg_handle *h, const uint64_t *outer, const uint64_t *middle,
+    const uint64_t *inner);
+/* Test hook, no device needed: the inner table the kernels read.  out[code(seen, ones)] = 1 iff
+   some f in inner (4 words; NULL = all 256) has (f & seen) == ones, else 0, for every seen and
+   every ones within seen; code(S, V) = p3(S) + p3(V), p3(x) = the sum of 3^j over the set bits j
+   of x (6,561 entries). */
+int sbg_inner_table(const uint64_t *inner, uint8_t *out);
 
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense

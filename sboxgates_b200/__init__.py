@@ -12,7 +12,8 @@ from .lut import LutEngine, SearchResult, NO_GATE, search_5lut, search_7lut, shu
     shuffled_orders7, ordering_row, solve_inner, lut_table, lut_search, LutSearchResult, \
     Enumeration, enumerate_3lut, enumerate_5lut, enumerate_7lut, enumerate_lut_search, \
     match_to_ret, match_to_lut3, decode_key3, decode_key5, decode_key7, sample_matches, \
-    match_depth, shallowest_matches
+    match_depth, shallowest_matches, AFFINE_FUNCTIONS, gate_functions, match_functions_allowed, \
+    allowed_fill, inner_table
 from .native import load_library, NativeLibraryError, MATCH_DTYPE, SBG_MAX_DEPTH, SBG_DEPTH_BINS
 
 __all__ = [
@@ -21,5 +22,6 @@ __all__ = [
     "lut_search", "LutSearchResult", "Enumeration", "enumerate_3lut", "enumerate_5lut",
     "enumerate_7lut", "enumerate_lut_search", "match_to_ret", "match_to_lut3", "decode_key3",
     "decode_key5", "decode_key7", "sample_matches", "match_depth", "shallowest_matches",
+    "AFFINE_FUNCTIONS", "gate_functions", "match_functions_allowed", "allowed_fill", "inner_table",
     "MATCH_DTYPE", "SBG_MAX_DEPTH", "SBG_DEPTH_BINS", "load_library", "NativeLibraryError",
 ]

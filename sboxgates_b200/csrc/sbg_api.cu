@@ -170,13 +170,17 @@ struct sbg_lane {
 };
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
-// (widths 5 and 7) or the gate order (width 3), and the depth filter if one was installed
-// (sbg_enum_set_depth; its histogram pointer is the lane's, set at launch).
+// (widths 5 and 7) or the gate order (width 3), the depth filter if one was installed
+// (sbg_enum_set_depth; its histogram pointer is the lane's, set at launch), and the function
+// filter if one was installed (sbg_enum_set_functions; with it, depth holds the neutral filter
+// when `filtered` is false).
 struct EnumInputs {
   EnumOrders ord;
   EnumGateOrder gates;
   bool filtered;
   EnumDepth<true> depth;
+  bool fn_on;
+  EnumFunc fn;
 };
 
 // The depth filter of a handle (sbg_enum_set_depth): the depths of n gates and the bound.
@@ -185,6 +189,12 @@ struct DepthFilter {
   int n = 0;
   uint32_t max_depth = 0;
   uint16_t depth[SBG_MAX_GATES] = {};
+};
+
+// The function filter of a handle (sbg_enum_set_functions), ready for the kernels.
+struct FunctionFilter {
+  bool on = false;
+  EnumFunc fn = {};
 };
 
 // The enumeration cursor: what sbg_enum_fetch / sbg_enum_pick need of the last counted enumeration
@@ -269,6 +279,7 @@ struct sbg_handle {
   uint64_t api_seq = 0;
   EnumCursor cursor;
   DepthFilter filter;   // read by sbg_enum3 / sbg_enum5 / sbg_enum7 only
+  FunctionFilter functions;   // likewise
 };
 
 namespace {
@@ -1434,6 +1445,10 @@ static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
     && offsetof(sbg_match, func_outer) == offsetof(DevMatch, func_outer)
     && offsetof(sbg_match, inner_seen) == offsetof(DevMatch, inner_seen)
     && offsetof(sbg_match, width) == offsetof(DevMatch, width), "sbg_match and DevMatch agree");
+// The largest enumeration form, k_enum3_fn: the gate order, the depth filter and the function
+// filter, plus at most 128 bytes of pointers and scalars, within the 4 KB kernel-parameter limit.
+static_assert(sizeof(EnumGateOrder) + sizeof(EnumDepth<true>) + sizeof(EnumFunc) + 128 <= 4096,
+    "k_enum3_fn's parameters fit in 4 KB");
 
 // Count-free windows start at this many tickets and double: a first-match search then costs a few
 // windows of work past the first match, a search without one about twice the counting sweep's
@@ -1499,10 +1514,22 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
             h->d_tab, dep);
       }
     };
-    if (!in.filtered) return run_form(std::false_type(), EnumDepth<false>());
+    if (!in.filtered && !in.fn_on) return run_form(std::false_type(), EnumDepth<false>());
     EnumDepth<true> dep = in.depth;
     dep.hist = L.d_ehist;
-    return run_form(std::true_type(), dep);
+    if (!in.fn_on) return run_form(std::true_type(), dep);
+    // the function-filtered form, with the depth filter or the neutral one
+    if constexpr (WIDTH == 3) {
+      return run(k_enum3_fn<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates, L.d_ecount,
+          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, dep, in.fn);
+    } else if constexpr (WIDTH == 5) {
+      return run(k_enum5_fn<NW, MODE>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
+          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, dep, in.fn);
+    } else {
+      return run(k_enum7_fn<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
+          L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts,
+          h->d_tab, dep, in.fn);
+    }
   });
   if (rc != SBG_OK) return rc;
   if (MODE == kEnumCount) {
@@ -1554,7 +1581,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   if ((rc = grow(h, L, L.d_ecount, L.ecount_cap, room)) != SBG_OK) return rc;
   if ((rc = grow(h, L, L.d_eoffset, L.eoffset_cap, room)) != SBG_OK) return rc;
   SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
-  if (in.filtered) {
+  if (in.filtered || in.fn_on) {
     if ((rc = grow(h, L, L.d_ehist, L.ehist_cap, (uint64_t)kDepthBins)) != SBG_OK) return rc;
     SBG_CUDA(h, cudaMemsetAsync(L.d_ehist, 0, kDepthBins * sizeof(unsigned long long), L.stream));
   }
@@ -1603,8 +1630,9 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   }
   if (total != nullptr) *total = ec.carry;
   if (feasible != nullptr) {
-    // width 3: every feasible triple is a match
-    *feasible = WIDTH == 7 ? (uint64_t)L.list_count : WIDTH == 3 ? ec.total : ec.feasible;
+    // width 3: every feasible triple is a match (the function-filtered form counts them apart)
+    *feasible = WIDTH == 7 ? (uint64_t)L.list_count
+        : WIDTH == 3 && !in.fn_on ? ec.total : ec.feasible;
   }
   return SBG_OK;
 }
@@ -1625,11 +1653,24 @@ int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, s
   return SBG_OK;
 }
 
-// The handle's depth filter, if any, into the inputs of an sbg_enum* call on the current problem.
+// The handle's depth and function filters, if any, into the inputs of an sbg_enum* call on the
+// current problem.
 int take_filter(sbg_handle *h, EnumInputs &in) {
   const DepthFilter &f = h->filter;
   in.filtered = f.on;
-  if (!f.on) return SBG_OK;
+  in.fn_on = h->functions.on;
+  if (in.fn_on) {
+    in.fn = h->functions.fn;
+    in.fn.depth_on = f.on;
+  }
+  if (!f.on) {
+    if (in.fn_on) {
+      // the neutral depth filter: every gate at depth 0, a bound no match exceeds
+      memset(&in.depth, 0, sizeof(in.depth));
+      in.depth.max_depth = kDepthBins - 1;
+    }
+    return SBG_OK;
+  }
   const int n = cur(h).n;
   if (f.n != n) {
     return fail(h, SBG_ERR_ARG, "the depth filter holds %d gates, the problem has %d", f.n, n);
@@ -2837,6 +2878,47 @@ int sbg_enum_depth_counts(sbg_handle *h, uint64_t *out, uint32_t nbins) {
       L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   h->d2h_bytes += nbins * sizeof(uint64_t);
+  return SBG_OK;
+}
+
+int sbg_inner_table(const uint64_t *inner, uint8_t *out) {
+  if (out == nullptr) return SBG_ERR_ARG;
+  memset(out, 0, kMinpos3);
+  int p3[256];
+  for (int x = 0; x < 256; x++) {
+    p3[x] = 0;
+    for (int c = 7; c >= 0; c--) p3[x] = 3 * p3[x] + ((x >> c) & 1);
+  }
+  for (int f = 0; f < 256; f++) {
+    if (inner != nullptr && ((inner[f >> 6] >> (f & 63)) & 1u) == 0) continue;
+    for (int seen = 0; seen < 256; seen++) out[p3[seen] + p3[f & seen]] = 1;
+  }
+  return SBG_OK;
+}
+
+int sbg_enum_set_functions(sbg_handle *h, const uint64_t *outer, const uint64_t *middle,
+    const uint64_t *inner) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
+  FunctionFilter &f = h->functions;
+  if (outer == nullptr && middle == nullptr && inner == nullptr) {
+    f.on = false;
+    return SBG_OK;
+  }
+  memset(&f.fn, 0, sizeof(f.fn));
+  const uint64_t *sets[2] = {outer, middle};
+  for (int r = 0; r < 2; r++) {
+    for (int w = 0; w < 8; w++) {
+      f.fn.sets[8 * r + w] = sets[r] == nullptr ? 0xffffffffu
+          : (uint32_t)(sets[r][w >> 1] >> (32 * (w & 1)));
+    }
+  }
+  uint8_t table[kMinpos3];
+  sbg_inner_table(inner, table);
+  for (int c = 0; c < kMinpos3; c++) f.fn.sets[16 + (c >> 5)] |= (uint32_t)table[c] << (c & 31);
+  f.fn.inner_all = inner == nullptr
+      || (inner[0] & inner[1] & inner[2] & inner[3]) == ~0ull;
+  f.on = true;
   return SBG_OK;
 }
 

@@ -370,9 +370,11 @@ __device__ __forceinline__ void summary5(const uint32_t *s_tabs, int npad, const
 }
 
 // Ordering k of a tuple with summary H1 / H0: ok[hi] bit lane and ok[7 - hi] bit 31 - lane both
-// set <=> outer function hi*32+lane decomposes.
-__device__ __forceinline__ void outer_ok5(uint32_t H1, uint32_t H0, int k, int lane,
-    const DevTables *__restrict__ tab, uint32_t *ok) {
+// set <=> outer function hi*32+lane decomposes.  rr[hi] (lane's): the inner cells (1, d, e) of
+// outer function fo = hi*32+lane, bits 0-3 = cells d<<1 | e with a masked 1, bits 4-7 = with a
+// masked 0; the cells (0, d, e) of fo are those of ~fo, rr[7 - hi] of lane 31 - lane.
+__device__ __forceinline__ void outer_ok5_rr(uint32_t H1, uint32_t H0, int k, int lane,
+    const DevTables *__restrict__ tab, uint32_t *ok, uint32_t *rr_out) {
   const int s = tab->src5[k][lane];
   const uint32_t b1 = __ballot_sync(kFull, (H1 >> s) & 1u);
   const uint32_t b0 = __ballot_sync(kFull, (H0 >> s) & 1u);
@@ -390,9 +392,16 @@ __device__ __forceinline__ void outer_ok5(uint32_t H1, uint32_t H0, int k, int l
     if (hi & 1) rr |= SBG_W5(5);
     if (hi & 2) rr |= SBG_W5(6);
     if (hi & 4) rr |= SBG_W5(7);
+    rr_out[hi] = rr;
     ok[hi] = __ballot_sync(kFull, ((rr & (rr >> 4)) & 0xfu) == 0);
   }
 #undef SBG_W5
+}
+
+__device__ __forceinline__ void outer_ok5(uint32_t H1, uint32_t H0, int k, int lane,
+    const DevTables *__restrict__ tab, uint32_t *ok) {
+  uint32_t rr[8];
+  outer_ok5_rr(H1, H0, k, lane, tab, ok, rr);
 }
 
 template <int NW>
@@ -2939,16 +2948,91 @@ __device__ __forceinline__ int depth7(const int *d7, int k) {
   return max(2 + m6, 1 + dg);
 }
 
+// ---- function filter (sbg_enum_set_functions) --------------------------------------------------
+// The function-filtered forms (k_enum3_fn / k_enum5_fn / k_enum7_fn) keep only the matches whose
+// outer LUT lies in the outer set, whose middle LUT lies in the middle set, and whose inner LUT can
+// be completed inside the inner set: some f in it has (f & inner_seen) == func_inner.  The last
+// test is a lookup in the inner table, indexed by minpos3's code(seen, ones) = p3(seen) + p3(ones).
+// The sets are indexed by function value, as the survivor words of k_enum5 / k_enum7 and
+// cube_union's set over fm are, so the outer and middle tests are ANDs with 8 words.  These forms
+// also take the depth filter: without one the host gives every gate depth 0 and the bound
+// kDepthBins - 1, which keeps every match and prunes nothing, and depth_on = 0 skips the histogram.
+constexpr int kInnerWords = (kMinpos3 + 31) / 32;
+struct EnumFunc {
+  uint32_t sets[16 + kInnerWords];   // words 0-7: outer set, 8-15: middle set, then the inner table
+  int inner_all;                     // the inner set holds all 256 functions (the table is all ones)
+  int depth_on;                      // a depth filter is installed: fill its histogram
+};
+
+__device__ __forceinline__ uint32_t *func_smem() {
+  __shared__ uint32_t s_func[16 + kInnerWords];
+  return s_func;
+}
+
+// The sets to shared memory; the kernel's __syncthreads after its own staging covers these stores.
+__device__ __forceinline__ const uint32_t *stage_func(const EnumFunc &fn) {
+  uint32_t *s = func_smem();
+  for (int i = threadIdx.x; i < 16 + kInnerWords; i += blockDim.x) s[i] = fn.sets[i];
+  return s;
+}
+
+__device__ __forceinline__ bool in_set(const uint32_t *set, uint32_t f) {
+  return (set[f >> 5] >> (f & 31u)) & 1u;
+}
+
+// Whether an inner LUT with solved bits `ones` over the cells `seen` completes inside the inner set.
+__device__ __forceinline__ bool inner_ok(const uint32_t *s_fn, uint32_t seen, uint32_t ones) {
+  uint32_t code = 0;
+#pragma unroll
+  for (int c = 7; c >= 0; c--) code = 3 * code + ((seen >> c) & 1u) + ((ones >> c) & 1u);
+  return in_set(s_fn + 16, code);
+}
+
+// The 5-LUT inner test of outer function fo, from rr1 = its rr (the x = 1 cells) and rr0 = the rr
+// of ~fo (the x = 0 cells); see outer_ok5_rr.
+__device__ __forceinline__ bool inner_ok5(const uint32_t *s_fn, uint32_t rr1, uint32_t rr0) {
+  const uint32_t ones = ((rr1 & 0xfu) << 4) | (rr0 & 0xfu);
+  const uint32_t zeros = (rr1 & 0xf0u) | ((rr0 >> 4) & 0xfu);
+  return inner_ok(s_fn, ones | zeros, ones);
+}
+
+// The 7-LUT inner cells of one outer function (r1 / r0 as for middle_cubes) and ordering row (b):
+// for the four (x, g), A = the middle patterns with a masked 1 in cell (x, *, g), B = with a masked
+// 0 (middle_cubes' A and B before it drops the inactive ones).
+__device__ __forceinline__ void inner_cells7(uint32_t r1, uint32_t r0, int b, uint32_t *AB) {
+#pragma unroll
+  for (int ci = 0; ci < 4; ci++) AB[ci] = compress16x2((ci & 2) ? r1 : r0, b, ci & 1);
+}
+
+// The 7-LUT inner test of middle function fm: inner cell (x, y, g) holds a masked 1 iff fm sends a
+// pattern of A to y, a masked 0 likewise with B.
+__device__ __forceinline__ bool inner_ok7(const uint32_t *s_fn, const uint32_t *AB, uint32_t fm) {
+  uint32_t ones = 0, seen = 0;
+#pragma unroll
+  for (int ci = 0; ci < 4; ci++) {
+    const uint32_t c0 = (ci & 2) << 1 | (ci & 1);   // cell x<<2 | 0<<1 | g
+    const uint32_t A = AB[ci] & 0xffu, B = AB[ci] >> 16;
+    if (A & fm) ones |= 1u << (c0 | 2);
+    if (A & ~fm) ones |= 1u << c0;
+    if ((A | B) & fm) seen |= 1u << (c0 | 2);
+    if ((A | B) & ~fm) seen |= 1u << c0;
+  }
+  return inner_ok(s_fn, seen, ones);
+}
+
 // The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
 // 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
 // feasible tuple and ordering the set of working outer functions from outer_ok5.  DF: the depth
 // filter (see depth5); `feasible` then counts the feasible tuples with an ordering within the bound.
-template <int NW, int MODE, bool DF>
-__global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+// FF: the function filter (see EnumFunc), applied to the survivor words of each ordering, so the
+// emit loop sees only the outer functions the count pass counted.
+template <int NW, int MODE, bool DF, bool FF>
+__device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders &ord, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn) {
+  static_assert(DF || !FF, "the function-filtered form carries the depth filter");
   constexpr int P = 3, K = 5, NC = 1 << P;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[256];
@@ -2963,6 +3047,12 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
   const uint16_t *s_dep = nullptr;
   if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
   const int B = depth_bound(dep);
+  const uint32_t *s_fn = nullptr;
+  bool inner_all = true;
+  if constexpr (FF) {
+    s_fn = stage_func(*fn);
+    inner_all = fn->inner_all != 0;
+  }
   __syncthreads();
   uint32_t T[NW], M[NW];
 #pragma unroll
@@ -3066,17 +3156,30 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
               if (kd > B) continue;
             }
             uint32_t ok[8], surv_mine = 0;
-            outer_ok5(H1, H0, k, lane, tab, ok);
+            uint32_t rr[8];
+            if constexpr (FF) outer_ok5_rr(H1, H0, k, lane, tab, ok, rr);
+            else outer_ok5(H1, H0, k, lane, tab, ok);
             uint32_t c = 0;
 #pragma unroll
             for (int hi = 0; hi < 8; hi++) {
-              const uint32_t surv = ok[hi] & __brev(ok[7 - hi]);
+              uint32_t surv = ok[hi] & __brev(ok[7 - hi]);
+              if constexpr (FF) {
+                surv &= s_fn[hi];
+                if (!inner_all) {
+                  const uint32_t rr0 = __shfl_sync(kFull, rr[7 - hi], 31 - lane);
+                  surv &= __ballot_sync(kFull, inner_ok5(s_fn, rr[hi], rr0));
+                }
+              }
               c += __popc(surv);
               if (lane == hi) surv_mine = surv;
             }
             if (MODE == kEnumCount) {
               tk.count += c;
-              if (DF && lane == 0 && c != 0) hist_add(kd, c);
+              if constexpr (FF) {
+                if (fn->depth_on && lane == 0 && c != 0) hist_add(kd, c);
+              } else {
+                if (DF && lane == 0 && c != 0) hist_add(kd, c);
+              }
               continue;
             }
             if (c == 0) continue;
@@ -3097,6 +3200,26 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
     }
   });
   flush_hist<MODE>(dep);
+}
+
+template <int NW, int MODE, bool DF>
+__global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
+  enum5_body<NW, MODE, DF, false>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
+      part, nparts, tab, dep, nullptr);
+}
+
+template <int NW, int MODE>
+__global__ void __launch_bounds__(kThreads) k_enum5_fn(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn) {
+  enum5_body<NW, MODE, true, true>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
+      part, nparts, tab, dep, &fn);
 }
 
 // Middle functions of one cube set (see middle_cubes) as a 256-bit set over fm, word wd = fm >> 5.
@@ -3129,13 +3252,18 @@ __device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (
 // the middle-function cubes.  Count: one lane per outer function; emit: positions in ascending
 // order, outer position in the loop, middle position across the lanes.  DF: the depth filter (see
 // depth7); an entry without an ordering within the bound is skipped, and so is every row above it.
-template <int NW, int MODE, bool DF>
-__global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
+// FF: the function filter (see EnumFunc).  The outer set cuts the survivors, the middle set the
+// cube union.  A restricted inner set depends on the whole of fm, not only on its cube, so the
+// count pass then runs the emit loop (positions over the lanes) in place of the popcounts, and
+// both passes apply inner_ok7 to each lane's (fo, fm).
+template <int NW, int MODE, bool DF, bool FF>
+__device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders &ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn) {
+  static_assert(DF || !FF, "the function-filtered form carries the depth filter");
   constexpr bool EMIT = MODE != kEnumCount;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
@@ -3153,6 +3281,12 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
   const uint16_t *s_dep = nullptr;
   if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
   const int B = depth_bound(dep);
+  const uint32_t *s_fn = nullptr;
+  bool slow = false;   // FF with a restricted inner set: the count pass runs the emit loop
+  if constexpr (FF) {
+    s_fn = stage_func(*fn);
+    slow = fn->inner_all == 0;
+  }
   __syncthreads();
   uint32_t T[NW], M[NW];
 #pragma unroll
@@ -3199,14 +3333,15 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
         uint32_t any = 0, surv_mine = 0;
 #pragma unroll
         for (int hi = 0; hi < 8; hi++) {
-          const uint32_t sv = ok[hi] & __brev(ok[7 - hi]);
+          uint32_t sv = ok[hi] & __brev(ok[7 - hi]);
+          if constexpr (FF) sv &= s_fn[hi];
           any |= sv;
           if (lane == hi) surv_mine = sv;
         }
         if (any == 0) continue;
         const int k0 = c_j_first_k[j];
         const int nrows = c_j_rows[j];
-        if (!EMIT) {
+        if (!EMIT && !slow) {
           int ns = 0;
           __syncwarp();
 #pragma unroll
@@ -3237,9 +3372,18 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
               bool hok[2][4];
               middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
               cube_union(hv, hok, S, ov, bits);
+              if constexpr (FF) {
+#pragma unroll
+                for (int wd = 0; wd < 8; wd++) bits[wd] &= s_fn[8 + wd];
+              }
 #pragma unroll
               for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd]);
-              if constexpr (DF) {
+              if constexpr (FF) {
+                if (fn->depth_on) {
+                  const uint32_t s = __reduce_add_sync(kFull, have ? c - c_before : 0u);
+                  if (lane == 0 && s != 0) hist_add(rd, s);
+                }
+              } else if constexpr (DF) {
                 // rows differ in depth: each row's matches go to its own bin
                 const uint32_t s = __reduce_add_sync(kFull, have ? c - c_before : 0u);
                 if (lane == 0 && s != 0) hist_add(rd, s);
@@ -3249,9 +3393,10 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
           }
         }
 #pragma unroll 1
-        for (int row = 0; EMIT && row < nrows && !done; row++) {
+        for (int row = 0; (EMIT || slow) && row < nrows && !done; row++) {
           const int k = k0 + row;
           if (DF && depth7(d7, k) > B) continue;
+          [[maybe_unused]] const uint32_t row_start = tk.count;
 #pragma unroll 1
           for (int po = 0; po < 256 && !done; po++) {
             const uint32_t fo = s_ord[0][po];
@@ -3264,6 +3409,8 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
             uint32_t hv[2][4], S, ov;
             bool hok[2][4];
             middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
+            [[maybe_unused]] uint32_t AB[4] = {0, 0, 0, 0};
+            if (FF && slow) inner_cells7(r1, r0, c_row_b[k], AB);
             const unsigned long long key_hi = (idx << 23) | ((uint64_t)k << 16) | ((uint64_t)po << 8);
 #pragma unroll 1
             for (int w = 0; w < 8; w++) {
@@ -3278,9 +3425,16 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
                       && (fm & S) == (hv[0][c0] | hv[1][c1]);
                 }
               }
+              if constexpr (FF) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
               done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
                 write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
               });
+            }
+          }
+          if constexpr (FF && MODE == kEnumCount) {
+            // the slow count pass: this row's matches to its depth's bin
+            if (fn->depth_on && lane == 0 && tk.count != row_start) {
+              hist_add(depth7(d7, k), tk.count - row_start);
             }
           }
         }
@@ -3288,6 +3442,28 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
     }
   });
   flush_hist<MODE>(dep);
+}
+
+template <int NW, int MODE, bool DF>
+__global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
+    unsigned int list_count, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
+  enum7_body<NW, MODE, DF, false>(prob, ectl, ord, list, list_count, counts, offsets, out, max_out,
+      t_begin, t_end, part, nparts, tab, dep, nullptr);
+}
+
+template <int NW, int MODE>
+__global__ void __launch_bounds__(kThreads) k_enum7_fn(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
+    unsigned int list_count, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn) {
+  enum7_body<NW, MODE, true, true>(prob, ectl, ord, list, list_count, counts, offsets, out, max_out,
+      t_begin, t_end, part, nparts, tab, dep, &fn);
 }
 
 
@@ -3304,13 +3480,16 @@ struct EnumGateOrder {
 // ticket's matches are consecutive keys in the order of its lanes.  A match's record: the gates in
 // position order, func_inner = cells holding a masked 1, inner_seen = cells holding a masked
 // position (sbg_solve_inner's closed form).  DF: the depth filter; a pair with a gate of depth
-// >= max_depth is skipped.
-template <int NW, int MODE, bool DF>
-__global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
+// >= max_depth is skipped.  FF: the function filter; the lane's (seen, ones) must complete inside
+// the inner set.  `feasible` then counts the triples within the depth bound, whatever their
+// function (the matches of the unfiltered or depth-filtered count).
+template <int NW, int MODE, bool DF, bool FF>
+__device__ __forceinline__ void enum3_body(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumGateOrder &go, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const EnumDepth<DF> dep) {
+    int nparts, const EnumDepth<DF> &dep, const EnumFunc *fn) {
+  static_assert(DF || !FF, "the function-filtered form carries the depth filter");
   extern __shared__ uint32_t smem[];
   __shared__ uint16_t s_order[kMaxGatesPad];
   const int lane = threadIdx.x & 31;
@@ -3322,6 +3501,8 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
   const uint16_t *s_dep = nullptr;
   if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
   const int B = depth_bound(dep);
+  const uint32_t *s_fn = nullptr;
+  if constexpr (FF) s_fn = stage_func(*fn);
   __syncthreads();
   uint32_t T[NW], Z[NW];   // masked positions with target 1 / with target 0
 #pragma unroll
@@ -3332,7 +3513,7 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
   const uint64_t pairs = (uint64_t)(n * (n - 1) / 2);
 
   enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
-      [&](unsigned long long t, EnumTicket &tk, unsigned long long &) {
+      [&](unsigned long long t, EnumTicket &tk, [[maybe_unused]] unsigned long long &feasible) {
     const uint64_t dealt = dealt_item(t, part, nparts);
     if (dealt < pairs) {
       int pi, pk;
@@ -3372,7 +3553,11 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
         if constexpr (DF) {
           const int dm = 1 + max(dab, (int)s_dep[s_order[pm < n ? pm : pk]]);
           ok &= dm <= B;
-          if (MODE == kEnumCount) {
+          if constexpr (FF) {
+            if (MODE == kEnumCount) feasible += __popc(__ballot_sync(kFull, ok));
+            ok = ok && inner_ok(s_fn, seen, ones);
+          }
+          if (MODE == kEnumCount && (!FF || fn->depth_on)) {
             // one histogram atomic per distinct depth of the ballot, by its lowest lane
             const uint32_t peers = __match_any_sync(kFull, ok ? dm : -1);
             if (ok && (peers & lanemask_lt()) == 0) hist_add(dm, __popc(peers));
@@ -3387,6 +3572,26 @@ __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict
     }
   });
   flush_hist<MODE>(dep);
+}
+
+template <int NW, int MODE, bool DF>
+__global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const EnumDepth<DF> dep) {
+  enum3_body<NW, MODE, DF, false>(prob, ectl, go, counts, offsets, out, max_out, t_begin, t_end,
+      part, nparts, dep, nullptr);
+}
+
+template <int NW, int MODE>
+__global__ void __launch_bounds__(kThreads) k_enum3_fn(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const EnumDepth<true> dep, const EnumFunc fn) {
+  enum3_body<NW, MODE, true, true>(prob, ectl, go, counts, offsets, out, max_out, t_begin, t_end,
+      part, nparts, dep, &fn);
 }
 
 

@@ -279,6 +279,15 @@ class DistributedLutSearch:
     def clear_depth_filter(self):
         self.engine.clear_depth_filter()
 
+    # -- function filter -------------------------------------------------------------------------
+    def set_function_filter(self, outer=None, middle=None, inner=None):
+        """The engine's function filter (LutEngine.set_function_filter), on every rank: later
+        enumerations count, rank and fetch within the matches whose LUTs lie in the sets."""
+        self.engine.set_function_filter(outer, middle, inner)
+
+    def clear_function_filter(self):
+        self.engine.clear_function_filter()
+
     def depth_counts(self):
         """The whole's matches per depth of the last enumerate* call (counted under a filter):
         one all-reduce(SUM) of the ranks' histograms.  Trimmed after the last non-empty bin."""

@@ -511,6 +511,38 @@ class LutEngine:
                                                    SBG_DEPTH_BINS))
         return _trim(out)
 
+    # -- function filter: the realisations whose LUTs lie in given sets of functions -------------
+    def set_function_filter(self, outer=None, middle=None, inner=None):
+        """Later enumerate3/5/7 calls keep only the matches whose LUTs lie in the given sets of
+        3-input functions (iterables of function numbers 0..255, None = all 256; see
+        match_functions_allowed): the outer LUT in `outer` (5- and 7-LUT), the middle LUT in
+        `middle` (7-LUT), and the inner LUT completable inside `inner`.  Combines with the depth
+        filter.  Ends the cursor.  The searches never read the filter."""
+        sets = [_function_set(s, r) for s, r in ((outer, "outer"), (middle, "middle"),
+                                                  (inner, "inner"))]
+        if all(s is None for s in sets):
+            # all three given as None: a filter that keeps everything, i.e. none
+            self.clear_function_filter()
+            return
+        ptrs = [None if s is None else s.ctypes.data_as(native.u64p) for s in sets]
+        self._check(self.lib.sbg_enum_set_functions(self._h, *ptrs))
+
+    def clear_function_filter(self):
+        """Removes the function filter.  Ends the cursor."""
+        self._check(self.lib.sbg_enum_set_functions(self._h, None, None, None))
+
+
+def inner_table(inner=None):
+    """sbg_inner_table: a uint8 array of 6,561 entries, entry p3(seen) + p3(ones) = 1 iff some
+    function of `inner` (None: all 256) has (f & seen) == ones."""
+    lib = native.load_library()
+    s = _function_set(inner, "inner")
+    out = np.zeros(6561, dtype=np.uint8)
+    ptr = None if s is None else s.ctypes.data_as(native.u64p)
+    if lib.sbg_inner_table(ptr, out.ctypes.data_as(C.POINTER(C.c_uint8))) != 0:
+        raise NativeLibraryError("sbg_inner_table failed")
+    return out
+
 
 def _depth_args(depth, max_depth):
     """A depth filter's arguments, checked: (uint16 array of the gate depths, bound)."""
@@ -569,6 +601,95 @@ def shallowest_matches(engine, width, orders, depth, max_matches):
     engine.set_depth_filter(depth, dmin)
     e = run(*orders, max_matches)
     return dmin, int(e.total), e.matches
+
+
+# -- function filter: the realisations whose LUTs lie in given sets of functions -----------------
+# 3-input functions are numbered as for lut_table: bit in1 << 2 | in2 << 1 | in3 of the number is
+# the output.  The truth tables of the three inputs in that numbering:
+_IN3 = (0xF0, 0xCC, 0xAA)
+
+
+def _affine_functions():
+    out = set()
+    for c in range(2):
+        for sel in range(8):
+            f = 0xFF if c else 0
+            for i in range(3):
+                if (sel >> i) & 1:
+                    f ^= _IN3[i]
+            out.add(f)
+    return frozenset(out)
+
+
+AFFINE_FUNCTIONS = _affine_functions()
+"""The 16 3-input functions of algebraic degree <= 1: constants, inputs and their XORs, and their
+complements (cheap under masking, MPC and FHE)."""
+
+
+def gate_functions(available_gates):
+    """The 3-input functions one two-input gate computes: graph.gate2_table(t, x, y) for a gate
+    type t whose bit is set in `available_gates` (the reference's --available-gates bitfield over
+    the 16 types of graph.GATE_NAMES) and x, y any of the LUT's three inputs, equal ones included
+    (so a gate that passes or inverts an input, or gives a constant, counts as itself).  194 is
+    AND, OR and XOR."""
+    from .graph import gate2_table
+    available_gates = int(available_gates)
+    if not 0 <= available_gates < 1 << 16:
+        raise ValueError("available_gates must be a 16-bit gate-type bitfield")
+    out = set()
+    for t in range(16):
+        if (available_gates >> t) & 1:
+            for x in _IN3:
+                for y in _IN3:
+                    out.add(gate2_table(t, x, y) & 0xFF)
+    return frozenset(out)
+
+
+def _function_set(funcs, role):
+    """A function filter role, checked: None (all 256) or the 4-word uint64 bitmap of a set."""
+    if funcs is None:
+        return None
+    if isinstance(funcs, (str, bytes)):
+        raise ValueError("%s must be an iterable of function numbers" % role)
+    words = np.zeros(4, dtype=np.uint64)
+    for f in funcs:
+        if isinstance(f, (bool, np.bool_)) or not isinstance(f, (int, np.integer)):
+            raise ValueError("%s: function numbers must be integers, not %r" % (role, f))
+        f = int(f)
+        if not 0 <= f < 256:
+            raise ValueError("%s: function %d outside 0..255" % (role, f))
+        words[f >> 6] |= np.uint64(1 << (f & 63))
+    return words
+
+
+def inner_completes(func_inner, inner_seen, f):
+    """Whether function f agrees with an inner LUT's solved bits: (f & inner_seen) == func_inner."""
+    return (int(f) & int(inner_seen)) == int(func_inner)
+
+
+def allowed_fill(func_inner, inner_seen, inner=None):
+    """The smallest function of `inner` (None: all 256) that completes an inner LUT's solved bits
+    (func_inner over the cells inner_seen), or None if none does.  With it a caller builds a circuit
+    whose LUTs all lie in the filter's sets; match_to_ret's random fill may leave `inner`."""
+    cands = range(256) if inner is None else sorted(int(f) for f in inner)
+    for f in cands:
+        if inner_completes(func_inner, inner_seen, f):
+            return f
+    return None
+
+
+def match_functions_allowed(record, outer=None, middle=None, inner=None):
+    """The function filter's test on one enumerated match (a MATCH_DTYPE record), sets as for
+    LutEngine.set_function_filter (None: all 256): func_outer in outer (5- and 7-LUT), func_middle
+    in middle (7-LUT), and allowed_fill finds an inner function."""
+    width = int(record["width"])
+    if width not in (3, 5, 7):
+        raise ValueError("not a match record (width %d)" % width)
+    if width > 3 and outer is not None and int(record["func_outer"]) not in set(outer):
+        return False
+    if width == 7 and middle is not None and int(record["func_middle"]) not in set(middle):
+        return False
+    return allowed_fill(record["func_inner"], record["inner_seen"], inner) is not None
 
 
 def _torch_stream_done(t):

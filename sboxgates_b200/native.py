@@ -113,6 +113,8 @@ SIGNATURES = {
     "sbg_enum_set_global": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, u64p, C.c_int, u64p]),
     "sbg_enum_set_depth": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint16), C.c_int, C.c_uint32]),
     "sbg_enum_depth_counts": (C.c_int, [C.c_void_p, u64p, C.c_uint32]),
+    "sbg_enum_set_functions": (C.c_int, [C.c_void_p, u64p, u64p, u64p]),
+    "sbg_inner_table": (C.c_int, [u64p, C.POINTER(C.c_uint8)]),
 }
 
 _lib = None
