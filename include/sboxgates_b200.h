@@ -293,6 +293,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
        sbg_enum_set_global and sbg_enum_depth_counts keep it;
      - sbg_enum_set_depth ends it, whatever the call returns.
      - sbg_enum_set_functions ends it, whatever the call returns.
+     - sbg_enum_set_grouping ends it, whatever the call returns.
    Without a cursor both calls return SBG_ERR_STATE.
    A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
    a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT) or a list
@@ -397,6 +398,29 @@ int sbg_enum_set_functions(sbg_handle *h, const uint64_t *outer, const uint64_t 
    every ones within seen; code(S, V) = p3(S) + p3(V), p3(x) = the sum of 3^j over the set bits j
    of x (6,561 entries). */
 int sbg_inner_table(const uint64_t *inner, uint8_t *out);
+
+/* ---- grouping: the distinct gate sets and wirings that realise a state ----------------------- */
+/* A realisation (one key) fixes the gates, the ordering row and the functions of the LUTs.  Under a
+   grouping, sbg_enum3 / sbg_enum5 / sbg_enum7 enumerate groups of matches instead: the matches
+   sharing a key prefix,
+     SBG_GROUP_SHAPE: the gates and the ordering row (the wiring): 5-LUT key >> 8, 7-LUT key >> 16;
+     SBG_GROUP_TUPLE: the gate set: 5-LUT key >> 12, 7-LUT key >> 23.
+   A 3-LUT key already is its gate set and wiring, so at width 3 every grouping is the identity.
+   The total is the number of groups holding at least one match (after the depth and function
+   filters); each group has one record, its first match (smallest key), byte-identical to the
+   ungrouped record of that key, in ascending key order; ranks count groups.  The cursor keeps the
+   grouping it was counted under, so fetch, pick, the count-free first K, sbg_enum_block_sums and
+   sbg_enum_set_global serve the grouped set.  *feasible keeps its meaning, the 7-LUT list is still
+   the phase-1 list, and searches never read the setting.  sbg_enum_depth_counts bins each group
+   once, at the depth of its record: every match of a shape has the same depth, but a gate set's
+   record is its first match, which need not be its shallowest (a histogram by shallowest gate set
+   needs no grouping or shape grouping).  How many matches a group holds is not reported. */
+#define SBG_GROUP_NONE 0    /* every match (the default) */
+#define SBG_GROUP_SHAPE 1   /* one per (gates, ordering row) */
+#define SBG_GROUP_TUPLE 2   /* one per gate set */
+/* Sets the grouping of the later sbg_enum3 / sbg_enum5 / sbg_enum7 calls on the handle.  Any other
+   value: SBG_ERR_ARG, with the setting left as it was.  The call ends the cursor. */
+int sbg_enum_set_grouping(sbg_handle *h, int grouping);
 
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense

@@ -13,7 +13,7 @@ from .lut import LutEngine, SearchResult, NO_GATE, search_5lut, search_7lut, shu
     Enumeration, enumerate_3lut, enumerate_5lut, enumerate_7lut, enumerate_lut_search, \
     match_to_ret, match_to_lut3, decode_key3, decode_key5, decode_key7, sample_matches, \
     match_depth, shallowest_matches, AFFINE_FUNCTIONS, gate_functions, match_functions_allowed, \
-    allowed_fill, inner_table
+    allowed_fill, inner_table, match_group
 from .native import load_library, NativeLibraryError, MATCH_DTYPE, SBG_MAX_DEPTH, SBG_DEPTH_BINS
 
 __all__ = [
@@ -23,5 +23,6 @@ __all__ = [
     "enumerate_7lut", "enumerate_lut_search", "match_to_ret", "match_to_lut3", "decode_key3",
     "decode_key5", "decode_key7", "sample_matches", "match_depth", "shallowest_matches",
     "AFFINE_FUNCTIONS", "gate_functions", "match_functions_allowed", "allowed_fill", "inner_table",
+    "match_group",
     "MATCH_DTYPE", "SBG_MAX_DEPTH", "SBG_DEPTH_BINS", "load_library", "NativeLibraryError",
 ]

@@ -173,7 +173,8 @@ struct sbg_lane {
 // (widths 5 and 7) or the gate order (width 3), the depth filter if one was installed
 // (sbg_enum_set_depth; its histogram pointer is the lane's, set at launch), and the function
 // filter if one was installed (sbg_enum_set_functions; with it, depth holds the neutral filter
-// when `filtered` is false).
+// when `filtered` is false), and the grouping (sbg_enum_set_grouping; under a grouping of width 5
+// or 7 the grouped forms run, with the neutral depth and function filters for those not installed).
 struct EnumInputs {
   EnumOrders ord;
   EnumGateOrder gates;
@@ -181,6 +182,7 @@ struct EnumInputs {
   EnumDepth<true> depth;
   bool fn_on;
   EnumFunc fn;
+  int grouping;
 };
 
 // The depth filter of a handle (sbg_enum_set_depth): the depths of n gates and the bound.
@@ -280,6 +282,7 @@ struct sbg_handle {
   EnumCursor cursor;
   DepthFilter filter;   // read by sbg_enum3 / sbg_enum5 / sbg_enum7 only
   FunctionFilter functions;   // likewise
+  int grouping = SBG_GROUP_NONE;   // likewise (sbg_enum_set_grouping)
 };
 
 namespace {
@@ -1514,6 +1517,22 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
             h->d_tab, dep);
       }
     };
+    if constexpr (WIDTH != 3) {
+      if (in.grouping != SBG_GROUP_NONE) {
+        // the grouped form, with the installed filters or the neutral ones
+        EnumDepth<true> dep = in.depth;
+        dep.hist = L.d_ehist;
+        if constexpr (WIDTH == 5) {
+          return run(k_enum5_gr<NW, MODE>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
+              L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, dep, in.fn,
+              in.grouping);
+        } else {
+          return run(k_enum7_gr<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
+              L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts,
+              h->d_tab, dep, in.fn, in.grouping);
+        }
+      }
+    }
     if (!in.filtered && !in.fn_on) return run_form(std::false_type(), EnumDepth<false>());
     EnumDepth<true> dep = in.depth;
     dep.hist = L.d_ehist;
@@ -1581,7 +1600,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   if ((rc = grow(h, L, L.d_ecount, L.ecount_cap, room)) != SBG_OK) return rc;
   if ((rc = grow(h, L, L.d_eoffset, L.eoffset_cap, room)) != SBG_OK) return rc;
   SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
-  if (in.filtered || in.fn_on) {
+  if (in.filtered || in.fn_on || (WIDTH != 3 && in.grouping != SBG_GROUP_NONE)) {
     if ((rc = grow(h, L, L.d_ehist, L.ehist_cap, (uint64_t)kDepthBins)) != SBG_OK) return rc;
     SBG_CUDA(h, cudaMemsetAsync(L.d_ehist, 0, kDepthBins * sizeof(unsigned long long), L.stream));
   }
@@ -1653,18 +1672,42 @@ int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, s
   return SBG_OK;
 }
 
-// The handle's depth and function filters, if any, into the inputs of an sbg_enum* call on the
-// current problem.
+// A function filter's sets (host memory, 4 words each; NULL = all 256 functions) as the kernels read
+// them (EnumFunc); all three NULL gives the filter that keeps every match.
+void make_functions(const uint64_t *outer, const uint64_t *middle, const uint64_t *inner,
+    EnumFunc &fn) {
+  memset(&fn, 0, sizeof(fn));
+  const uint64_t *sets[2] = {outer, middle};
+  for (int r = 0; r < 2; r++) {
+    for (int w = 0; w < 8; w++) {
+      fn.sets[8 * r + w] = sets[r] == nullptr ? 0xffffffffu
+          : (uint32_t)(sets[r][w >> 1] >> (32 * (w & 1)));
+    }
+  }
+  uint8_t table[kMinpos3];
+  sbg_inner_table(inner, table);
+  for (int c = 0; c < kMinpos3; c++) fn.sets[16 + (c >> 5)] |= (uint32_t)table[c] << (c & 31);
+  fn.inner_all = inner == nullptr
+      || (inner[0] & inner[1] & inner[2] & inner[3]) == ~0ull;
+}
+
+// The handle's depth and function filters, if any, and its grouping into the inputs of an sbg_enum*
+// call on the current problem.  The forms that carry both filters (function-filtered or grouped)
+// get the neutral ones in place of those not installed.
 int take_filter(sbg_handle *h, EnumInputs &in) {
   const DepthFilter &f = h->filter;
   in.filtered = f.on;
   in.fn_on = h->functions.on;
+  in.grouping = h->grouping;
+  const bool both = in.fn_on || in.grouping != SBG_GROUP_NONE;
   if (in.fn_on) {
     in.fn = h->functions.fn;
-    in.fn.depth_on = f.on;
+  } else if (both) {
+    make_functions(nullptr, nullptr, nullptr, in.fn);   // keeps every match
   }
+  if (both) in.fn.depth_on = f.on;
   if (!f.on) {
-    if (in.fn_on) {
+    if (both) {
       // the neutral depth filter: every gate at depth 0, a bound no match exceeds
       memset(&in.depth, 0, sizeof(in.depth));
       in.depth.max_depth = kDepthBins - 1;
@@ -2905,20 +2948,18 @@ int sbg_enum_set_functions(sbg_handle *h, const uint64_t *outer, const uint64_t 
     f.on = false;
     return SBG_OK;
   }
-  memset(&f.fn, 0, sizeof(f.fn));
-  const uint64_t *sets[2] = {outer, middle};
-  for (int r = 0; r < 2; r++) {
-    for (int w = 0; w < 8; w++) {
-      f.fn.sets[8 * r + w] = sets[r] == nullptr ? 0xffffffffu
-          : (uint32_t)(sets[r][w >> 1] >> (32 * (w & 1)));
-    }
-  }
-  uint8_t table[kMinpos3];
-  sbg_inner_table(inner, table);
-  for (int c = 0; c < kMinpos3; c++) f.fn.sets[16 + (c >> 5)] |= (uint32_t)table[c] << (c & 31);
-  f.fn.inner_all = inner == nullptr
-      || (inner[0] & inner[1] & inner[2] & inner[3]) == ~0ull;
+  make_functions(outer, middle, inner, f.fn);
   f.on = true;
+  return SBG_OK;
+}
+
+int sbg_enum_set_grouping(sbg_handle *h, int grouping) {
+  if (h == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
+  if (grouping != SBG_GROUP_NONE && grouping != SBG_GROUP_SHAPE && grouping != SBG_GROUP_TUPLE) {
+    return fail(h, SBG_ERR_ARG, "grouping %d is none of SBG_GROUP_NONE, _SHAPE, _TUPLE", grouping);
+  }
+  h->grouping = grouping;
   return SBG_OK;
 }
 

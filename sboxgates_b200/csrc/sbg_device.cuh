@@ -3020,19 +3020,34 @@ __device__ __forceinline__ bool inner_ok7(const uint32_t *s_fn, const uint32_t *
   return inner_ok(s_fn, seen, ones);
 }
 
+// ---- grouping (sbg_enum_set_grouping) ------------------------------------------------------------
+// The grouped forms (k_enum5_gr / k_enum7_gr) enumerate groups of matches instead of matches: the
+// matches sharing a key prefix, the gates and ordering row (kGroupShape: 5-LUT key >> 8, 7-LUT
+// key >> 16) or the gate set (kGroupTuple: key >> 12, key >> 23).  A group counts once if it holds
+// a match, and emits its first match (smallest key), the record the ungrouped forms emit for that
+// key.  A key prefix names a 3-gate prefix ticket's tuple (5-LUT) or a list entry (7-LUT), so no
+// group crosses a ticket, and the count and emit passes stop at the same first match of a group.
+// The grouped forms carry the depth and function filters (neutral when none is installed); the
+// kind is a warp-uniform runtime argument.
+constexpr int kGroupShape = 1, kGroupTuple = 2;   // SBG_GROUP_SHAPE, SBG_GROUP_TUPLE
+
 // The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
 // 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
 // feasible tuple and ordering the set of working outer functions from outer_ok5.  DF: the depth
 // filter (see depth5); `feasible` then counts the feasible tuples with an ordering within the bound.
 // FF: the function filter (see EnumFunc), applied to the survivor words of each ordering, so the
-// emit loop sees only the outer functions the count pass counted.
-template <int NW, int MODE, bool DF, bool FF>
+// emit loop sees only the outer functions the count pass counted.  GR: grouped (see "grouping"
+// above k_enum5_gr); a (tuple, ordering) counts once if its survivor set is not empty and emits its
+// lowest position, and under kGroupTuple the tuple ends there.
+template <int NW, int MODE, bool DF, bool FF, bool GR = false>
 __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders &ord, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn) {
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn,
+    int grouping = 0) {
   static_assert(DF || !FF, "the function-filtered form carries the depth filter");
+  static_assert(FF || !GR, "the grouped form carries both filters");
   constexpr int P = 3, K = 5, NC = 1 << P;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[256];
@@ -3170,8 +3185,18 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
                   surv &= __ballot_sync(kFull, inner_ok5(s_fn, rr[hi], rr0));
                 }
               }
-              c += __popc(surv);
+              if constexpr (GR) c |= surv;   // only whether the set is empty
+              else c += __popc(surv);
               if (lane == hi) surv_mine = surv;
+            }
+            if constexpr (GR) {
+              if (MODE == kEnumCount) {
+                if (c == 0) continue;
+                tk.count++;
+                if (fn->depth_on && lane == 0) hist_add(kd, 1);
+                if (grouping == kGroupTuple) break;
+                continue;
+              }
             }
             if (MODE == kEnumCount) {
               tk.count += c;
@@ -3189,10 +3214,23 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
             for (int w = 0; w < 8; w++) {
               const uint32_t pos = 32u * w + lane;
               const uint32_t fo = s_ord[pos];
-              const bool hit = (__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u;
+              bool hit = (__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u;
+              if constexpr (GR) {
+                // the group's record: its lowest position with a hit
+                const uint32_t bal = __ballot_sync(kFull, hit);
+                if (bal == 0) continue;
+                hit = hit && (bal & lanemask_lt()) == 0;
+                done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
+                  write_match<NW, 5>(out + i, key_hi | pos, g5, k, fo, 0, s_tabs, npad, T, M);
+                });
+                break;
+              }
               done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
                 write_match<NW, 5>(out + i, key_hi | pos, g5, k, fo, 0, s_tabs, npad, T, M);
               });
+            }
+            if constexpr (GR) {
+              if (grouping == kGroupTuple) break;
             }
           }
         }
@@ -3220,6 +3258,17 @@ __global__ void __launch_bounds__(kThreads) k_enum5_fn(const DevProblem *__restr
     int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn) {
   enum5_body<NW, MODE, true, true>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
       part, nparts, tab, dep, &fn);
+}
+
+template <int NW, int MODE>
+__global__ void __launch_bounds__(kThreads) k_enum5_gr(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn,
+    int grouping) {
+  enum5_body<NW, MODE, true, true, true>(prob, ectl, ord, counts, offsets, out, max_out, t_begin,
+      t_end, part, nparts, tab, dep, &fn, grouping);
 }
 
 // Middle functions of one cube set (see middle_cubes) as a 256-bit set over fm, word wd = fm >> 5.
@@ -3255,15 +3304,21 @@ __device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (
 // FF: the function filter (see EnumFunc).  The outer set cuts the survivors, the middle set the
 // cube union.  A restricted inner set depends on the whole of fm, not only on its cube, so the
 // count pass then runs the emit loop (positions over the lanes) in place of the popcounts, and
-// both passes apply inner_ok7 to each lane's (fo, fm).
-template <int NW, int MODE, bool DF, bool FF>
+// both passes apply inner_ok7 to each lane's (fo, fm).  GR: grouped (see "grouping" above
+// enum5_body).  The count pass takes a row once when some surviving outer function leaves a
+// non-empty cube union (rows outer, outer functions inner, stopping at the first); the emit loop
+// emits a row's first hit (first po, lowest pm) and moves to the next row.  Under kGroupTuple both
+// end the entry at its first row with a match.
+template <int NW, int MODE, bool DF, bool FF, bool GR = false>
 __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders &ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn) {
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn,
+    int grouping = 0) {
   static_assert(DF || !FF, "the function-filtered form carries the depth filter");
+  static_assert(FF || !GR, "the grouped form carries both filters");
   constexpr bool EMIT = MODE != kEnumCount;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
@@ -3351,6 +3406,38 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
             ns += __popc(sv);
           }
           __syncwarp();
+          if constexpr (GR) {
+#pragma unroll 1
+            for (int row = 0; row < nrows; row++) {
+              const int rd = depth7(d7, k0 + row);
+              if (rd > B) continue;
+              bool found = false;
+              for (int i0 = 0; i0 < ns && !found; i0 += 32) {
+                const bool have = i0 + lane < ns;
+                const int fo = have ? fo_list[i0 + lane] : 0;
+                uint32_t r1 = 0, r0 = 0;
+#pragma unroll
+                for (int u = 0; u < 8; u++) {
+                  if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
+                }
+                uint32_t hv[2][4], S, ov, bits[8], nz = 0;
+                bool hok[2][4];
+                middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
+                cube_union(hv, hok, S, ov, bits);
+#pragma unroll
+                for (int wd = 0; wd < 8; wd++) nz |= bits[wd] & s_fn[8 + wd];
+                found = __any_sync(kFull, have && nz != 0);
+              }
+              if (!found) continue;
+              tk.count++;
+              if (fn->depth_on && lane == 0) hist_add(rd, 1);
+              if (grouping == kGroupTuple) {
+                done = true;   // the entry is the group
+                break;
+              }
+            }
+            continue;
+          }
           for (int i0 = 0; i0 < ns; i0 += 32) {
             const bool have = i0 + lane < ns;
             const int fo = have ? fo_list[i0 + lane] : 0;
@@ -3397,6 +3484,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
           const int k = k0 + row;
           if (DF && depth7(d7, k) > B) continue;
           [[maybe_unused]] const uint32_t row_start = tk.count;
+          [[maybe_unused]] bool row_hit = false;   // GR: the row's group is emitted
 #pragma unroll 1
           for (int po = 0; po < 256 && !done; po++) {
             const uint32_t fo = s_ord[0][po];
@@ -3426,16 +3514,28 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
                 }
               }
               if constexpr (FF) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
+              if constexpr (GR) {
+                // the group's record: the first hit of the row
+                const uint32_t bal = __ballot_sync(kFull, hit);
+                if (bal == 0) continue;
+                hit = hit && (bal & lanemask_lt()) == 0;
+                row_hit = true;
+              }
               done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
                 write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
               });
+              if (GR && row_hit) break;
             }
+            if (GR && row_hit) break;
           }
           if constexpr (FF && MODE == kEnumCount) {
             // the slow count pass: this row's matches to its depth's bin
             if (fn->depth_on && lane == 0 && tk.count != row_start) {
               hist_add(depth7(d7, k), tk.count - row_start);
             }
+          }
+          if constexpr (GR) {
+            if (row_hit && grouping == kGroupTuple) done = true;   // the entry is the group
           }
         }
       }
@@ -3464,6 +3564,18 @@ __global__ void __launch_bounds__(kThreads) k_enum7_fn(const DevProblem *__restr
     int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn) {
   enum7_body<NW, MODE, true, true>(prob, ectl, ord, list, list_count, counts, offsets, out, max_out,
       t_begin, t_end, part, nparts, tab, dep, &fn);
+}
+
+template <int NW, int MODE>
+__global__ void __launch_bounds__(kThreads) k_enum7_gr(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
+    unsigned int list_count, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn,
+    int grouping) {
+  enum7_body<NW, MODE, true, true, true>(prob, ectl, ord, list, list_count, counts, offsets, out,
+      max_out, t_begin, t_end, part, nparts, tab, dep, &fn, grouping);
 }
 
 

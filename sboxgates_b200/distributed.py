@@ -288,6 +288,12 @@ class DistributedLutSearch:
     def clear_function_filter(self):
         self.engine.clear_function_filter()
 
+    # -- grouping --------------------------------------------------------------------------------
+    def set_grouping(self, grouping):
+        """The engine's grouping (LutEngine.set_grouping), on every rank: later enumerations count,
+        rank and fetch groups of matches (None, "shape" or "tuple")."""
+        self.engine.set_grouping(grouping)
+
     def depth_counts(self):
         """The whole's matches per depth of the last enumerate* call (counted under a filter):
         one all-reduce(SUM) of the ranks' histograms.  Trimmed after the last non-empty bin."""

@@ -531,6 +531,17 @@ class LutEngine:
         """Removes the function filter.  Ends the cursor."""
         self._check(self.lib.sbg_enum_set_functions(self._h, None, None, None))
 
+    # -- grouping: the distinct gate sets and wirings that realise a state -----------------------
+    def set_grouping(self, grouping):
+        """Later enumerate5/7 calls enumerate groups of matches (see match_group): None = every
+        match, "shape" = one per gate set and ordering row (the wiring), "tuple" = one per gate set.
+        A group counts if one of its matches passes the depth and function filters, and its record
+        is its first match, the ungrouped record of that key; ranks count groups.  enumerate3 is
+        unchanged (a 3-LUT key is its own group).  Ends the cursor.  The searches never read it."""
+        if grouping not in _GROUPINGS:
+            raise ValueError("grouping must be None, 'shape' or 'tuple', not %r" % (grouping,))
+        self._check(self.lib.sbg_enum_set_grouping(self._h, _GROUPINGS[grouping]))
+
 
 def inner_table(inner=None):
     """sbg_inner_table: a uint8 array of 6,561 entries, entry p3(seen) + p3(ones) = 1 iff some
@@ -542,6 +553,30 @@ def inner_table(inner=None):
     if lib.sbg_inner_table(ptr, out.ctypes.data_as(C.POINTER(C.c_uint8))) != 0:
         raise NativeLibraryError("sbg_inner_table failed")
     return out
+
+
+# -- grouping: the distinct gate sets and wirings that realise a state ---------------------------
+_GROUPINGS = {None: native.SBG_GROUP_NONE, "shape": native.SBG_GROUP_SHAPE,
+              "tuple": native.SBG_GROUP_TUPLE}
+# the key bits below a group's id, per (grouping, width): positions (shape), then the ordering row
+_GROUP_SHIFT = {("shape", 5): 8, ("shape", 7): 16, ("tuple", 5): 12, ("tuple", 7): 23}
+
+
+def match_group(key, width, grouping):
+    """The id of the group an enumerated match's key belongs to under a grouping (see
+    LutEngine.set_grouping): the key itself for None and for width 3, else key >> 8 / key >> 16
+    (shape, 5- / 7-LUT) or key >> 12 / key >> 23 (tuple).  Matches of one group have equal ids;
+    groups come in ascending id order."""
+    if grouping not in _GROUPINGS:
+        raise ValueError("grouping must be None, 'shape' or 'tuple', not %r" % (grouping,))
+    if width not in (3, 5, 7):
+        raise ValueError("width must be 3, 5 or 7")
+    key = int(key)
+    if not 0 <= key < 2**64:
+        raise ValueError("key must lie in 0..2**64-1")
+    if grouping is None or width == 3:
+        return key
+    return key >> _GROUP_SHIFT[(grouping, width)]
 
 
 def _depth_args(depth, max_depth):
@@ -588,7 +623,9 @@ def shallowest_matches(engine, width, orders, depth, max_matches):
     (func_order,) or (outer, middle).  Returns (minimum depth or None, the number of matches at
     it, the first max_matches of them in key order).  The filter stays installed at the minimum
     depth, so the engine's cursor serves the shallowest set (fetch_matches, pick_matches).
-    `engine` is a LutEngine or a DistributedLutSearch."""
+    `engine` is a LutEngine or a DistributedLutSearch.  Use it with no grouping or with "shape"
+    grouping: under "tuple" grouping a gate set is binned at the depth of its first match, which
+    need not be its shallowest."""
     if width not in (3, 5, 7):
         raise ValueError("width must be 3, 5 or 7")
     run = getattr(engine, "enumerate%d" % width)

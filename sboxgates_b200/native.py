@@ -57,6 +57,9 @@ SBG_ENUM_MAX_MATCHES = 1 << 24
 SBG_MAX_GATES = 500
 SBG_MAX_DEPTH = 1020      # largest gate depth of a depth filter
 SBG_DEPTH_BINS = 1024     # bins of the depth histogram
+SBG_GROUP_NONE = 0        # enumeration groupings (sbg_enum_set_grouping): every match,
+SBG_GROUP_SHAPE = 1       #   one per (gates, ordering row),
+SBG_GROUP_TUPLE = 2       #   one per gate set
 
 SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7 = 1, 2, 4
 SBG_LANES = 8
@@ -115,6 +118,7 @@ SIGNATURES = {
     "sbg_enum_depth_counts": (C.c_int, [C.c_void_p, u64p, C.c_uint32]),
     "sbg_enum_set_functions": (C.c_int, [C.c_void_p, u64p, u64p, u64p]),
     "sbg_inner_table": (C.c_int, [u64p, C.POINTER(C.c_uint8)]),
+    "sbg_enum_set_grouping": (C.c_int, [C.c_void_p, C.c_int]),
 }
 
 _lib = None
