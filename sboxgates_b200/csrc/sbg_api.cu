@@ -170,19 +170,13 @@ struct sbg_lane {
 };
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
-// (widths 5 and 7) or the gate order (width 3), the depth filter if one was installed
-// (sbg_enum_set_depth; its histogram pointer is the lane's, set at launch), and the function
-// filter if one was installed (sbg_enum_set_functions; with it, depth holds the neutral filter
-// when `filtered` is false), and the grouping (sbg_enum_set_grouping; under a grouping of width 5
-// or 7 the grouped forms run, with the neutral depth and function filters for those not installed).
+// (widths 5 and 7) or the gate order (width 3), the kernel form (EnumForm) and, for the filtered and
+// grouped forms, the filter block (take_filter; its histogram pointer is the lane's, set at launch).
 struct EnumInputs {
   EnumOrders ord;
   EnumGateOrder gates;
-  bool filtered;
-  EnumDepth<true> depth;
-  bool fn_on;
-  EnumFunc fn;
-  int grouping;
+  int form;
+  EnumFilter filter;
 };
 
 // The depth filter of a handle (sbg_enum_set_depth): the depths of n gates and the bound.
@@ -193,10 +187,12 @@ struct DepthFilter {
   uint16_t depth[SBG_MAX_GATES] = {};
 };
 
-// The function filter of a handle (sbg_enum_set_functions), ready for the kernels.
+// The function filter of a handle (sbg_enum_set_functions): the sets and inner_all of EnumFilter,
+// ready for the kernels.
 struct FunctionFilter {
   bool on = false;
-  EnumFunc fn = {};
+  uint32_t sets[16 + kInnerWords] = {};
+  int inner_all = 0;
 };
 
 // The enumeration cursor: what sbg_enum_fetch / sbg_enum_pick need of the last counted enumeration
@@ -382,6 +378,17 @@ auto with_nw(int nw, F &&f) {
     case 4: return f(std::integral_constant<int, 4>());
     default: return f(std::integral_constant<int, 8>());
   }
+}
+
+// f(form_c) with the enumeration kernel form (EnumForm) as the compile-time constant
+// decltype(form_c)::value.  Width 3 has no grouped form (take_filter never picks it there).
+template <int WIDTH, class F>
+auto with_form(int form, F &&f) {
+  if constexpr (WIDTH != 3) {
+    if (form == kFormGrouped) return f(std::integral_constant<int, kFormGrouped>());
+  }
+  if (form == kFormFiltered) return f(std::integral_constant<int, kFormFiltered>());
+  return f(std::integral_constant<int, kFormPlain>());
 }
 
 // Prefixes per ticket batch.  One batch costs one global atomic; batches should hold enough pairs
@@ -1448,10 +1455,10 @@ static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
     && offsetof(sbg_match, func_outer) == offsetof(DevMatch, func_outer)
     && offsetof(sbg_match, inner_seen) == offsetof(DevMatch, inner_seen)
     && offsetof(sbg_match, width) == offsetof(DevMatch, width), "sbg_match and DevMatch agree");
-// The largest enumeration form, k_enum3_fn: the gate order, the depth filter and the function
-// filter, plus at most 128 bytes of pointers and scalars, within the 4 KB kernel-parameter limit.
-static_assert(sizeof(EnumGateOrder) + sizeof(EnumDepth<true>) + sizeof(EnumFunc) + 128 <= 4096,
-    "k_enum3_fn's parameters fit in 4 KB");
+// The largest enumeration form, the filtered k_enum3: the gate order and the filter block, plus at
+// most 128 bytes of pointers and scalars, within the 4 KB kernel-parameter limit.
+static_assert(sizeof(EnumGateOrder) + sizeof(EnumFilter) + 128 <= 4096,
+    "the filtered k_enum3's parameters fit in 4 KB");
 
 // Count-free windows start at this many tickets and double: a first-match search then costs a few
 // windows of work past the first match, a search without one about twice the counting sweep's
@@ -1502,53 +1509,25 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
       if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "enumeration launch: %s", cudaGetErrorString(e));
       return SBG_OK;
     };
-    // the unfiltered or the filtered form (DF) of the width's kernel
-    auto run_form = [&](auto df_c, const EnumDepth<decltype(df_c)::value> &dep) {
-      constexpr bool DF = decltype(df_c)::value;
+    return with_form<WIDTH>(in.form, [&](auto form_c) {
+      constexpr int FORM = decltype(form_c)::value;
+      EnumFilterOf<FORM> flt = {};
+      if constexpr (FORM != kFormPlain) {
+        flt = in.filter;
+        flt.hist = L.d_ehist;
+      }
       if constexpr (WIDTH == 3) {
-        return run(k_enum3<NW, MODE, DF>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates, L.d_ecount,
-            L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, dep);
+        return run(k_enum3<NW, MODE, FORM>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates,
+            L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, flt);
       } else if constexpr (WIDTH == 5) {
-        return run(k_enum5<NW, MODE, DF>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
-            L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, dep);
+        return run(k_enum5<NW, MODE, FORM>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
+            L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, flt);
       } else {
-        return run(k_enum7<NW, MODE, DF>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
+        return run(k_enum7<NW, MODE, FORM>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
             L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts,
-            h->d_tab, dep);
+            h->d_tab, flt);
       }
-    };
-    if constexpr (WIDTH != 3) {
-      if (in.grouping != SBG_GROUP_NONE) {
-        // the grouped form, with the installed filters or the neutral ones
-        EnumDepth<true> dep = in.depth;
-        dep.hist = L.d_ehist;
-        if constexpr (WIDTH == 5) {
-          return run(k_enum5_gr<NW, MODE>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
-              L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, dep, in.fn,
-              in.grouping);
-        } else {
-          return run(k_enum7_gr<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
-              L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts,
-              h->d_tab, dep, in.fn, in.grouping);
-        }
-      }
-    }
-    if (!in.filtered && !in.fn_on) return run_form(std::false_type(), EnumDepth<false>());
-    EnumDepth<true> dep = in.depth;
-    dep.hist = L.d_ehist;
-    if (!in.fn_on) return run_form(std::true_type(), dep);
-    // the function-filtered form, with the depth filter or the neutral one
-    if constexpr (WIDTH == 3) {
-      return run(k_enum3_fn<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates, L.d_ecount,
-          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, dep, in.fn);
-    } else if constexpr (WIDTH == 5) {
-      return run(k_enum5_fn<NW, MODE>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
-          L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, dep, in.fn);
-    } else {
-      return run(k_enum7_fn<NW, MODE>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
-          L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts,
-          h->d_tab, dep, in.fn);
-    }
+    });
   });
   if (rc != SBG_OK) return rc;
   if (MODE == kEnumCount) {
@@ -1600,7 +1579,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   if ((rc = grow(h, L, L.d_ecount, L.ecount_cap, room)) != SBG_OK) return rc;
   if ((rc = grow(h, L, L.d_eoffset, L.eoffset_cap, room)) != SBG_OK) return rc;
   SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
-  if (in.filtered || in.fn_on || (WIDTH != 3 && in.grouping != SBG_GROUP_NONE)) {
+  if (in.form != kFormPlain) {
     if ((rc = grow(h, L, L.d_ehist, L.ehist_cap, (uint64_t)kDepthBins)) != SBG_OK) return rc;
     SBG_CUDA(h, cudaMemsetAsync(L.d_ehist, 0, kDepthBins * sizeof(unsigned long long), L.stream));
   }
@@ -1649,9 +1628,9 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   }
   if (total != nullptr) *total = ec.carry;
   if (feasible != nullptr) {
-    // width 3: every feasible triple is a match (the function-filtered form counts them apart)
+    // width 3: every feasible triple is a match (the filtered form counts them apart)
     *feasible = WIDTH == 7 ? (uint64_t)L.list_count
-        : WIDTH == 3 && !in.fn_on ? ec.total : ec.feasible;
+        : WIDTH == 3 && in.form == kFormPlain ? ec.total : ec.feasible;
   }
   return SBG_OK;
 }
@@ -1673,10 +1652,10 @@ int check_enum_args(sbg_handle *h, int part, int nparts, uint64_t max_matches, s
 }
 
 // A function filter's sets (host memory, 4 words each; NULL = all 256 functions) as the kernels read
-// them (EnumFunc); all three NULL gives the filter that keeps every match.
+// them (EnumFilter::sets and inner_all); all three NULL gives the filter that keeps every match.
 void make_functions(const uint64_t *outer, const uint64_t *middle, const uint64_t *inner,
-    EnumFunc &fn) {
-  memset(&fn, 0, sizeof(fn));
+    FunctionFilter &fn) {
+  memset(fn.sets, 0, sizeof(fn.sets));
   const uint64_t *sets[2] = {outer, middle};
   for (int r = 0; r < 2; r++) {
     for (int w = 0; w < 8; w++) {
@@ -1691,37 +1670,45 @@ void make_functions(const uint64_t *outer, const uint64_t *middle, const uint64_
       || (inner[0] & inner[1] & inner[2] & inner[3]) == ~0ull;
 }
 
-// The handle's depth and function filters, if any, and its grouping into the inputs of an sbg_enum*
-// call on the current problem.  The forms that carry both filters (function-filtered or grouped)
-// get the neutral ones in place of those not installed.
-int take_filter(sbg_handle *h, EnumInputs &in) {
+// The function filter that keeps every match, built once (the inner table takes 65,536 steps).
+const FunctionFilter &neutral_functions() {
+  static const FunctionFilter all = [] {
+    FunctionFilter f;
+    make_functions(nullptr, nullptr, nullptr, f);
+    return f;
+  }();
+  return all;
+}
+
+// The handle's depth and function filters and its grouping, for an sbg_enum* call of `width` on the
+// current problem, into the kernel form and its filter block.  Any setting picks the filtered form
+// (grouped at widths 5 and 7 under a grouping), with the neutral filter in place of one not
+// installed; none picks the plain form.
+int take_filter(sbg_handle *h, int width, EnumInputs &in) {
   const DepthFilter &f = h->filter;
-  in.filtered = f.on;
-  in.fn_on = h->functions.on;
-  in.grouping = h->grouping;
-  const bool both = in.fn_on || in.grouping != SBG_GROUP_NONE;
-  if (in.fn_on) {
-    in.fn = h->functions.fn;
-  } else if (both) {
-    make_functions(nullptr, nullptr, nullptr, in.fn);   // keeps every match
-  }
-  if (both) in.fn.depth_on = f.on;
-  if (!f.on) {
-    if (both) {
-      // the neutral depth filter: every gate at depth 0, a bound no match exceeds
-      memset(&in.depth, 0, sizeof(in.depth));
-      in.depth.max_depth = kDepthBins - 1;
+  const FunctionFilter &fn = h->functions;
+  const int grouping = width == 3 ? SBG_GROUP_NONE : h->grouping;   // the identity at width 3
+  in.form = grouping != SBG_GROUP_NONE ? kFormGrouped
+      : f.on || fn.on ? kFormFiltered : kFormPlain;
+  EnumFilter &flt = in.filter;
+  memset(&flt, 0, sizeof(flt));
+  if (in.form == kFormPlain) return SBG_OK;
+  if (f.on) {
+    const int n = cur(h).n;
+    if (f.n != n) {
+      return fail(h, SBG_ERR_ARG, "the depth filter holds %d gates, the problem has %d", f.n, n);
     }
-    return SBG_OK;
+    memcpy(flt.d, f.depth, sizeof(uint16_t) * (size_t)n);
+    // no match is deeper than kDepthBins - 2, so a larger bound filters nothing more
+    flt.max_depth = (int)std::min<uint32_t>(f.max_depth, kDepthBins - 1);
+  } else {
+    flt.max_depth = kDepthBins - 1;   // the neutral depth filter: every gate at depth 0
   }
-  const int n = cur(h).n;
-  if (f.n != n) {
-    return fail(h, SBG_ERR_ARG, "the depth filter holds %d gates, the problem has %d", f.n, n);
-  }
-  memset(&in.depth, 0, sizeof(in.depth));
-  memcpy(in.depth.d, f.depth, sizeof(uint16_t) * (size_t)n);
-  // no match is deeper than kDepthBins - 2, so a larger bound filters nothing more
-  in.depth.max_depth = (int)std::min<uint32_t>(f.max_depth, kDepthBins - 1);
+  flt.hist_on = f.on;
+  const FunctionFilter &use = fn.on ? fn : neutral_functions();
+  memcpy(flt.sets, use.sets, sizeof(flt.sets));
+  flt.inner_all = use.inner_all;
+  flt.grouping = grouping;
   return SBG_OK;
 }
 
@@ -2631,7 +2618,7 @@ int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, ui
   EnumInputs in5;
   memcpy(in5.ord.order[0], func_order, 256);
   memset(in5.ord.order[1], 0, 256);
-  if ((rc = take_filter(h, in5)) != SBG_OK) return rc;
+  if ((rc = take_filter(h, 5, in5)) != SBG_OK) return rc;
   return run_enum<5>(h, kBeginSearch5, in, in5, part, nparts, max_matches, out, n_out, total,
       feasible);
 }
@@ -2648,7 +2635,7 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
   EnumInputs in7;
   memcpy(in7.ord.order[0], outer_order, 256);
   memcpy(in7.ord.order[1], middle_order, 256);
-  if ((rc = take_filter(h, in7)) != SBG_OK) return rc;
+  if ((rc = take_filter(h, 7, in7)) != SBG_OK) return rc;
   // the installed list: only bring the problem block up to date
   return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
       total, feasible);
@@ -2672,7 +2659,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
   EnumInputs in3;
   memset(&in3, 0, sizeof(in3));
   memcpy(in3.gates.order, gate_order, sizeof(uint16_t) * (size_t)n);
-  if ((rc = take_filter(h, in3)) != SBG_OK) return rc;
+  if ((rc = take_filter(h, 3, in3)) != SBG_OK) return rc;
   // only bring the problem block up to date: the control words of an installed 7-LUT list stay
   return run_enum<3>(h, kBeginKeepCtl, CallInputs(), in3, part, nparts, max_matches, out, n_out,
       total, feasible);
@@ -2911,7 +2898,7 @@ int sbg_enum_depth_counts(sbg_handle *h, uint64_t *out, uint32_t nbins) {
   if (out == nullptr && nbins > 0) return fail(h, SBG_ERR_ARG, "null output");
   int rc;
   if ((rc = check_cursor(h)) != SBG_OK) return rc;
-  if (!h->cursor.in.filtered) {
+  if (!h->cursor.in.filter.hist_on) {
     return fail(h, SBG_ERR_STATE, "the enumeration cursor was counted without a depth filter");
   }
   if (nbins == 0) return SBG_OK;
@@ -2948,7 +2935,7 @@ int sbg_enum_set_functions(sbg_handle *h, const uint64_t *outer, const uint64_t 
     f.on = false;
     return SBG_OK;
   }
-  make_functions(outer, middle, inner, f.fn);
+  make_functions(outer, middle, inner, f);
   f.on = true;
   return SBG_OK;
 }

@@ -2859,28 +2859,49 @@ __device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned
   store_match<WIDTH>(dst, key, G, fo, fm, ones, seen);
 }
 
+// ---- kernel forms --------------------------------------------------------------------------------
+// k_enum3/5/7 come in three forms (template parameter FORM):
+//   kFormPlain     every match: no filter, no grouping;
+//   kFormFiltered  the matches that pass the depth filter and the function filter below, both read
+//                  from one EnumFilter block.  For a filter not installed the host gives the
+//                  neutral one (every gate at depth 0 and the bound kDepthBins - 1, or all 256
+//                  functions in every set), which keeps every match and prunes nothing;
+//   kFormGrouped   the filtered form's matches, counted and emitted as groups (see "grouping"
+//                  below).  Widths 5 and 7 only: a 3-LUT group is one match.
+enum EnumForm : int { kFormPlain = 0, kFormFiltered = 1, kFormGrouped = 2 };
+
 // ---- depth filter (sbg_enum_set_depth) -----------------------------------------------------------
-// The filtered forms of k_enum3/5/7 (template flag DF) keep only the matches whose depth is at most
-// max_depth.  A match's depth is that of the output gate it would add, from the caller's gate
-// depths D: 1 + max(Da, Db, Dc) (width 3), 1 + max(1 + max(Da, Db, Dc), Dd, De) (width 5),
-// 1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df), Dg) (width 7), gates in reference order.  It
+// The filtered and grouped forms keep only the matches whose depth is at most max_depth.  A match's depth
+// is that of the output gate it would add, from the caller's gate depths D: 1 + max(Da, Db, Dc)
+// (width 3), 1 + max(1 + max(Da, Db, Dc), Dd, De) (width 5), 1 + max(1 + max(Da, Db, Dc),
+// 1 + max(Dd, De, Df), Dg) (width 7), gates in reference order.  It
 // depends on the ticket and the lane's third position (width 3) or the ordering row (widths 5 and
 // 7) only, so the count and emit passes apply the same test and a ticket emits what it counted.
 // Pruning: a gate with D >= max_depth occurs in no match, and the shallowest ordering of a 5-tuple
 // has depth max(2 + third deepest, 1 + deepest) (any 3 of the 5 may be the outer inputs), of a
 // 7-tuple max(2 + second deepest, 1 + deepest) (any of the 7 may be the last input); tickets and
-// (d,e) pairs none of whose orderings fit are dropped before their feasibility work.  The filtered
-// count pass fills a histogram of the matches by depth, per CTA in shared memory (one atomic per
-// (tuple, ordering), per (list entry, row, 32 outer functions), or per distinct depth of a 3-LUT
-// ballot), flushed to global memory once at the end.
+// (d,e) pairs none of whose orderings fit are dropped before their feasibility work.  When a depth
+// filter is installed (hist_on), the count pass fills a histogram of the matches by depth, per CTA
+// in shared memory (one atomic per (tuple, ordering), per (list entry, row, 32 outer functions), or
+// per distinct depth of a 3-LUT ballot), flushed to global memory once at the end.
 constexpr int kDepthBins = 1024;   // SBG_DEPTH_BINS: every depth (at most 1,022) has a bin
+constexpr int kInnerWords = (kMinpos3 + 31) / 32;
+constexpr int kGroupShape = 1, kGroupTuple = 2;   // SBG_GROUP_SHAPE, SBG_GROUP_TUPLE
 
-template <bool DF> struct EnumDepth {};   // the unfiltered forms take no filter
-template <> struct EnumDepth<true> {
-  uint16_t d[kMaxGatesPad];     // depth of each gate of the problem
-  int max_depth;                // the bound, at most kDepthBins - 1
-  unsigned long long *hist;     // count pass: matches per depth, kDepthBins bins
+// What the filtered and grouped forms read besides the problem: the depth filter, the function
+// filter (see "function filter" below) and the grouping kind.
+struct EnumFilter {
+  uint16_t d[kMaxGatesPad];          // depth of each gate of the problem
+  int max_depth;                     // the bound, at most kDepthBins - 1
+  int hist_on;                       // count pass: fill the depth histogram (a depth filter is set)
+  unsigned long long *hist;          //   matches per depth, kDepthBins bins
+  uint32_t sets[16 + kInnerWords];   // words 0-7: outer set, 8-15: middle set, then the inner table
+  int inner_all;                     // the inner set holds all 256 functions (the table is all ones)
+  int grouping;                      // grouped form: kGroupShape or kGroupTuple
 };
+struct EnumNoFilter {};   // the plain form takes no filter
+template <int FORM>
+using EnumFilterOf = std::conditional_t<FORM == kFormPlain, EnumNoFilter, EnumFilter>;
 
 __device__ __forceinline__ uint16_t *depth_smem() {
   __shared__ uint16_t s_depth[kMaxGatesPad];
@@ -2892,21 +2913,25 @@ __device__ __forceinline__ unsigned long long *hist_smem() {
   return s_hist;
 }
 
-// The gate depths to shared memory (and a zero histogram for the count pass); the kernel's
-// __syncthreads after its own staging covers these stores.
+__device__ __forceinline__ uint32_t *func_smem() {
+  __shared__ uint32_t s_func[16 + kInnerWords];
+  return s_func;
+}
+
+// The gate depths and the function sets to shared memory (and a zero histogram for the count
+// pass); the kernel's __syncthreads after its own staging covers these stores.
 template <int MODE>
-__device__ __forceinline__ const uint16_t *stage_depth(const EnumDepth<true> &dep, int n) {
-  uint16_t *s = depth_smem();
-  for (int i = threadIdx.x; i < n; i += blockDim.x) s[i] = dep.d[i];
+__device__ __forceinline__ void stage_filter(const EnumFilter &flt, int n, const uint16_t *&s_dep,
+    const uint32_t *&s_fn) {
+  uint16_t *sd = depth_smem();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) sd[i] = flt.d[i];
   if (MODE == kEnumCount) {
     for (int i = threadIdx.x; i < kDepthBins; i += blockDim.x) hist_smem()[i] = 0;
   }
-  return s;
-}
-
-template <bool DF>
-__device__ __forceinline__ int depth_bound(const EnumDepth<DF> &dep) {
-  if constexpr (DF) return dep.max_depth; else return 0;
+  uint32_t *sf = func_smem();
+  for (int i = threadIdx.x; i < 16 + kInnerWords; i += blockDim.x) sf[i] = flt.sets[i];
+  s_dep = sd;
+  s_fn = sf;
 }
 
 // c more matches of depth d in the CTA's histogram.
@@ -2914,14 +2939,14 @@ __device__ __forceinline__ void hist_add(int d, unsigned long long c) {
   atomicAdd(hist_smem() + d, c);
 }
 
-// The end of a filtered count pass: the CTA's histogram into dep.hist.
-template <int MODE, bool DF>
-__device__ __forceinline__ void flush_hist(const EnumDepth<DF> &dep) {
-  if constexpr (DF && MODE == kEnumCount) {
+// The end of a count pass of the filtered or grouped form: the CTA's histogram into flt.hist.
+template <int MODE, int FORM>
+__device__ __forceinline__ void flush_hist(const EnumFilterOf<FORM> &flt) {
+  if constexpr (FORM != kFormPlain && MODE == kEnumCount) {
     __syncthreads();
     const unsigned long long *s = hist_smem();
     for (int i = threadIdx.x; i < kDepthBins; i += blockDim.x) {
-      if (s[i] != 0) atomicAdd(dep.hist + i, s[i]);
+      if (s[i] != 0) atomicAdd(flt.hist + i, s[i]);
     }
   }
 }
@@ -2949,32 +2974,12 @@ __device__ __forceinline__ int depth7(const int *d7, int k) {
 }
 
 // ---- function filter (sbg_enum_set_functions) --------------------------------------------------
-// The function-filtered forms (k_enum3_fn / k_enum5_fn / k_enum7_fn) keep only the matches whose
-// outer LUT lies in the outer set, whose middle LUT lies in the middle set, and whose inner LUT can
-// be completed inside the inner set: some f in it has (f & inner_seen) == func_inner.  The last
-// test is a lookup in the inner table, indexed by minpos3's code(seen, ones) = p3(seen) + p3(ones).
-// The sets are indexed by function value, as the survivor words of k_enum5 / k_enum7 and
-// cube_union's set over fm are, so the outer and middle tests are ANDs with 8 words.  These forms
-// also take the depth filter: without one the host gives every gate depth 0 and the bound
-// kDepthBins - 1, which keeps every match and prunes nothing, and depth_on = 0 skips the histogram.
-constexpr int kInnerWords = (kMinpos3 + 31) / 32;
-struct EnumFunc {
-  uint32_t sets[16 + kInnerWords];   // words 0-7: outer set, 8-15: middle set, then the inner table
-  int inner_all;                     // the inner set holds all 256 functions (the table is all ones)
-  int depth_on;                      // a depth filter is installed: fill its histogram
-};
-
-__device__ __forceinline__ uint32_t *func_smem() {
-  __shared__ uint32_t s_func[16 + kInnerWords];
-  return s_func;
-}
-
-// The sets to shared memory; the kernel's __syncthreads after its own staging covers these stores.
-__device__ __forceinline__ const uint32_t *stage_func(const EnumFunc &fn) {
-  uint32_t *s = func_smem();
-  for (int i = threadIdx.x; i < 16 + kInnerWords; i += blockDim.x) s[i] = fn.sets[i];
-  return s;
-}
+// The filtered and grouped forms keep only the matches whose outer LUT lies in the outer set, whose
+// middle LUT lies in the middle set, and whose inner LUT can be completed inside the inner set:
+// some f in it has (f & inner_seen) == func_inner.  The last test is a lookup in the inner table,
+// indexed by minpos3's code(seen, ones) = p3(seen) + p3(ones).  The sets are indexed by function
+// value, as the survivor words of k_enum5 / k_enum7 and cube_union's set over fm are, so the outer
+// and middle tests are ANDs with 8 words.
 
 __device__ __forceinline__ bool in_set(const uint32_t *set, uint32_t f) {
   return (set[f >> 5] >> (f & 31u)) & 1u;
@@ -3021,33 +3026,29 @@ __device__ __forceinline__ bool inner_ok7(const uint32_t *s_fn, const uint32_t *
 }
 
 // ---- grouping (sbg_enum_set_grouping) ------------------------------------------------------------
-// The grouped forms (k_enum5_gr / k_enum7_gr) enumerate groups of matches instead of matches: the
-// matches sharing a key prefix, the gates and ordering row (kGroupShape: 5-LUT key >> 8, 7-LUT
-// key >> 16) or the gate set (kGroupTuple: key >> 12, key >> 23).  A group counts once if it holds
-// a match, and emits its first match (smallest key), the record the ungrouped forms emit for that
+// The grouped form enumerates groups of matches instead of matches: the matches sharing a key
+// prefix, the gates and ordering row (kGroupShape: 5-LUT key >> 8, 7-LUT key >> 16) or the gate
+// set (kGroupTuple: key >> 12, key >> 23).  A group counts once if it holds a match that passes the
+// filters, and emits its first match (smallest key), the record the ungrouped forms emit for that
 // key.  A key prefix names a 3-gate prefix ticket's tuple (5-LUT) or a list entry (7-LUT), so no
 // group crosses a ticket, and the count and emit passes stop at the same first match of a group.
-// The grouped forms carry the depth and function filters (neutral when none is installed); the
-// kind is a warp-uniform runtime argument.
-constexpr int kGroupShape = 1, kGroupTuple = 2;   // SBG_GROUP_SHAPE, SBG_GROUP_TUPLE
+// The kind, EnumFilter::grouping, is warp-uniform.
 
 // The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
 // 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
-// feasible tuple and ordering the set of working outer functions from outer_ok5.  DF: the depth
-// filter (see depth5); `feasible` then counts the feasible tuples with an ordering within the bound.
-// FF: the function filter (see EnumFunc), applied to the survivor words of each ordering, so the
-// emit loop sees only the outer functions the count pass counted.  GR: grouped (see "grouping"
-// above k_enum5_gr); a (tuple, ordering) counts once if its survivor set is not empty and emits its
-// lowest position, and under kGroupTuple the tuple ends there.
-template <int NW, int MODE, bool DF, bool FF, bool GR = false>
+// feasible tuple and ordering the set of working outer functions from outer_ok5.  Filtered and
+// grouped forms: the depth filter (see depth5), and `feasible` then counts the feasible tuples with
+// an ordering within the bound; the function filter, applied to the survivor words of each
+// ordering, so the emit loop sees only the outer functions the count pass counted.  Grouped form:
+// a (tuple, ordering) counts once if its survivor set is not empty and emits its lowest position,
+// and under kGroupTuple the tuple ends there.
+template <int NW, int MODE, int FORM>
 __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders &ord, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn,
-    int grouping = 0) {
-  static_assert(DF || !FF, "the function-filtered form carries the depth filter");
-  static_assert(FF || !GR, "the grouped form carries both filters");
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> &flt) {
+  constexpr bool FILTER = FORM != kFormPlain, GR = FORM == kFormGrouped;
   constexpr int P = 3, K = 5, NC = 1 << P;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[256];
@@ -3060,13 +3061,13 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
   stage_tables(s_tabs, prob, NW, npad);
   for (int i = threadIdx.x; i < 256; i += blockDim.x) s_ord[i] = ord.order[0][i];
   const uint16_t *s_dep = nullptr;
-  if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
-  const int B = depth_bound(dep);
   const uint32_t *s_fn = nullptr;
+  int B = 0;
   bool inner_all = true;
-  if constexpr (FF) {
-    s_fn = stage_func(*fn);
-    inner_all = fn->inner_all != 0;
+  if constexpr (FILTER) {
+    stage_filter<MODE>(flt, n, s_dep, s_fn);
+    B = flt.max_depth;
+    inner_all = flt.inner_all != 0;
   }
   __syncthreads();
   uint32_t T[NW], M[NW];
@@ -3088,8 +3089,8 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
       bool rejected = false;
 #pragma unroll
       for (int i = 0; i < P; i++) rejected |= (pre[i] < 8) && ((inmask >> pre[i]) & 1u);
-      int pre_deep = 0;   // DF: prefix gates of depth B - 1 (at most two gates of a match may have it)
-      if constexpr (DF) {
+      int pre_deep = 0;   // prefix gates of depth B - 1 (at most two gates of a match may have it)
+      if constexpr (FILTER) {
 #pragma unroll
         for (int i = 0; i < P; i++) {
           rejected |= s_dep[pre[i]] >= B;
@@ -3132,7 +3133,7 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
         if (alive) unrank_pair(q, r, pi, pj);
         const int gf = last + 1 + pi, gg = last + 1 + pj;
         if ((gf < 8 && ((inmask >> gf) & 1u)) || (gg < 8 && ((inmask >> gg) & 1u))) alive = false;
-        if constexpr (DF) {
+        if constexpr (FILTER) {
           if (alive) {
             const int df = s_dep[gf], dg = s_dep[gg];
             alive = df < B && dg < B && pre_deep + (df >= B - 1) + (dg >= B - 1) <= 2;
@@ -3160,25 +3161,25 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
           uint32_t H1, H0;
           summary5<NW>(s_tabs, npad, g5, T, M, lane, H1, H0);
           int d5[5];
-          if constexpr (DF) {
+          if constexpr (FILTER) {
 #pragma unroll
             for (int i = 0; i < 5; i++) d5[i] = s_dep[g5[i]];
           }
           for (int k = 0; k < 10 && !done; k++) {
             int kd = 0;
-            if constexpr (DF) {
+            if constexpr (FILTER) {
               kd = depth5(d5, k);
               if (kd > B) continue;
             }
             uint32_t ok[8], surv_mine = 0;
             uint32_t rr[8];
-            if constexpr (FF) outer_ok5_rr(H1, H0, k, lane, tab, ok, rr);
+            if constexpr (FILTER) outer_ok5_rr(H1, H0, k, lane, tab, ok, rr);
             else outer_ok5(H1, H0, k, lane, tab, ok);
             uint32_t c = 0;
 #pragma unroll
             for (int hi = 0; hi < 8; hi++) {
               uint32_t surv = ok[hi] & __brev(ok[7 - hi]);
-              if constexpr (FF) {
+              if constexpr (FILTER) {
                 surv &= s_fn[hi];
                 if (!inner_all) {
                   const uint32_t rr0 = __shfl_sync(kFull, rr[7 - hi], 31 - lane);
@@ -3193,17 +3194,15 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
               if (MODE == kEnumCount) {
                 if (c == 0) continue;
                 tk.count++;
-                if (fn->depth_on && lane == 0) hist_add(kd, 1);
-                if (grouping == kGroupTuple) break;
+                if (flt.hist_on && lane == 0) hist_add(kd, 1);
+                if (flt.grouping == kGroupTuple) break;
                 continue;
               }
             }
             if (MODE == kEnumCount) {
               tk.count += c;
-              if constexpr (FF) {
-                if (fn->depth_on && lane == 0 && c != 0) hist_add(kd, c);
-              } else {
-                if (DF && lane == 0 && c != 0) hist_add(kd, c);
+              if constexpr (FILTER) {
+                if (flt.hist_on && lane == 0 && c != 0) hist_add(kd, c);
               }
               continue;
             }
@@ -3230,45 +3229,24 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
               });
             }
             if constexpr (GR) {
-              if (grouping == kGroupTuple) break;
+              if (flt.grouping == kGroupTuple) break;
             }
           }
         }
       }
     }
   });
-  flush_hist<MODE>(dep);
+  flush_hist<MODE, FORM>(flt);
 }
 
-template <int NW, int MODE, bool DF>
+template <int NW, int MODE, int FORM>
 __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
-  enum5_body<NW, MODE, DF, false>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
-      part, nparts, tab, dep, nullptr);
-}
-
-template <int NW, int MODE>
-__global__ void __launch_bounds__(kThreads) k_enum5_fn(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
-    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
-    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn) {
-  enum5_body<NW, MODE, true, true>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
-      part, nparts, tab, dep, &fn);
-}
-
-template <int NW, int MODE>
-__global__ void __launch_bounds__(kThreads) k_enum5_gr(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
-    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
-    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn,
-    int grouping) {
-  enum5_body<NW, MODE, true, true, true>(prob, ectl, ord, counts, offsets, out, max_out, t_begin,
-      t_end, part, nparts, tab, dep, &fn, grouping);
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
+  enum5_body<NW, MODE, FORM>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
+      part, nparts, tab, flt);
 }
 
 // Middle functions of one cube set (see middle_cubes) as a 256-bit set over fm, word wd = fm >> 5.
@@ -3299,26 +3277,24 @@ __device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (
 // nparts + part), one warp per entry: the summary and stage-1 filter of k_decomp7 on the TRUE gate
 // tables (no stale outer cache), then per surviving outer function and ordering row the union of
 // the middle-function cubes.  Count: one lane per outer function; emit: positions in ascending
-// order, outer position in the loop, middle position across the lanes.  DF: the depth filter (see
-// depth7); an entry without an ordering within the bound is skipped, and so is every row above it.
-// FF: the function filter (see EnumFunc).  The outer set cuts the survivors, the middle set the
-// cube union.  A restricted inner set depends on the whole of fm, not only on its cube, so the
-// count pass then runs the emit loop (positions over the lanes) in place of the popcounts, and
-// both passes apply inner_ok7 to each lane's (fo, fm).  GR: grouped (see "grouping" above
-// enum5_body).  The count pass takes a row once when some surviving outer function leaves a
+// order, outer position in the loop, middle position across the lanes.  Filtered and grouped
+// forms: the depth filter (see depth7); an entry without an ordering within the bound is skipped,
+// and so is every row above it.  The function filter: the outer set cuts the survivors, the middle
+// set the cube union.  A restricted inner set depends on the whole of fm, not only on its cube, so
+// the count pass then runs the emit loop (positions over the lanes) in place of the popcounts, and
+// both passes apply inner_ok7 to each lane's (fo, fm).  Grouped form (see "grouping" above
+// enum5_body): the count pass takes a row once when some surviving outer function leaves a
 // non-empty cube union (rows outer, outer functions inner, stopping at the first); the emit loop
 // emits a row's first hit (first po, lowest pm) and moves to the next row.  Under kGroupTuple both
 // end the entry at its first row with a match.
-template <int NW, int MODE, bool DF, bool FF, bool GR = false>
+template <int NW, int MODE, int FORM>
 __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders &ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> &dep, const EnumFunc *fn,
-    int grouping = 0) {
-  static_assert(DF || !FF, "the function-filtered form carries the depth filter");
-  static_assert(FF || !GR, "the grouped form carries both filters");
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> &flt) {
+  constexpr bool FILTER = FORM != kFormPlain, GR = FORM == kFormGrouped;
   constexpr bool EMIT = MODE != kEnumCount;
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
@@ -3334,13 +3310,13 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
   for (int i = threadIdx.x; i < 25 * 32; i += blockDim.x) s_src7[i] = tab->src7[i >> 5][i & 31];
   for (int i = threadIdx.x; i < 512; i += blockDim.x) s_ord[i >> 8][i & 255] = ord.order[i >> 8][i & 255];
   const uint16_t *s_dep = nullptr;
-  if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
-  const int B = depth_bound(dep);
   const uint32_t *s_fn = nullptr;
-  bool slow = false;   // FF with a restricted inner set: the count pass runs the emit loop
-  if constexpr (FF) {
-    s_fn = stage_func(*fn);
-    slow = fn->inner_all == 0;
+  int B = 0;
+  bool slow = false;   // a restricted inner set: the count pass runs the emit loop
+  if constexpr (FILTER) {
+    stage_filter<MODE>(flt, n, s_dep, s_fn);
+    B = flt.max_depth;
+    slow = flt.inner_all == 0;
   }
   __syncthreads();
   uint32_t T[NW], M[NW];
@@ -3361,7 +3337,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
 #pragma unroll
       for (int i = 0; i < 7; i++) g[i] = (int)((cur >> (9 * (6 - i))) & 0x1ffu);
       int d7[7];
-      if constexpr (DF) {
+      if constexpr (FILTER) {
         // no gate of depth >= B, and at most one of depth B - 1 (it must be the last input)
         int deep = 0;
         bool over = false;
@@ -3378,7 +3354,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
       bool done = false;
       for (int j = 0; j < 25 && !done; j++) {
         if (((pass_j >> j) & 1u) == 0) continue;
-        if constexpr (DF) {
+        if constexpr (FILTER) {
           bool fits = false;
           for (int row = 0; row < c_j_rows[j]; row++) fits |= depth7(d7, c_j_first_k[j] + row) <= B;
           if (!fits) continue;
@@ -3389,7 +3365,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
 #pragma unroll
         for (int hi = 0; hi < 8; hi++) {
           uint32_t sv = ok[hi] & __brev(ok[7 - hi]);
-          if constexpr (FF) sv &= s_fn[hi];
+          if constexpr (FILTER) sv &= s_fn[hi];
           any |= sv;
           if (lane == hi) surv_mine = sv;
         }
@@ -3430,8 +3406,8 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
               }
               if (!found) continue;
               tk.count++;
-              if (fn->depth_on && lane == 0) hist_add(rd, 1);
-              if (grouping == kGroupTuple) {
+              if (flt.hist_on && lane == 0) hist_add(rd, 1);
+              if (flt.grouping == kGroupTuple) {
                 done = true;   // the entry is the group
                 break;
               }
@@ -3450,7 +3426,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
 #pragma unroll 1
             for (int row = 0; row < nrows; row++) {
               int rd = 0;
-              if constexpr (DF) {
+              if constexpr (FILTER) {
                 rd = depth7(d7, k0 + row);
                 if (rd > B) continue;
               }
@@ -3459,21 +3435,18 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
               bool hok[2][4];
               middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
               cube_union(hv, hok, S, ov, bits);
-              if constexpr (FF) {
+              if constexpr (FILTER) {
 #pragma unroll
                 for (int wd = 0; wd < 8; wd++) bits[wd] &= s_fn[8 + wd];
               }
 #pragma unroll
               for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd]);
-              if constexpr (FF) {
-                if (fn->depth_on) {
+              if constexpr (FILTER) {
+                if (flt.hist_on) {
+                  // rows differ in depth: each row's matches go to its own bin
                   const uint32_t s = __reduce_add_sync(kFull, have ? c - c_before : 0u);
                   if (lane == 0 && s != 0) hist_add(rd, s);
                 }
-              } else if constexpr (DF) {
-                // rows differ in depth: each row's matches go to its own bin
-                const uint32_t s = __reduce_add_sync(kFull, have ? c - c_before : 0u);
-                if (lane == 0 && s != 0) hist_add(rd, s);
               }
             }
             tk.count += __reduce_add_sync(kFull, have ? c : 0u);
@@ -3482,9 +3455,9 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
 #pragma unroll 1
         for (int row = 0; (EMIT || slow) && row < nrows && !done; row++) {
           const int k = k0 + row;
-          if (DF && depth7(d7, k) > B) continue;
+          if (FILTER && depth7(d7, k) > B) continue;
           [[maybe_unused]] const uint32_t row_start = tk.count;
-          [[maybe_unused]] bool row_hit = false;   // GR: the row's group is emitted
+          [[maybe_unused]] bool row_hit = false;   // grouped: the row's group is emitted
 #pragma unroll 1
           for (int po = 0; po < 256 && !done; po++) {
             const uint32_t fo = s_ord[0][po];
@@ -3498,7 +3471,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
             bool hok[2][4];
             middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
             [[maybe_unused]] uint32_t AB[4] = {0, 0, 0, 0};
-            if (FF && slow) inner_cells7(r1, r0, c_row_b[k], AB);
+            if (FILTER && slow) inner_cells7(r1, r0, c_row_b[k], AB);
             const unsigned long long key_hi = (idx << 23) | ((uint64_t)k << 16) | ((uint64_t)po << 8);
 #pragma unroll 1
             for (int w = 0; w < 8; w++) {
@@ -3513,7 +3486,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
                       && (fm & S) == (hv[0][c0] | hv[1][c1]);
                 }
               }
-              if constexpr (FF) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
+              if constexpr (FILTER) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
               if constexpr (GR) {
                 // the group's record: the first hit of the row
                 const uint32_t bal = __ballot_sync(kFull, hit);
@@ -3528,54 +3501,31 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
             }
             if (GR && row_hit) break;
           }
-          if constexpr (FF && MODE == kEnumCount) {
+          if constexpr (FILTER && MODE == kEnumCount) {
             // the slow count pass: this row's matches to its depth's bin
-            if (fn->depth_on && lane == 0 && tk.count != row_start) {
+            if (flt.hist_on && lane == 0 && tk.count != row_start) {
               hist_add(depth7(d7, k), tk.count - row_start);
             }
           }
           if constexpr (GR) {
-            if (row_hit && grouping == kGroupTuple) done = true;   // the entry is the group
+            if (row_hit && flt.grouping == kGroupTuple) done = true;   // the entry is the group
           }
         }
       }
     }
   });
-  flush_hist<MODE>(dep);
+  flush_hist<MODE, FORM>(flt);
 }
 
-template <int NW, int MODE, bool DF>
+template <int NW, int MODE, int FORM>
 __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<DF> dep) {
-  enum7_body<NW, MODE, DF, false>(prob, ectl, ord, list, list_count, counts, offsets, out, max_out,
-      t_begin, t_end, part, nparts, tab, dep, nullptr);
-}
-
-template <int NW, int MODE>
-__global__ void __launch_bounds__(kThreads) k_enum7_fn(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
-    unsigned int list_count, uint32_t *__restrict__ counts,
-    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
-    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn) {
-  enum7_body<NW, MODE, true, true>(prob, ectl, ord, list, list_count, counts, offsets, out, max_out,
-      t_begin, t_end, part, nparts, tab, dep, &fn);
-}
-
-template <int NW, int MODE>
-__global__ void __launch_bounds__(kThreads) k_enum7_gr(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
-    unsigned int list_count, uint32_t *__restrict__ counts,
-    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
-    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const DevTables *__restrict__ tab, const EnumDepth<true> dep, const EnumFunc fn,
-    int grouping) {
-  enum7_body<NW, MODE, true, true, true>(prob, ectl, ord, list, list_count, counts, offsets, out,
-      max_out, t_begin, t_end, part, nparts, tab, dep, &fn, grouping);
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
+  enum7_body<NW, MODE, FORM>(prob, ectl, ord, list, list_count, counts, offsets, out, max_out,
+      t_begin, t_end, part, nparts, tab, flt);
 }
 
 
@@ -3591,17 +3541,16 @@ struct EnumGateOrder {
 // of the target (scan3_blocks' test, here on the compressed tables).  Key i << 18 | k << 9 | m, so a
 // ticket's matches are consecutive keys in the order of its lanes.  A match's record: the gates in
 // position order, func_inner = cells holding a masked 1, inner_seen = cells holding a masked
-// position (sbg_solve_inner's closed form).  DF: the depth filter; a pair with a gate of depth
-// >= max_depth is skipped.  FF: the function filter; the lane's (seen, ones) must complete inside
-// the inner set.  `feasible` then counts the triples within the depth bound, whatever their
-// function (the matches of the unfiltered or depth-filtered count).
-template <int NW, int MODE, bool DF, bool FF>
+// position (sbg_solve_inner's closed form).  Filtered form: the depth filter, where a pair with a
+// gate of depth >= max_depth is skipped, and the function filter, where the lane's (seen, ones)
+// must complete inside the inner set.  `feasible` then counts the triples within the depth bound, whatever their function.
+template <int NW, int MODE, int FORM>
 __device__ __forceinline__ void enum3_body(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumGateOrder &go, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const EnumDepth<DF> &dep, const EnumFunc *fn) {
-  static_assert(DF || !FF, "the function-filtered form carries the depth filter");
+    int nparts, const EnumFilterOf<FORM> &flt) {
+  constexpr bool FILTER = FORM != kFormPlain;
   extern __shared__ uint32_t smem[];
   __shared__ uint16_t s_order[kMaxGatesPad];
   const int lane = threadIdx.x & 31;
@@ -3611,10 +3560,12 @@ __device__ __forceinline__ void enum3_body(const DevProblem *__restrict__ prob,
   stage_tables(s_tabs, prob, NW, npad);
   for (int i = threadIdx.x; i < n; i += blockDim.x) s_order[i] = go.order[i];
   const uint16_t *s_dep = nullptr;
-  if constexpr (DF) s_dep = stage_depth<MODE>(dep, n);
-  const int B = depth_bound(dep);
   const uint32_t *s_fn = nullptr;
-  if constexpr (FF) s_fn = stage_func(*fn);
+  int B = 0;
+  if constexpr (FILTER) {
+    stage_filter<MODE>(flt, n, s_dep, s_fn);
+    B = flt.max_depth;
+  }
   __syncthreads();
   uint32_t T[NW], Z[NW];   // masked positions with target 1 / with target 0
 #pragma unroll
@@ -3630,8 +3581,8 @@ __device__ __forceinline__ void enum3_body(const DevProblem *__restrict__ prob,
     if (dealt < pairs) {
       int pi, pk;
       unrank_pair((uint32_t)dealt, n, pi, pk);
-      int dab = 0;   // DF: the deeper of the pair's gates; a match's depth is 1 + max(dab, Dc)
-      if constexpr (DF) {
+      int dab = 0;   // the deeper of the pair's gates; a match's depth is 1 + max(dab, Dc)
+      if constexpr (FILTER) {
         dab = max((int)s_dep[s_order[pi]], (int)s_dep[s_order[pk]]);
         if (dab >= B) return;
       }
@@ -3662,14 +3613,12 @@ __device__ __forceinline__ void enum3_body(const DevProblem *__restrict__ prob,
           if (one[c] != 0) ones |= 1u << c;
           if ((one[c] | zero[c]) != 0) seen |= 1u << c;
         }
-        if constexpr (DF) {
+        if constexpr (FILTER) {
           const int dm = 1 + max(dab, (int)s_dep[s_order[pm < n ? pm : pk]]);
           ok &= dm <= B;
-          if constexpr (FF) {
-            if (MODE == kEnumCount) feasible += __popc(__ballot_sync(kFull, ok));
-            ok = ok && inner_ok(s_fn, seen, ones);
-          }
-          if (MODE == kEnumCount && (!FF || fn->depth_on)) {
+          if (MODE == kEnumCount) feasible += __popc(__ballot_sync(kFull, ok));
+          ok = ok && inner_ok(s_fn, seen, ones);
+          if (MODE == kEnumCount && flt.hist_on) {
             // one histogram atomic per distinct depth of the ballot, by its lowest lane
             const uint32_t peers = __match_any_sync(kFull, ok ? dm : -1);
             if (ok && (peers & lanemask_lt()) == 0) hist_add(dm, __popc(peers));
@@ -3683,27 +3632,17 @@ __device__ __forceinline__ void enum3_body(const DevProblem *__restrict__ prob,
       }
     }
   });
-  flush_hist<MODE>(dep);
+  flush_hist<MODE, FORM>(flt);
 }
 
-template <int NW, int MODE, bool DF>
+template <int NW, int MODE, int FORM>
 __global__ void __launch_bounds__(kThreads) k_enum3(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const EnumDepth<DF> dep) {
-  enum3_body<NW, MODE, DF, false>(prob, ectl, go, counts, offsets, out, max_out, t_begin, t_end,
-      part, nparts, dep, nullptr);
-}
-
-template <int NW, int MODE>
-__global__ void __launch_bounds__(kThreads) k_enum3_fn(const DevProblem *__restrict__ prob,
-    EnumCtl *__restrict__ ectl, const EnumGateOrder go, uint32_t *__restrict__ counts,
-    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
-    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
-    int nparts, const EnumDepth<true> dep, const EnumFunc fn) {
-  enum3_body<NW, MODE, true, true>(prob, ectl, go, counts, offsets, out, max_out, t_begin, t_end,
-      part, nparts, dep, &fn);
+    int nparts, const EnumFilterOf<FORM> flt) {
+  enum3_body<NW, MODE, FORM>(prob, ectl, go, counts, offsets, out, max_out, t_begin, t_end,
+      part, nparts, flt);
 }
 
 
