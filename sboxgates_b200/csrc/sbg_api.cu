@@ -106,29 +106,42 @@ constexpr uint64_t kTicketTableMax = (uint64_t)1 << 24;    // tickets per launch
 constexpr uint64_t kTicketSlack = 16384;                   // tickets fetched past the end (one per warp)
 }  // namespace
 
+// A device array the handle owns: cap elements at p (none until the first grow), freed with its
+// owner.  The handle's device is current whenever an owner is destroyed (sbg_destroy); a handle
+// that never bound a device holds no array, so destroying it makes no CUDA call.
+template <class T>
+struct DevArray {
+  T *p = nullptr;
+  uint64_t cap = 0;
+  DevArray() = default;
+  DevArray(const DevArray &) = delete;
+  DevArray &operator=(const DevArray &) = delete;
+  ~DevArray() {
+    if (p != nullptr) cudaFree(p);
+  }
+  int grow(sbg_handle *h, cudaStream_t stream, uint64_t need);
+};
+
 // One lane = one CUDA stream with its own control words, parameter block, hit buffers and result
 // block: the unit a search chain runs on.  Single calls use lane 0; sbg_search_batch() spreads
 // independent searches over the lanes so that their kernels overlap on the device.
 struct sbg_lane {
   cudaStream_t own_stream = nullptr;
   cudaStream_t stream = nullptr;
-  DevCtl *d_ctl = nullptr;
-  DevParams7 *d_par7 = nullptr;
-  uint8_t *d_pos5 = nullptr;
-  uint16_t *d_order3 = nullptr;
+  DevArray<DevCtl> d_ctl;
+  DevArray<DevParams7> d_par7;
+  DevArray<uint8_t> d_pos5;
   HostOut *h_out = nullptr;      // mapped pinned: written by the device, polled here
   HostOut *d_out = nullptr;      // the same block through its device address
   DevCtl *h_ctl = nullptr;       // pinned: control words read back by the step-by-step calls
-  uint64_t *d_hits = nullptr;    // unordered hits (filter7) / (rank, tuple) pairs (two-kernel search5)
-  uint64_t *d_aux = nullptr;     // (ticket, index in ticket) of each hit
-  uint64_t *d_sorted = nullptr;  // the ordered, capped list (SBG_LIST_CAP entries)
-  uint32_t *d_tcount = nullptr;  // hits per ticket
-  uint32_t *d_toffset = nullptr; // their exclusive prefix sum
-  uint32_t *d_gcount = nullptr;  // hits per group of 1,024 tickets
-  uint64_t *d_sieve3 = nullptr;  // phase 1's pair sieve per 3-gate prefix (k_sieve3)
-  uint64_t sieve3_entries = 0;
-  size_t hits_cap = 0;
-  size_t tickets_alloc = 0;
+  // d_hits and d_aux grow together: d_hits.cap is the hit buffers' capacity
+  DevArray<uint64_t> d_hits;     // unordered hits (filter7) / (rank, tuple) pairs (two-kernel search5)
+  DevArray<uint64_t> d_aux;      // (ticket, index in ticket) of each hit
+  DevArray<uint64_t> d_sorted;   // the ordered, capped list (SBG_LIST_CAP entries)
+  DevArray<uint32_t> d_tcount;   // hits per ticket
+  DevArray<uint32_t> d_toffset;  // their exclusive prefix sum
+  DevArray<uint32_t> d_gcount;   // hits per group of 1,024 tickets
+  DevArray<uint64_t> d_sieve3;   // phase 1's pair sieve per 3-gate prefix (k_sieve3)
   cudaEvent_t ev[8] = {};        // timing (only with sbg_set_timing)
   cudaEvent_t ev_done = nullptr; // end of the lane's last chain
   bool ev_ready = false;
@@ -149,24 +162,25 @@ struct sbg_lane {
   float ms[4] = {0, 0, 0, 0};
   uint64_t last_key = SBG_KEY_NONE;   // sbg_decomp7_part's result and the two list entries behind it
   uint64_t last_tuple = 0, last_tuple_prev = 0;
-  // enumeration (sbg_enum5 / sbg_enum7; allocated on the first call)
-  EnumCtl *d_ectl = nullptr;
-  uint32_t *d_ecount = nullptr;             // matches per ticket
-  unsigned long long *d_eoffset = nullptr;  // their exclusive prefix sum
-  DevMatch *d_ematch = nullptr;             // the emitted records
-  unsigned long long *d_ehist = nullptr;    // filtered count: matches per depth (kDepthBins)
-  uint64_t ecount_cap = 0, eoffset_cap = 0, ematch_cap = 0, ehist_cap = 0;
-  // fetch and pick on an enumeration cursor (allocated on the first call)
-  unsigned long long *d_pranks = nullptr;   // requested ranks, ascending
-  unsigned int *d_pslots = nullptr;         // their output slots
-  unsigned long long *d_ptickets = nullptr; // ticket of each rank, then the distinct tickets
-  unsigned int *d_pfirst = nullptr;         // each distinct ticket's first rank in d_pranks
-  uint64_t pranks_cap = 0, pslots_cap = 0, ptickets_cap = 0, pfirst_cap = 0;
-  // global ranks (sbg_enum_block_sums / sbg_enum_set_global; allocated on the first call)
-  unsigned long long *d_bsums = nullptr;    // the share's block sums
-  unsigned long long *d_delta = nullptr;    // what k_enum_rebase adds to each of its blocks
-  unsigned long long *d_gsums = nullptr;    // every share's block sums, one row per part
-  uint64_t bsums_cap = 0, delta_cap = 0, gsums_cap = 0;
+};
+
+// The enumeration's device buffers, each allocated on its first need.  Enumerations run on lane 0
+// only, so the handle holds one set and grows it on lane 0's stream.
+struct EnumBuffers {
+  DevArray<EnumCtl> d_ectl;
+  DevArray<uint32_t> d_ecount;             // matches per ticket
+  DevArray<unsigned long long> d_eoffset;  // their exclusive prefix sum
+  DevArray<DevMatch> d_ematch;             // the emitted records
+  DevArray<unsigned long long> d_ehist;    // filtered count: matches per depth (kDepthBins)
+  // fetch and pick on an enumeration cursor
+  DevArray<unsigned long long> d_pranks;   // requested ranks, ascending
+  DevArray<unsigned int> d_pslots;         // their output slots
+  DevArray<unsigned long long> d_ptickets; // ticket of each rank, then the distinct tickets
+  DevArray<unsigned int> d_pfirst;         // each distinct ticket's first rank in d_pranks
+  // global ranks (sbg_enum_block_sums / sbg_enum_set_global)
+  DevArray<unsigned long long> d_bsums;    // the share's block sums
+  DevArray<unsigned long long> d_delta;    // what k_enum_rebase adds to each of its blocks
+  DevArray<unsigned long long> d_gsums;    // every share's block sums, one row per part
 };
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
@@ -196,7 +210,8 @@ struct FunctionFilter {
 };
 
 // The enumeration cursor: what sbg_enum_fetch / sbg_enum_pick need of the last counted enumeration
-// besides the counts and offsets it left in lane 0.  Valid while seq equals the handle's api_seq.
+// besides the counts and offsets it left in the handle's EnumBuffers.  Valid while seq equals the
+// handle's api_seq.
 struct EnumCursor {
   bool made = false;
   uint64_t seq = 0;
@@ -214,10 +229,11 @@ struct sbg_handle {
   sbg_lane lane[kLanes];
   cudaStream_t user_stream = nullptr;
 
-  DevProblem *d_slots = nullptr; // kSlots device-resident problems
+  DevArray<DevProblem> d_slots;  // kSlots device-resident problems
   uint64_t *h_stage = nullptr;   // pinned staging block for large table changes
-  DevTables *d_tab = nullptr;    // lane-indexed ordering tables
-  uint32_t *d_scratch = nullptr; // sbg_alu_peak
+  DevArray<DevTables> d_tab;     // lane-indexed ordering tables
+  DevArray<uint32_t> d_scratch;  // sbg_alu_peak
+  EnumBuffers ebuf;
 
   // host copies of the staged problems (for sbg_finish*)
   struct HostProblem {
@@ -301,6 +317,24 @@ int fail(sbg_handle *h, int code, const char *fmt, ...) {
           __FILE__, __LINE__);                                                             \
     }                                                                                      \
   } while (0)
+
+}  // namespace
+
+// Grows the array to `need` elements.  Work queued on `stream` may still read the old array, so
+// growing waits for it; the contents are not kept.
+template <class T>
+int DevArray<T>::grow(sbg_handle *h, cudaStream_t stream, uint64_t need) {
+  if (cap >= need) return SBG_OK;
+  SBG_CUDA(h, cudaStreamSynchronize(stream));
+  cudaFree(p);
+  p = nullptr;
+  cap = 0;
+  SBG_CUDA(h, cudaMalloc(&p, need * sizeof(T)));
+  cap = need;
+  return SBG_OK;
+}
+
+namespace {
 
 template <int NW>
 size_t sweep_smem(int n) {
@@ -512,54 +546,33 @@ sbg_handle::HostProblem &cur(sbg_handle *h) { return h->slots[h->cur_slot]; }
 
 // ---- lane resources (allocated on first need: most graphs never run a large 7-LUT search) ------
 
-int ensure_hits(sbg_handle *h, sbg_lane &L, size_t cap) {
-  if (L.d_hits != nullptr && L.hits_cap >= cap) return SBG_OK;
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  if (L.d_hits != nullptr) {
-    cudaFree(L.d_hits);
-    cudaFree(L.d_aux);
-    L.d_hits = L.d_aux = nullptr;
-  }
-  SBG_CUDA(h, cudaMalloc(&L.d_hits, cap * sizeof(uint64_t)));
-  SBG_CUDA(h, cudaMalloc(&L.d_aux, cap * sizeof(uint64_t)));
-  L.hits_cap = cap;
-  if (L.d_sorted == nullptr) {
-    SBG_CUDA(h, cudaMalloc(&L.d_sorted, (size_t)SBG_LIST_CAP * sizeof(uint64_t)));
-  }
-  return SBG_OK;
+int ensure_hits(sbg_handle *h, sbg_lane &L, uint64_t cap) {
+  int rc;
+  if ((rc = L.d_hits.grow(h, L.stream, cap)) != SBG_OK) return rc;
+  if ((rc = L.d_aux.grow(h, L.stream, cap)) != SBG_OK) return rc;
+  return L.d_sorted.grow(h, L.stream, SBG_LIST_CAP);
 }
 
 int ensure_tickets(sbg_handle *h, sbg_lane &L, uint64_t tickets) {
-  if (L.d_tcount != nullptr && L.tickets_alloc >= tickets) return SBG_OK;
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  if (L.d_tcount != nullptr) {
-    cudaFree(L.d_tcount);
-    cudaFree(L.d_toffset);
-    cudaFree(L.d_gcount);
+  uint64_t want = L.d_tcount.cap;
+  if (want < tickets) {
+    // grow generously: reallocation synchronises the lane
+    want = std::max<uint64_t>(tickets, (uint64_t)1 << 18);
+    want = std::min<uint64_t>(std::max<uint64_t>(want, 2 * L.d_tcount.cap),
+        h->ticket_table_max + kTicketSlack);
+    want = std::max<uint64_t>(want, tickets);
   }
-  // grow generously: reallocation synchronises the lane
-  uint64_t want = std::max<uint64_t>(tickets, (uint64_t)1 << 18);
-  want = std::min<uint64_t>(std::max<uint64_t>(want, 2 * L.tickets_alloc), h->ticket_table_max + kTicketSlack);
-  want = std::max<uint64_t>(want, tickets);
-  SBG_CUDA(h, cudaMalloc(&L.d_tcount, want * sizeof(uint32_t)));
-  SBG_CUDA(h, cudaMalloc(&L.d_toffset, want * sizeof(uint32_t)));
-  SBG_CUDA(h, cudaMalloc(&L.d_gcount, (want / kTicketGroup + 2) * sizeof(uint32_t)));
-  L.tickets_alloc = want;
-  return SBG_OK;
+  int rc;
+  if ((rc = L.d_tcount.grow(h, L.stream, want)) != SBG_OK) return rc;
+  if ((rc = L.d_toffset.grow(h, L.stream, want)) != SBG_OK) return rc;
+  return L.d_gcount.grow(h, L.stream, want / kTicketGroup + 2);
 }
 
 // The k_sieve3 table for n gates: C(n - 4, 3) entries of kSieve3Words words, 7.3 MB at n = 40,
 // 28.4 MB at n = 60 (the shifted windows' limit).  Entry ranks do not depend on n, so a table
 // allocated for a larger n serves every smaller one.
 int ensure_sieve3(sbg_handle *h, sbg_lane &L, int n) {
-  const uint64_t entries = h_binom[n - 4][3];
-  if (L.d_sieve3 != nullptr && L.sieve3_entries >= entries) return SBG_OK;
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  cudaFree(L.d_sieve3);
-  L.d_sieve3 = nullptr;
-  SBG_CUDA(h, cudaMalloc(&L.d_sieve3, entries * kSieve3Words * sizeof(uint64_t)));
-  L.sieve3_entries = entries;
-  return SBG_OK;
+  return L.d_sieve3.grow(h, L.stream, h_binom[n - 4][3] * kSieve3Words);
 }
 
 // The chain about to be enqueued on lane L reads problem slot `slot`: order it after the slot's
@@ -621,7 +634,8 @@ int wait_stage(sbg_handle *h, sbg_lane &L, int stage) {
 
 // Control words of the lane, by copy (the step-by-step calls, which do not close a stage).
 int fetch_ctl(sbg_handle *h, sbg_lane &L) {
-  SBG_CUDA(h, cudaMemcpyAsync(L.h_ctl, L.d_ctl, sizeof(DevCtl), cudaMemcpyDeviceToHost, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(L.h_ctl, L.d_ctl.p, sizeof(DevCtl), cudaMemcpyDeviceToHost,
+      L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   return SBG_OK;
 }
@@ -679,12 +693,13 @@ int enqueue_search5(sbg_handle *h, sbg_lane &L, int part, int nparts, bool two, 
     const int grid = grid_for(h, k_sweep<NW>, smem, tickets + chunk_tickets);
     const uint64_t bsz = pick_batch(h, tickets, n, P);
     cudaError_t e = launch(h, k_sweep<NW>, grid, kThreads, smem, L.stream, !h->timing,
-        h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_pos5, L.d_hits, (unsigned long long)L.hits_cap,
-        part, nparts, (int)bsz, two, h->d_tab, pl.all ? (unsigned long long)total : pl.t_offset,
-        pl.items, std::max(1, pl.chunks), (unsigned long long)chunk_tickets);
+        h->d_slots.p + L.slot, L.d_ctl.p, L.d_out, L.d_pos5.p, L.d_hits.p,
+        (unsigned long long)L.d_hits.cap, part, nparts, (int)bsz, two, h->d_tab.p,
+        pl.all ? (unsigned long long)total : pl.t_offset, pl.items, std::max(1, pl.chunks),
+        (unsigned long long)chunk_tickets);
     if (e == cudaSuccess && two) {
       e = launch(h, k_decomp5<NW>, 2 * h->sm_count, kThreads, decomp_smem<NW>(n), L.stream, true,
-          h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_pos5, L.d_hits, h->d_tab);
+          h->d_slots.p + L.slot, L.d_ctl.p, L.d_out, L.d_pos5.p, L.d_hits.p, h->d_tab.p);
     }
     return e;
   });
@@ -783,7 +798,7 @@ FilterPlan plan_filter_p(const sbg_handle *h, const sbg_lane &L, const sbg_handl
   // fewer than cap + w x (hits one item can emit) entries; a whole prefix stops by itself after
   // cap + one chunk.
   fp.max_warps = !retry ? 0 : (int)std::max<size_t>(1, fp.pl.all
-      ? (L.hits_cap - SBG_LIST_CAP) / kPerChunkMax : L.hits_cap / kPerPrefixMax - 1);
+      ? (L.d_hits.cap - SBG_LIST_CAP) / kPerChunkMax : L.d_hits.cap / kPerPrefixMax - 1);
   fp.tickets = fp.pl.all ? 0 : (fp.total - fp.pl.t_offset + nparts - 1) / nparts;
   // chunk tickets of one part: whole deal blocks, the same count for every part
   fp.chunk_tickets = (fp.pl.items + kDeal * nparts - 1) / (kDeal * nparts) * kDeal;
@@ -840,12 +855,12 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
       int grid = grid_for(h, kernel, smem, fp.tickets + fp.chunk_tickets);
       if (fp.max_warps > 0) grid = std::min(grid, (fp.max_warps + kWarpsPerCta - 1) / kWarpsPerCta);
       const cudaError_t e = launch(h, kernel, grid, kThreads, smem, L.stream, !h->timing,
-          h->d_slots + L.slot, L.d_ctl, L.d_hits, L.d_aux, L.d_tcount, L.d_gcount,
-          (unsigned long long)L.hits_cap, (unsigned long long)fp.tickets_cap, part, nparts,
+          h->d_slots.p + L.slot, L.d_ctl.p, L.d_hits.p, L.d_aux.p, L.d_tcount.p, L.d_gcount.p,
+          (unsigned long long)L.d_hits.cap, (unsigned long long)fp.tickets_cap, part, nparts,
           list_cap, (int)fp.batch, fp.max_warps,
           pl.all ? (unsigned long long)fp.total : pl.t_offset, pl.items, std::max(1, pl.chunks),
           (unsigned long long)fp.chunk_tickets, (unsigned long long)fp.seg_base,
-          h->opt_packed ? 15 : 0, fp.wt, (const uint64_t *)L.d_sieve3);
+          h->opt_packed ? 15 : 0, fp.wt, (const uint64_t *)L.d_sieve3.p);
       if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_filter7_pm: %s", cudaGetErrorString(e));
       return SBG_OK;
     };
@@ -856,7 +871,7 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
           if ((rc = ensure_sieve3(h, L, n)) != SBG_OK) return rc;
           const int grid = (int)((h_binom[n - 4][3] + kWarpsPerCta - 1) / kWarpsPerCta);
           const cudaError_t e = launch(h, k_sieve3<NW>, grid, kThreads, 0, L.stream, !h->timing,
-              h->d_slots + L.slot, (const DevCtl *)L.d_ctl, L.d_sieve3);
+              h->d_slots.p + L.slot, (const DevCtl *)L.d_ctl.p, L.d_sieve3.p);
           if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_sieve3: %s", cudaGetErrorString(e));
         }
         return run(k_filter7_pm<NW, 1, P, true, true, true>, true, true);
@@ -885,12 +900,13 @@ int enqueue_filter7(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int part, 
   if (h->timing) cudaEventRecord(L.ev[1], L.stream);
   const uint64_t groups = (fp.tickets_cap + kTicketGroup - 1) / kTicketGroup;
   // the grid covers the tickets that can have been handed out; CTAs past the counter return at once
-  cudaError_t e = launch(h, k_offsets, (int)groups, 256, 0, L.stream, !h->timing, L.d_ctl,
-      L.d_tcount, L.d_gcount, L.d_toffset, (unsigned long long)fp.tickets_cap,
+  cudaError_t e = launch(h, k_offsets, (int)groups, 256, 0, L.stream, !h->timing, L.d_ctl.p,
+      L.d_tcount.p, L.d_gcount.p, L.d_toffset.p, (unsigned long long)fp.tickets_cap,
       (unsigned int)SBG_LIST_CAP, (unsigned int)fp.list_base);
   if (e == cudaSuccess) {
-    e = launch(h, k_scatter, 2 * h->sm_count, 256, 0, L.stream, true, L.d_ctl, L.d_hits, L.d_aux,
-        L.d_toffset, L.d_sorted, (unsigned long long)L.hits_cap, (unsigned int)SBG_LIST_CAP);
+    e = launch(h, k_scatter, 2 * h->sm_count, 256, 0, L.stream, true, L.d_ctl.p, L.d_hits.p,
+        L.d_aux.p, L.d_toffset.p, L.d_sorted.p, (unsigned long long)L.d_hits.cap,
+        (unsigned int)SBG_LIST_CAP);
   }
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "ordering launch: %s", cudaGetErrorString(e));
   if (h->timing) {
@@ -909,8 +925,8 @@ int enqueue_decomp7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint64_t i
     const size_t smem = decomp_smem<NW>(n);
     const int grid = grid_for(h, k_decomp7<NW>, smem, items_hint);
     return launch(h, k_decomp7<NW>, grid, kThreads, smem, L.stream, !h->timing,
-        h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_par7, L.d_sorted, part, nparts, h->d_tab,
-        h->opt_decomp_filter);
+        h->d_slots.p + L.slot, L.d_ctl.p, L.d_out, L.d_par7.p, L.d_sorted.p, part, nparts,
+        h->d_tab.p, h->opt_decomp_filter);
   });
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_decomp7: %s", cudaGetErrorString(e));
   if (h->timing) cudaEventRecord(L.ev[3], L.stream);
@@ -956,7 +972,7 @@ int run_filter7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint32_t *coun
   bool retry = false;
   if (overflowed_already) {
     // the caller's own launch (the fused chain) has just overflowed this buffer: do not repeat it
-    if (!h->hits_cap_forced && L.hits_cap < kGrownHitsCap) {
+    if (!h->hits_cap_forced && L.d_hits.cap < kGrownHitsCap) {
       if ((rc = ensure_hits(h, L, kGrownHitsCap)) != SBG_OK) return rc;
     } else {
       retry = true;
@@ -966,7 +982,7 @@ int run_filter7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint32_t *coun
   uint32_t list_base = 0;
   float ms_filter = 0.f, ms_order = 0.f;
   for (int overflows = 0;;) {
-    if ((rc = ensure_hits(h, L, std::max(L.hits_cap, h->hits_cap_default))) != SBG_OK) return rc;
+    if ((rc = ensure_hits(h, L, std::max(L.d_hits.cap, h->hits_cap_default))) != SBG_OK) return rc;
     FilterPlan fp = plan_filter(h, L, hp, nparts, retry, seg_base);
     fp.list_base = list_base;
     if ((rc = ensure_tickets(h, L, fp.tickets_cap)) != SBG_OK) return rc;
@@ -988,9 +1004,9 @@ int run_filter7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint32_t *coun
       // parallelism: a prefix stops contributing once it has emitted SBG_LIST_CAP hits and items
       // are handed out in order, so with w warps at work (w + 1) * (hits per item) entries suffice
       if (++overflows > 2) {
-        return fail(h, SBG_ERR_OVERFLOW, "7-LUT hit buffer (%zu entries) overflowed", L.hits_cap);
+        return fail(h, SBG_ERR_OVERFLOW, "7-LUT hit buffer (%zu entries) overflowed", L.d_hits.cap);
       }
-      if (!h->hits_cap_forced && L.hits_cap < kGrownHitsCap && !retry) {
+      if (!h->hits_cap_forced && L.d_hits.cap < kGrownHitsCap && !retry) {
         if ((rc = ensure_hits(h, L, kGrownHitsCap)) != SBG_OK) return rc;
       } else {
         retry = true;
@@ -1036,7 +1052,7 @@ int apply_pending(sbg_handle *h, int slot, cudaStream_t stream, BeginArgs &a, bo
     if (changed > kArgGates) {
       SBG_CUDA(h, cudaStreamSynchronize(stream));   // the staging block may still be in flight
       memcpy(h->h_stage, hp.tables[hp.dev_n], (size_t)changed * 32);
-      SBG_CUDA(h, cudaMemcpyAsync(&h->d_slots[slot].full[hp.dev_n][0], h->h_stage,
+      SBG_CUDA(h, cudaMemcpyAsync(&h->d_slots.p[slot].full[hp.dev_n][0], h->h_stage,
           (size_t)changed * 32, cudaMemcpyHostToDevice, stream));
       h->uploads_full++;
       h->h2d_bytes += (uint64_t)changed * 32;
@@ -1132,7 +1148,7 @@ int stage_problem(sbg_handle *h, int slot, const uint64_t *tables, int n, const 
     const int ctas = prep_ctas(hp, a);
     if (ctas > 0) {
       const cudaError_t e = launch(h, k_prepare_problem, ctas, 1024, 0, h->lane[0].stream, false,
-          h->d_slots + slot, a);
+          h->d_slots.p + slot, a);
       if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_prepare_problem: %s", cudaGetErrorString(e));
     }
     if (hp.uploaded != nullptr) SBG_CUDA(h, cudaEventRecord(hp.uploaded, h->lane[0].stream));
@@ -1175,7 +1191,8 @@ int enqueue_begin(sbg_handle *h, sbg_lane &L, uint32_t flags, const CallInputs &
   // shared memory
   const size_t smem = std::max<size_t>(sizeof(uint32_t) * kMinpos3, (size_t)hp.n * 32);
   const cudaError_t e = launch(h, k_begin, 1 + prep + scan, 1024, smem, L.stream, false,
-      h->d_slots + L.slot, L.d_ctl, L.d_out, L.d_par7, L.d_pos5, L.d_gcount, h->d_tab, prep, a);
+      h->d_slots.p + L.slot, L.d_ctl.p, L.d_out, L.d_par7.p, L.d_pos5.p, L.d_gcount.p, h->d_tab.p,
+      prep, a);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_begin: %s", cudaGetErrorString(e));
   L.prepared = (a.flags & kBeginProblem) != 0;
   if (L.prepared && L.mark_begun) SBG_CUDA(h, cudaEventRecord(L.ev_begun, L.stream));
@@ -1196,7 +1213,7 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
   uint32_t gcount_n = 0;
   FilterPlan fp;
   if (flags & kBeginSearch7) {
-    if ((rc = ensure_hits(h, L, std::max(L.hits_cap, h->hits_cap_default))) != SBG_OK) return rc;
+    if ((rc = ensure_hits(h, L, std::max(L.d_hits.cap, h->hits_cap_default))) != SBG_OK) return rc;
     fp = plan_filter(h, L, hp, 1, false);
     if ((rc = ensure_tickets(h, L, fp.tickets_cap)) != SBG_OK) return rc;
     gcount_n = (uint32_t)(fp.tickets_cap / kTicketGroup + 1);
@@ -1467,24 +1484,10 @@ constexpr uint64_t kEnumWindow3 = kNominalWarps;
 constexpr uint64_t kEnumWindow5 = kNominalWarps;
 constexpr uint64_t kEnumWindow7 = kNominalWarps / 4;
 
-// Grows the lane's device buffer p (cap elements now) to `need` elements.  The lane's queued work
-// may still read the old buffer, so growing waits for it; the contents are not kept.
-template <class T>
-int grow(sbg_handle *h, sbg_lane &L, T *&p, uint64_t &cap, uint64_t need) {
-  if (cap >= need) return SBG_OK;
-  SBG_CUDA(h, cudaStreamSynchronize(L.stream));
-  cudaFree(p);
-  p = nullptr;
-  cap = 0;
-  SBG_CUDA(h, cudaMalloc(&p, need * sizeof(T)));
-  cap = need;
-  return SBG_OK;
-}
-
 // The first n emitted records to the caller's out.
 int copy_matches(sbg_handle *h, sbg_lane &L, sbg_match *out, uint64_t n) {
-  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ematch, n * sizeof(sbg_match), cudaMemcpyDeviceToHost,
-      L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(out, h->ebuf.d_ematch.p, n * sizeof(sbg_match),
+      cudaMemcpyDeviceToHost, L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   h->d2h_bytes += n * sizeof(sbg_match);
   return SBG_OK;
@@ -1498,7 +1501,8 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
   static_assert(WIDTH == 3 || WIDTH == 5 || WIDTH == 7, "enumeration widths are 3, 5 and 7");
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const int n = hp.n;
-  const DevProblem *prob = h->d_slots + L.slot;
+  const DevProblem *prob = h->d_slots.p + L.slot;
+  const EnumBuffers &E = h->ebuf;
   const int rc = with_nw(hp.nw, [&](auto nw_c) {
     constexpr int NW = decltype(nw_c)::value;
     auto run = [&](auto kernel, size_t smem, auto... args) {
@@ -1514,25 +1518,27 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
       EnumFilterOf<FORM> flt = {};
       if constexpr (FORM != kFormPlain) {
         flt = in.filter;
-        flt.hist = L.d_ehist;
+        flt.hist = E.d_ehist.p;
       }
       if constexpr (WIDTH == 3) {
-        return run(k_enum3<NW, MODE, FORM>, decomp_smem<NW>(n), prob, L.d_ectl, in.gates,
-            L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, flt);
+        return run(k_enum3<NW, MODE, FORM>, decomp_smem<NW>(n), prob, E.d_ectl.p, in.gates,
+            E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, flt);
       } else if constexpr (WIDTH == 5) {
-        return run(k_enum5<NW, MODE, FORM>, sweep_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_ecount,
-            L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts, h->d_tab, flt);
+        return run(k_enum5<NW, MODE, FORM>, sweep_smem<NW>(n), prob, E.d_ectl.p, in.ord,
+            E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, h->d_tab.p,
+            flt);
       } else {
-        return run(k_enum7<NW, MODE, FORM>, decomp_smem<NW>(n), prob, L.d_ectl, in.ord, L.d_sorted,
-            L.list_count, L.d_ecount, L.d_eoffset, L.d_ematch, max_out, a, b, part, nparts,
-            h->d_tab, flt);
+        return run(k_enum7<NW, MODE, FORM>, decomp_smem<NW>(n), prob, E.d_ectl.p, in.ord,
+            L.d_sorted.p, L.list_count, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b,
+            part, nparts, h->d_tab.p, flt);
       }
     });
   });
   if (rc != SBG_OK) return rc;
   if (MODE == kEnumCount) {
-    const cudaError_t e = launch(h, k_enum_scan, 1, 1024, 0, L.stream, false, L.d_ectl,
-        (const uint32_t *)L.d_ecount, L.d_eoffset, (unsigned long long)a, (unsigned long long)b);
+    const cudaError_t e = launch(h, k_enum_scan, 1, 1024, 0, L.stream, false, E.d_ectl.p,
+        (const uint32_t *)E.d_ecount.p, E.d_eoffset.p, (unsigned long long)a,
+        (unsigned long long)b);
     if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_scan: %s", cudaGetErrorString(e));
   }
   return SBG_OK;
@@ -1558,6 +1564,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
     uint64_t *feasible) {
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
+  EnumBuffers &E = h->ebuf;
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
   if (WIDTH == 7 && !(L.list_ready && list_of_current(h))) {
@@ -1574,14 +1581,14 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   const uint64_t items = WIDTH == 3 ? h_binom[n][2] : WIDTH == 5 ? h_binom[n - 2][3] : L.list_count;
   const uint64_t blocks = (items + B - 1) / B;
   const uint64_t tickets = deal_share(blocks, part, nparts) * B;
-  if (L.d_ectl == nullptr) SBG_CUDA(h, cudaMalloc(&L.d_ectl, sizeof(EnumCtl)));
+  if ((rc = E.d_ectl.grow(h, L.stream, 1)) != SBG_OK) return rc;
   const uint64_t room = std::max<uint64_t>(tickets, 1);
-  if ((rc = grow(h, L, L.d_ecount, L.ecount_cap, room)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_eoffset, L.eoffset_cap, room)) != SBG_OK) return rc;
-  SBG_CUDA(h, cudaMemsetAsync(L.d_ectl, 0, sizeof(EnumCtl), L.stream));
+  if ((rc = E.d_ecount.grow(h, L.stream, room)) != SBG_OK) return rc;
+  if ((rc = E.d_eoffset.grow(h, L.stream, room)) != SBG_OK) return rc;
+  SBG_CUDA(h, cudaMemsetAsync(E.d_ectl.p, 0, sizeof(EnumCtl), L.stream));
   if (in.form != kFormPlain) {
-    if ((rc = grow(h, L, L.d_ehist, L.ehist_cap, (uint64_t)kDepthBins)) != SBG_OK) return rc;
-    SBG_CUDA(h, cudaMemsetAsync(L.d_ehist, 0, kDepthBins * sizeof(unsigned long long), L.stream));
+    if ((rc = E.d_ehist.grow(h, L.stream, (uint64_t)kDepthBins)) != SBG_OK) return rc;
+    SBG_CUDA(h, cudaMemsetAsync(E.d_ehist.p, 0, kDepthBins * sizeof(unsigned long long), L.stream));
   }
   const bool count_all = total != nullptr;
   uint64_t window = count_all ? tickets
@@ -1596,16 +1603,16 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
     window *= 2;
     if (!count_all) {
       // ordered stop: every later ticket holds larger keys only
-      SBG_CUDA(h, cudaMemcpyAsync(&ec, L.d_ectl, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
+      SBG_CUDA(h, cudaMemcpyAsync(&ec, E.d_ectl.p, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
       SBG_CUDA(h, cudaStreamSynchronize(L.stream));
       if (ec.carry >= max_matches) break;
     }
   }
-  SBG_CUDA(h, cudaMemcpyAsync(&ec, L.d_ectl, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(&ec, E.d_ectl.p, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   const uint64_t emit = std::min<uint64_t>(max_matches, ec.carry);
   if (emit > 0) {
-    if ((rc = grow(h, L, L.d_ematch, L.ematch_cap, emit)) != SBG_OK) return rc;
+    if ((rc = E.d_ematch.grow(h, L.stream, emit)) != SBG_OK) return rc;
     if ((rc = launch_enum<WIDTH, kEnumFirst>(h, L, in, part, nparts, emit, 0, done)) != SBG_OK) return rc;
     if ((rc = copy_matches(h, L, out, emit)) != SBG_OK) return rc;
   }
@@ -1722,49 +1729,52 @@ int check_cursor(sbg_handle *h) {
         "sbg_enum3 / sbg_enum5 / sbg_enum7 call with nothing in between");
   }
   const sbg_lane &L = h->lane[0];
-  if (L.slot != c.slot || L.ecount_cap < c.tickets || (c.width == 7 && L.list_count != c.list_count)) {
+  if (L.slot != c.slot || h->ebuf.d_ecount.cap < c.tickets
+      || (c.width == 7 && L.list_count != c.list_count)) {
     return fail(h, SBG_ERR_STATE, "internal: enumeration cursor out of step with its buffers");
   }
   return SBG_OK;
 }
 
-// Ticket of each of ranks[0..nranks-1] (already in L.d_pranks) into L.d_ptickets.  owned: ranks
+// Ticket of each of ranks[0..nranks-1] (already in d_pranks) into d_ptickets.  owned: ranks
 // outside their ticket's range (global ranks other shares hold) get kEnumUnowned.
 int locate_tickets(sbg_handle *h, sbg_lane &L, uint64_t nranks, bool owned = false) {
+  const EnumBuffers &E = h->ebuf;
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nranks + 255) / 256,
       (uint64_t)h->sm_count * 8));
   const cudaError_t e = launch(h, k_enum_locate, grid, 256, 0, L.stream, false,
-      (const unsigned long long *)L.d_eoffset, (unsigned long long)h->cursor.tickets,
-      (const unsigned long long *)L.d_pranks, (unsigned long long)nranks, L.d_ptickets,
-      owned ? (const uint32_t *)L.d_ecount : (const uint32_t *)nullptr);
+      (const unsigned long long *)E.d_eoffset.p, (unsigned long long)h->cursor.tickets,
+      (const unsigned long long *)E.d_pranks.p, (unsigned long long)nranks, E.d_ptickets.p,
+      owned ? (const uint32_t *)E.d_ecount.p : (const uint32_t *)nullptr);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_locate: %s", cudaGetErrorString(e));
   return SBG_OK;
 }
 
 // ---- global ranks across shares (sbg_enum_block_sums / sbg_enum_set_global) ---------------------
 
-// The cursor's block sums into L.d_bsums (and room for as many deltas in L.d_delta).
+// The cursor's block sums into d_bsums (and room for as many deltas in d_delta).
 int block_sums(sbg_handle *h, sbg_lane &L, uint64_t nblocks) {
+  EnumBuffers &E = h->ebuf;
   int rc;
-  if ((rc = grow(h, L, L.d_bsums, L.bsums_cap, nblocks)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_delta, L.delta_cap, nblocks)) != SBG_OK) return rc;
+  if ((rc = E.d_bsums.grow(h, L.stream, nblocks)) != SBG_OK) return rc;
+  if ((rc = E.d_delta.grow(h, L.stream, nblocks)) != SBG_OK) return rc;
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nblocks + 255) / 256,
       (uint64_t)h->sm_count * 8));
   const cudaError_t e = launch(h, k_enum_block_sums, grid, 256, 0, L.stream, false,
-      (const uint32_t *)L.d_ecount, (unsigned long long)nblocks, enum_block_size(h->cursor.width),
-      L.d_bsums);
+      (const uint32_t *)E.d_ecount.p, (unsigned long long)nblocks, enum_block_size(h->cursor.width),
+      E.d_bsums.p);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_block_sums: %s", cudaGetErrorString(e));
   return SBG_OK;
 }
 
 // A range or pick emit pass of the cursor's width over tickets [a, b) (pick: entries [a, b) of
-// sel.tickets) into L.d_ematch; sel travels in the lane's EnumCtl block.
+// sel.tickets) into d_ematch; sel travels in the EnumCtl block.
 template <int MODE>
 int emit_sel(sbg_handle *h, sbg_lane &L, uint64_t max_out, uint64_t a, uint64_t b,
     const EnumSel &sel) {
   const EnumCursor &c = h->cursor;
-  SBG_CUDA(h, cudaMemcpyAsync(reinterpret_cast<char *>(L.d_ectl) + offsetof(EnumCtl, sel), &sel,
-      sizeof(sel), cudaMemcpyHostToDevice, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(reinterpret_cast<char *>(h->ebuf.d_ectl.p) + offsetof(EnumCtl, sel),
+      &sel, sizeof(sel), cudaMemcpyHostToDevice, L.stream));
   switch (c.width) {
     case 3: return launch_enum<3, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
     case 5: return launch_enum<5, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
@@ -1925,6 +1935,7 @@ int sbg_create(sbg_handle **out, int device) {
     h->hits_cap_default = std::max<size_t>((size_t)strtoull(cap_env, nullptr, 10), 3 * kPerPrefixMax);
     h->hits_cap_forced = true;
   }
+  int rc;
   for (int i = 0; i < kLanes; i++) {
     sbg_lane &L = h->lane[i];
     SBG_CUDA(h, cudaStreamCreateWithFlags(&L.own_stream, cudaStreamNonBlocking));
@@ -1932,17 +1943,15 @@ int sbg_create(sbg_handle **out, int device) {
     for (int k = 0; k < 8; k++) SBG_CUDA(h, cudaEventCreate(&L.ev[k]));
     SBG_CUDA(h, cudaEventCreateWithFlags(&L.ev_done, cudaEventDisableTiming));
     SBG_CUDA(h, cudaEventCreateWithFlags(&L.ev_begun, cudaEventDisableTiming));
-    SBG_CUDA(h, cudaMalloc(&L.d_ctl, sizeof(DevCtl)));
+    if ((rc = L.d_ctl.grow(h, L.stream, 1)) != SBG_OK) return rc;
     {
       DevCtl init;
       memset(&init, 0, sizeof(init));
       init.best3 = ~0ull;   // the 3-LUT scan expects (and leaves) ~0 here
-      SBG_CUDA(h, cudaMemcpy(L.d_ctl, &init, sizeof(init), cudaMemcpyHostToDevice));
+      SBG_CUDA(h, cudaMemcpy(L.d_ctl.p, &init, sizeof(init), cudaMemcpyHostToDevice));
     }
-    SBG_CUDA(h, cudaMalloc(&L.d_par7, sizeof(DevParams7)));
-    SBG_CUDA(h, cudaMalloc(&L.d_pos5, 256));
-    SBG_CUDA(h, cudaMalloc(&L.d_order3, 512 * sizeof(uint16_t)));
-    SBG_CUDA(h, cudaMalloc(&L.d_gcount, 64 * sizeof(uint32_t)));   // replaced by ensure_tickets
+    if ((rc = L.d_par7.grow(h, L.stream, 1)) != SBG_OK) return rc;
+    if ((rc = L.d_pos5.grow(h, L.stream, 256)) != SBG_OK) return rc;
     SBG_CUDA(h, cudaHostAlloc(&L.h_out, sizeof(HostOut), cudaHostAllocMapped));
     memset(L.h_out, 0, sizeof(HostOut));
     SBG_CUDA(h, cudaHostGetDevicePointer(&L.d_out, L.h_out, 0));
@@ -2042,8 +2051,8 @@ int sbg_create(sbg_handle **out, int device) {
       }
       host_tab->m3_level[9] = fill;
     }
-    SBG_CUDA(h, cudaMalloc(&h->d_tab, sizeof(DevTables)));
-    SBG_CUDA(h, cudaMemcpy(h->d_tab, host_tab, sizeof(DevTables), cudaMemcpyHostToDevice));
+    if ((rc = h->d_tab.grow(h, h->lane[0].stream, 1)) != SBG_OK) return rc;
+    SBG_CUDA(h, cudaMemcpy(h->d_tab.p, host_tab, sizeof(DevTables), cudaMemcpyHostToDevice));
     delete host_tab;
     SBG_CUDA(h, cudaMemcpyToSymbol(c_j_first_k, first_k, sizeof(first_k)));
     SBG_CUDA(h, cudaMemcpyToSymbol(c_j_rows, nrows, sizeof(nrows)));
@@ -2055,7 +2064,7 @@ int sbg_create(sbg_handle **out, int device) {
     SBG_CUDA(h, cudaMemcpyToSymbol(c_rows7, rows7, sizeof(rows7)));
   }
 
-  SBG_CUDA(h, cudaMalloc(&h->d_slots, sizeof(DevProblem) * kSlots));
+  if ((rc = h->d_slots.grow(h, h->lane[0].stream, kSlots)) != SBG_OK) return rc;
   h->slots = new sbg_handle::HostProblem[kSlots];
   for (int i = 0; i < kSlots; i++) {
     SBG_CUDA(h, cudaEventCreateWithFlags(&h->slots[i].uploaded, cudaEventDisableTiming));
@@ -2067,17 +2076,12 @@ int sbg_create(sbg_handle **out, int device) {
 
 void sbg_destroy(sbg_handle *h) {
   if (h == nullptr) return;
-  if (h->sm_count != 0) {   // a device was bound: release whatever was created
+  const bool bound = h->sm_count != 0;   // a device was bound: release whatever was created
+  if (bound) {
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
     for (int i = 0; i < kLanes; i++) {
       sbg_lane &L = h->lane[i];
-      cudaFree(L.d_ctl); cudaFree(L.d_par7); cudaFree(L.d_pos5); cudaFree(L.d_order3);
-      cudaFree(L.d_hits); cudaFree(L.d_aux); cudaFree(L.d_sorted);
-      cudaFree(L.d_tcount); cudaFree(L.d_toffset); cudaFree(L.d_gcount); cudaFree(L.d_sieve3);
-      cudaFree(L.d_ectl); cudaFree(L.d_ecount); cudaFree(L.d_eoffset); cudaFree(L.d_ematch);
-      cudaFree(L.d_pranks); cudaFree(L.d_pslots); cudaFree(L.d_ptickets); cudaFree(L.d_pfirst);
-      cudaFree(L.d_bsums); cudaFree(L.d_delta); cudaFree(L.d_gsums); cudaFree(L.d_ehist);
       if (L.h_out != nullptr) cudaFreeHost(L.h_out);
       if (L.h_ctl != nullptr) cudaFreeHost(L.h_ctl);
       for (int k = 0; k < 8; k++) if (L.ev[k] != nullptr) cudaEventDestroy(L.ev[k]);
@@ -2085,17 +2089,14 @@ void sbg_destroy(sbg_handle *h) {
       if (L.ev_begun != nullptr) cudaEventDestroy(L.ev_begun);
       if (L.own_stream != nullptr) cudaStreamDestroy(L.own_stream);
     }
-    cudaFree(h->d_slots);
-    cudaFree(h->d_tab);
-    cudaFree(h->d_scratch);
     if (h->h_stage != nullptr) cudaFreeHost(h->h_stage);
     if (h->slots != nullptr) {
       for (int i = 0; i < kSlots; i++) if (h->slots[i].uploaded != nullptr) cudaEventDestroy(h->slots[i].uploaded);
     }
-    (void)cudaGetLastError();
   }
   delete[] h->slots;
-  delete h;
+  delete h;   // the handle's DevArrays free its device memory, on the device still current
+  if (bound) (void)cudaGetLastError();
 }
 
 const char *sbg_last_error(const sbg_handle *h) { return h != nullptr ? h->err : "null handle"; }
@@ -2148,12 +2149,13 @@ int sbg_alu_peak(sbg_handle *h, double *warp_instr_per_s) {
   SBG_CUDA(h, cudaSetDevice(h->device));
   const int blocks = h->sm_count * 8, threads = 256, iters = 2048;
   constexpr int CH = 8;
-  if (h->d_scratch == nullptr) SBG_CUDA(h, cudaMalloc(&h->d_scratch, (size_t)blocks * threads * 4));
   sbg_lane &L = h->lane[0];
+  const int rc = h->d_scratch.grow(h, L.stream, (uint64_t)blocks * threads);
+  if (rc != SBG_OK) return rc;
   double best = 0.0;
   for (int rep = 0; rep < 4; rep++) {
     cudaEventRecord(L.ev[4], L.stream);
-    k_lop3_peak<CH><<<blocks, threads, 0, L.stream>>>(h->d_scratch, iters, 12345u + rep);
+    k_lop3_peak<CH><<<blocks, threads, 0, L.stream>>>(h->d_scratch.p, iters, 12345u + rep);
     cudaEventRecord(L.ev[5], L.stream);
     SBG_CUDA(h, cudaStreamSynchronize(L.stream));
     const float ms = elapsed(L.ev[4], L.ev[5]);
@@ -2267,7 +2269,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   for (int i = 0; i < 4; i++) h->last_ms[i] = L.ms[i];
   *count = (int)keep;
   if (list != nullptr && keep > 0) {
-    SBG_CUDA(h, cudaMemcpyAsync(list, L.d_sorted, (size_t)keep * sizeof(uint64_t),
+    SBG_CUDA(h, cudaMemcpyAsync(list, L.d_sorted.p, (size_t)keep * sizeof(uint64_t),
         cudaMemcpyDeviceToHost, L.stream));
     SBG_CUDA(h, cudaStreamSynchronize(L.stream));
     h->d2h_bytes += (uint64_t)keep * 8;
@@ -2281,7 +2283,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
 int sbg_list7_device(sbg_handle *h, const uint64_t **list, int *count) {
   if (h == nullptr || list == nullptr || count == nullptr) return SBG_ERR_ARG;
   h->api_seq++;   // ends the enumeration cursor
-  *list = h->lane[0].d_sorted;
+  *list = h->lane[0].d_sorted.p;
   *count = list_of_current(h) ? (int)h->lane[0].list_count : 0;
   return SBG_OK;
 }
@@ -2294,7 +2296,7 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
   int rc;
-  if ((rc = ensure_hits(h, L, std::max(L.hits_cap, h->hits_cap_default))) != SBG_OK) return rc;
+  if ((rc = ensure_hits(h, L, std::max(L.d_hits.cap, h->hits_cap_default))) != SBG_OK) return rc;
   RunCounts rcnt;
   memset(&rcnt, 0, sizeof(rcnt));
   uint64_t total = 0;
@@ -2307,7 +2309,7 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((total + 255) / 256,
       (uint64_t)h->sm_count * 8));
   const cudaError_t e = launch(h, k_merge_runs, grid, 256, 0, L.stream, false, runs,
-      (unsigned long long)stride, rcnt, nruns, L.d_sorted, (unsigned int)SBG_LIST_CAP, L.d_ctl);
+      (unsigned long long)stride, rcnt, nruns, L.d_sorted.p, (unsigned int)SBG_LIST_CAP, L.d_ctl.p);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_merge_runs: %s", cudaGetErrorString(e));
   set_list(h, L, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP), true, h->cur_slot);
   return SBG_OK;
@@ -2319,8 +2321,8 @@ int sbg_set_list7(sbg_handle *h, const uint64_t *list, int count) {
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
   int rc;
-  if ((rc = ensure_hits(h, L, std::max(L.hits_cap, h->hits_cap_default))) != SBG_OK) return rc;
-  if ((size_t)count > L.hits_cap) return fail(h, SBG_ERR_ARG, "list of %d entries too long", count);
+  if ((rc = ensure_hits(h, L, std::max(L.d_hits.cap, h->hits_cap_default))) != SBG_OK) return rc;
+  if ((size_t)count > L.d_hits.cap) return fail(h, SBG_ERR_ARG, "list of %d entries too long", count);
   // the list must be a concatenation of ascending runs (what gathering the parts' ordered lists
   // gives); they are merged on the device
   int counts[kMaxRuns];
@@ -2335,7 +2337,7 @@ int sbg_set_list7(sbg_handle *h, const uint64_t *list, int count) {
     }
   }
   if (count > 0) {
-    SBG_CUDA(h, cudaMemcpyAsync(L.d_hits, list, (size_t)count * sizeof(uint64_t),
+    SBG_CUDA(h, cudaMemcpyAsync(L.d_hits.p, list, (size_t)count * sizeof(uint64_t),
         cudaMemcpyHostToDevice, L.stream));
     h->h2d_bytes += (uint64_t)count * 8;
   }
@@ -2343,19 +2345,19 @@ int sbg_set_list7(sbg_handle *h, const uint64_t *list, int count) {
   uint64_t stride = 0;
   for (int r = 0; r < nruns; r++) stride = std::max<uint64_t>(stride, (uint64_t)counts[r]);
   if (nruns > 1) {
-    if ((uint64_t)nruns * stride > L.hits_cap) {
+    if ((uint64_t)nruns * stride > L.d_hits.cap) {
       return fail(h, SBG_ERR_ARG, "list too long to stage (%d runs of up to %llu)", nruns,
           (unsigned long long)stride);
     }
     uint64_t off = 0;
     for (int r = 0; r < nruns; r++) {
-      SBG_CUDA(h, cudaMemcpyAsync(L.d_aux + (uint64_t)r * stride, L.d_hits + off,
+      SBG_CUDA(h, cudaMemcpyAsync(L.d_aux.p + (uint64_t)r * stride, L.d_hits.p + off,
           (size_t)counts[r] * sizeof(uint64_t), cudaMemcpyDeviceToDevice, L.stream));
       off += (uint64_t)counts[r];
     }
-    return sbg_set_list7_device(h, L.d_aux, stride, counts, nruns);
+    return sbg_set_list7_device(h, L.d_aux.p, stride, counts, nruns);
   }
-  return sbg_set_list7_device(h, L.d_hits, stride, counts, nruns);
+  return sbg_set_list7_device(h, L.d_hits.p, stride, counts, nruns);
 }
 
 int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total) {
@@ -2377,7 +2379,7 @@ int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total) {
     sbg_handle *h = hs[d];
     sbg_lane &L = h->lane[0];
     SBG_CUDA(h, cudaSetDevice(h->device));
-    int rc = ensure_hits(h, L, std::max<size_t>(std::max(L.hits_cap, h->hits_cap_default),
+    int rc = ensure_hits(h, L, std::max<size_t>(std::max(L.d_hits.cap, h->hits_cap_default),
         (size_t)nh * stride));
     if (rc != SBG_OK) return rc;
     for (int s = 0; s < nh; s++) {
@@ -2390,8 +2392,9 @@ int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total) {
           if (e != cudaSuccess) (void)cudaGetLastError();   // already enabled
         }
       }
-      SBG_CUDA(h, cudaMemcpyPeerAsync(L.d_aux + (uint64_t)s * stride, h->device,
-          hs[s]->lane[0].d_sorted, hs[s]->device, (size_t)counts[s] * sizeof(uint64_t), L.stream));
+      SBG_CUDA(h, cudaMemcpyPeerAsync(L.d_aux.p + (uint64_t)s * stride, h->device,
+          hs[s]->lane[0].d_sorted.p, hs[s]->device, (size_t)counts[s] * sizeof(uint64_t),
+          L.stream));
     }
   }
   // 2. only when every copy has landed may a device overwrite its own list with the merged one
@@ -2400,7 +2403,7 @@ int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total) {
     SBG_CUDA(hs[d], cudaStreamSynchronize(hs[d]->lane[0].stream));
   }
   for (int d = 0; d < nh; d++) {
-    int rc = sbg_set_list7_device(hs[d], hs[d]->lane[0].d_aux, stride, counts, nh);
+    int rc = sbg_set_list7_device(hs[d], hs[d]->lane[0].d_aux.p, stride, counts, nh);
     if (rc != SBG_OK) return rc;
   }
   return SBG_OK;
@@ -2428,7 +2431,7 @@ int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_o
   // k_decomp7 takes the list's length from the control words, which k_begin keeps here; but the
   // k_begin of a search_5lut or a 5-LUT enumeration since the list was installed has cleared them
   L.h_ctl->list_count = L.list_count;
-  SBG_CUDA(h, cudaMemcpyAsync(&L.d_ctl->list_count, &L.h_ctl->list_count, sizeof(uint32_t),
+  SBG_CUDA(h, cudaMemcpyAsync(&L.d_ctl.p->list_count, &L.h_ctl->list_count, sizeof(uint32_t),
       cudaMemcpyHostToDevice, L.stream));
   L.seq++;
   CallInputs in;
@@ -2471,7 +2474,7 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
       SBG_CUDA(h, cudaSetDevice(h->device));
       const size_t first = idx > 0 ? idx - 1 : 0;
       uint64_t tmp[2] = {0, 0};
-      SBG_CUDA(h, cudaMemcpyAsync(tmp, L.d_sorted + first, (idx > 0 ? 2 : 1) * sizeof(uint64_t),
+      SBG_CUDA(h, cudaMemcpyAsync(tmp, L.d_sorted.p + first, (idx > 0 ? 2 : 1) * sizeof(uint64_t),
           cudaMemcpyDeviceToHost, L.stream));
       SBG_CUDA(h, cudaStreamSynchronize(L.stream));
       pair[0] = idx > 0 ? tmp[0] : 0;
@@ -2680,18 +2683,19 @@ int sbg_enum_fetch(sbg_handle *h, uint64_t first, uint64_t count, sbg_match *out
   const uint64_t n = std::min(count, c.total - first);
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
-  if ((rc = grow(h, L, L.d_pranks, L.pranks_cap, 2)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_ptickets, L.ptickets_cap, 2)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_ematch, L.ematch_cap, n)) != SBG_OK) return rc;
+  EnumBuffers &E = h->ebuf;
+  if ((rc = E.d_pranks.grow(h, L.stream, 2)) != SBG_OK) return rc;
+  if ((rc = E.d_ptickets.grow(h, L.stream, 2)) != SBG_OK) return rc;
+  if ((rc = E.d_ematch.grow(h, L.stream, n)) != SBG_OK) return rc;
   // global ranks: the share writes the ranks it owns, zero records elsewhere
-  if (c.global) SBG_CUDA(h, cudaMemsetAsync(L.d_ematch, 0, n * sizeof(sbg_match), L.stream));
+  if (c.global) SBG_CUDA(h, cudaMemsetAsync(E.d_ematch.p, 0, n * sizeof(sbg_match), L.stream));
   // the tickets of the window's first and last rank; the launch covers them and those between
   // (global: the range emit skips the tickets whose ranks lie outside the window)
   const unsigned long long ends[2] = {first, first + n - 1};
   unsigned long long tk[2] = {0, 0};
-  SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, ends, sizeof(ends), cudaMemcpyHostToDevice, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(E.d_pranks.p, ends, sizeof(ends), cudaMemcpyHostToDevice, L.stream));
   if ((rc = locate_tickets(h, L, 2)) != SBG_OK) return rc;
-  SBG_CUDA(h, cudaMemcpyAsync(tk, L.d_ptickets, sizeof(tk), cudaMemcpyDeviceToHost, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(tk, E.d_ptickets.p, sizeof(tk), cudaMemcpyDeviceToHost, L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   EnumSel sel;
   memset(&sel, 0, sizeof(sel));
@@ -2733,23 +2737,24 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
   }
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
-  if ((rc = grow(h, L, L.d_pranks, L.pranks_cap, nranks)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_pslots, L.pslots_cap, nranks)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_ptickets, L.ptickets_cap, nranks)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_pfirst, L.pfirst_cap, nranks + 1)) != SBG_OK) return rc;
-  if ((rc = grow(h, L, L.d_ematch, L.ematch_cap, nranks)) != SBG_OK) return rc;
+  EnumBuffers &E = h->ebuf;
+  if ((rc = E.d_pranks.grow(h, L.stream, nranks)) != SBG_OK) return rc;
+  if ((rc = E.d_pslots.grow(h, L.stream, nranks)) != SBG_OK) return rc;
+  if ((rc = E.d_ptickets.grow(h, L.stream, nranks)) != SBG_OK) return rc;
+  if ((rc = E.d_pfirst.grow(h, L.stream, nranks + 1)) != SBG_OK) return rc;
+  if ((rc = E.d_ematch.grow(h, L.stream, nranks)) != SBG_OK) return rc;
   // global ranks: the share writes the ranks it owns, zero records elsewhere
-  if (c.global) SBG_CUDA(h, cudaMemsetAsync(L.d_ematch, 0, nranks * sizeof(sbg_match), L.stream));
+  if (c.global) SBG_CUDA(h, cudaMemsetAsync(E.d_ematch.p, 0, nranks * sizeof(sbg_match), L.stream));
   // a share without tickets (global ranks only) owns no rank
   if (c.tickets == 0) return copy_matches(h, L, out, nranks);
   // device: the ticket of every rank; host: the distinct tickets and their slices of the ranks.
   // Global ranks another share owns are dropped here, so that no warp sweeps a ticket for a rank
   // it never meets.
-  SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, sorted.data(), nranks * sizeof(unsigned long long),
+  SBG_CUDA(h, cudaMemcpyAsync(E.d_pranks.p, sorted.data(), nranks * sizeof(unsigned long long),
       cudaMemcpyHostToDevice, L.stream));
   if ((rc = locate_tickets(h, L, nranks, c.global)) != SBG_OK) return rc;
   std::vector<unsigned long long> tickets(nranks);
-  SBG_CUDA(h, cudaMemcpyAsync(tickets.data(), L.d_ptickets, nranks * sizeof(unsigned long long),
+  SBG_CUDA(h, cudaMemcpyAsync(tickets.data(), E.d_ptickets.p, nranks * sizeof(unsigned long long),
       cudaMemcpyDeviceToHost, L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   std::vector<unsigned int> firsts;
@@ -2766,21 +2771,21 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
   }
   firsts.push_back((unsigned int)m);
   if (m < nranks) {
-    SBG_CUDA(h, cudaMemcpyAsync(L.d_pranks, sorted.data(), m * sizeof(unsigned long long),
+    SBG_CUDA(h, cudaMemcpyAsync(E.d_pranks.p, sorted.data(), m * sizeof(unsigned long long),
         cudaMemcpyHostToDevice, L.stream));
   }
-  SBG_CUDA(h, cudaMemcpyAsync(L.d_ptickets, tickets.data(), d * sizeof(unsigned long long),
+  SBG_CUDA(h, cudaMemcpyAsync(E.d_ptickets.p, tickets.data(), d * sizeof(unsigned long long),
       cudaMemcpyHostToDevice, L.stream));
-  SBG_CUDA(h, cudaMemcpyAsync(L.d_pfirst, firsts.data(), (d + 1) * sizeof(unsigned int),
+  SBG_CUDA(h, cudaMemcpyAsync(E.d_pfirst.p, firsts.data(), (d + 1) * sizeof(unsigned int),
       cudaMemcpyHostToDevice, L.stream));
-  SBG_CUDA(h, cudaMemcpyAsync(L.d_pslots, slots.data(), m * sizeof(unsigned int),
+  SBG_CUDA(h, cudaMemcpyAsync(E.d_pslots.p, slots.data(), m * sizeof(unsigned int),
       cudaMemcpyHostToDevice, L.stream));
   EnumSel sel;
   sel.lo = 0;
-  sel.ranks = L.d_pranks;
-  sel.slots = L.d_pslots;
-  sel.tickets = L.d_ptickets;
-  sel.first = L.d_pfirst;
+  sel.ranks = E.d_pranks.p;
+  sel.slots = E.d_pslots.p;
+  sel.tickets = E.d_ptickets.p;
+  sel.first = E.d_pfirst.p;
   if (d > 0 && (rc = emit_sel<kEnumPick>(h, L, 0, 0, d, sel)) != SBG_OK) return rc;
   return copy_matches(h, L, out, nranks);
 }
@@ -2797,7 +2802,8 @@ int sbg_enum_block_sums(sbg_handle *h, uint64_t *out, uint64_t *nblocks) {
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
   if ((rc = block_sums(h, L, nb)) != SBG_OK) return rc;
-  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_bsums, nb * sizeof(uint64_t), cudaMemcpyDefault, L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(out, h->ebuf.d_bsums.p, nb * sizeof(uint64_t), cudaMemcpyDefault,
+      L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   return SBG_OK;
 }
@@ -2830,25 +2836,26 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
   if (sums == nullptr && widest > 0) return fail(h, SBG_ERR_ARG, "null sums");
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
+  EnumBuffers &E = h->ebuf;
   const unsigned int B = enum_block_size(c.width);
   const uint64_t nb = c.tickets / B;
   uint64_t whole = 0;
   if (c.blocks > 0) {
     // the rows, packed at stride `widest` on the device
-    if ((rc = grow(h, L, L.d_gsums, L.gsums_cap, (uint64_t)nparts * widest)) != SBG_OK) return rc;
+    if ((rc = E.d_gsums.grow(h, L.stream, (uint64_t)nparts * widest)) != SBG_OK) return rc;
     for (int q = 0; q < nparts; q++) {
       if (counts[q] == 0) continue;
-      SBG_CUDA(h, cudaMemcpyAsync(L.d_gsums + (uint64_t)q * widest, sums + (uint64_t)q * stride,
+      SBG_CUDA(h, cudaMemcpyAsync(E.d_gsums.p + (uint64_t)q * widest, sums + (uint64_t)q * stride,
           counts[q] * sizeof(uint64_t), cudaMemcpyDefault, L.stream));
     }
     if (nb > 0 && (rc = block_sums(h, L, nb)) != SBG_OK) return rc;
-    cudaError_t e = launch(h, k_enum_globalize, 1, 1024, 0, L.stream, false, L.d_ectl,
-        (const unsigned long long *)L.d_gsums, (unsigned long long)widest,
-        (unsigned long long)c.blocks, c.part, nparts, (const unsigned long long *)L.d_bsums,
-        (const unsigned long long *)L.d_eoffset, B, L.d_delta);
+    cudaError_t e = launch(h, k_enum_globalize, 1, 1024, 0, L.stream, false, E.d_ectl.p,
+        (const unsigned long long *)E.d_gsums.p, (unsigned long long)widest,
+        (unsigned long long)c.blocks, c.part, nparts, (const unsigned long long *)E.d_bsums.p,
+        (const unsigned long long *)E.d_eoffset.p, B, E.d_delta.p);
     if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_globalize: %s", cudaGetErrorString(e));
     EnumCtl ec;
-    SBG_CUDA(h, cudaMemcpyAsync(&ec, L.d_ectl, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
+    SBG_CUDA(h, cudaMemcpyAsync(&ec, E.d_ectl.p, sizeof(ec), cudaMemcpyDeviceToHost, L.stream));
     SBG_CUDA(h, cudaStreamSynchronize(L.stream));
     if (ec.gbad != 0) {
       return fail(h, SBG_ERR_ARG, "row %d of sums is not this share's block sums (rows gathered "
@@ -2858,8 +2865,8 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
     if (nb > 0) {
       const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((c.tickets + 255) / 256,
           (uint64_t)h->sm_count * 8));
-      e = launch(h, k_enum_rebase, grid, 256, 0, L.stream, false, L.d_eoffset,
-          (unsigned long long)c.tickets, B, (const unsigned long long *)L.d_delta);
+      e = launch(h, k_enum_rebase, grid, 256, 0, L.stream, false, E.d_eoffset.p,
+          (unsigned long long)c.tickets, B, (const unsigned long long *)E.d_delta.p);
       if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_rebase: %s", cudaGetErrorString(e));
       SBG_CUDA(h, cudaStreamSynchronize(L.stream));
     }
@@ -2904,8 +2911,8 @@ int sbg_enum_depth_counts(sbg_handle *h, uint64_t *out, uint32_t nbins) {
   if (nbins == 0) return SBG_OK;
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
-  SBG_CUDA(h, cudaMemcpyAsync(out, L.d_ehist, nbins * sizeof(uint64_t), cudaMemcpyDeviceToHost,
-      L.stream));
+  SBG_CUDA(h, cudaMemcpyAsync(out, h->ebuf.d_ehist.p, nbins * sizeof(uint64_t),
+      cudaMemcpyDeviceToHost, L.stream));
   SBG_CUDA(h, cudaStreamSynchronize(L.stream));
   h->d2h_bytes += nbins * sizeof(uint64_t);
   return SBG_OK;
