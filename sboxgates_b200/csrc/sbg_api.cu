@@ -152,14 +152,17 @@ struct sbg_lane {
   cudaEvent_t ev_begun = nullptr;
   uint64_t seq = 0;
   int slot = -1;                 // problem the lane's chain works on
-  uint32_t list_count = 0;
-  bool list_ready = false;
-  // the problem the list in d_sorted (installed, or a part's from sbg_filter7_part) was built for:
-  // a slot and that slot's version at the time (-1: none)
-  int list_slot = -1;
-  uint64_t list_version = 0;
   bool timed5 = false, timed7 = false;
   float ms[4] = {0, 0, 0, 0};
+};
+
+// The handle's 7-LUT list and what the last sbg_decomp7_part found in it.  Lane 0's d_sorted is the
+// list's storage; the other lanes' d_sorted serve only their own chains in sbg_search_batch.
+struct List7 {
+  uint32_t count = 0;
+  bool whole = false;   // the problem's full list, which phase 2 may use (else one part's)
+  int slot = -1;        // the problem it was built for: a slot and that slot's version (-1: none)
+  uint64_t version = 0;
   uint64_t last_key = SBG_KEY_NONE;   // sbg_decomp7_part's result and the two list entries behind it
   uint64_t last_tuple = 0, last_tuple_prev = 0;
 };
@@ -234,6 +237,7 @@ struct sbg_handle {
   DevArray<DevTables> d_tab;     // lane-indexed ordering tables
   DevArray<uint32_t> d_scratch;  // sbg_alu_peak
   EnumBuffers ebuf;
+  List7 list7;
 
   // host copies of the staged problems (for sbg_finish*)
   struct HostProblem {
@@ -1245,25 +1249,25 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
   return SBG_OK;
 }
 
-// Every install or drop of a lane's 7-LUT list goes through here.  The key and list entries the last
-// sbg_decomp7_part left behind belong to the list it searched, so any change of the list forgets them
-// (sbg_finish7 would otherwise decode an equal key of the new list with the old list's entries).
-// `slot`: the list in d_sorted was built for that slot's problem as it is staged now (-1: for none).
-void set_list(sbg_handle *h, sbg_lane &L, uint32_t count, bool ready, int slot = -1) {
-  L.list_count = count;
-  L.list_ready = ready;
-  L.last_key = SBG_KEY_NONE;
-  L.list_slot = slot;
-  L.list_version = slot >= 0 ? h->slots[slot].version : 0;
+// What lane 0's d_sorted now holds: the whole list of `slot`'s problem as it is staged now, one
+// part's list of it (sbg_filter7_part with nparts > 1), or no list.  Each replaces the whole record:
+// the key and list entries the last sbg_decomp7_part left behind belong to the list it searched
+// (sbg_finish7 would otherwise decode an equal key of a new list with the old list's entries).
+void install_list(sbg_handle *h, int slot, uint32_t count) {
+  h->list7 = {count, true, slot, h->slots[slot].version};
 }
+void record_part_list(sbg_handle *h, int slot, uint32_t count) {
+  h->list7 = {count, false, slot, h->slots[slot].version};
+}
+void drop_list(sbg_handle *h) { h->list7 = {}; }
 
-// Whether lane 0's list (installed, or a part's) belongs to the current problem as staged now.  A
-// batch leaves on lane 0 the list of its last wave's first job, whatever slot that job searched, and
-// restaging a slot changes its problem under the list; the list's consumers check this.
-bool list_of_current(const sbg_handle *h) {
-  const sbg_lane &L = h->lane[0];
-  return h->problem_ready && L.list_slot == h->cur_slot
-      && L.list_version == h->slots[h->cur_slot].version;
+// Whether the handle's list belongs to the current problem as it is staged now, and is whole unless
+// part_ok.  A batch leaves on lane 0 the list of its last wave's first job, whatever slot that job
+// searched, and restaging a slot changes its problem under the list; the list's consumers check this.
+bool list_is_current(const sbg_handle *h, bool part_ok) {
+  const List7 &l = h->list7;
+  return (l.whole || part_ok) && h->problem_ready && l.slot == h->cur_slot
+      && l.version == h->slots[h->cur_slot].version;
 }
 
 int check_job(sbg_handle *h, const sbg_job *job) {
@@ -1318,7 +1322,7 @@ int redo_search7_steps(sbg_handle *h, sbg_lane &L, const uint8_t *outer, const u
   int rc;
   uint32_t keep = 0;
   if ((rc = run_filter7(h, L, 0, 1, &keep, hit_buffer_overflowed)) != SBG_OK) return rc;
-  set_list(h, L, keep, true, L.slot);
+  if (&L == &h->lane[0]) install_list(h, L.slot, keep);
   L.seq++;
   CallInputs in;
   in.outer = outer;
@@ -1380,7 +1384,7 @@ int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, sbg_node_resul
           o->overflow[2] == 1)) != SBG_OK) return rc;
       swept7 = h->swept;
     }
-    set_list(h, L, (uint32_t)o->feasible[2], true, L.slot);
+    if (&L == &h->lane[0]) install_list(h, L.slot, (uint32_t)o->feasible[2]);
     if ((rc = finish7_slot(h, hp, o->key[2], job->outer7, job->middle7, o->tuple, o->tuple_prev,
         o->feasible[2], swept7, &res->r7)) != SBG_OK) return rc;
     if (res->r7.found) res->found_stage = 7;
@@ -1529,7 +1533,7 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
             flt);
       } else {
         return run(k_enum7<NW, MODE, FORM>, decomp_smem<NW>(n), prob, E.d_ectl.p, in.ord,
-            L.d_sorted.p, L.list_count, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b,
+            L.d_sorted.p, h->list7.count, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b,
             part, nparts, h->d_tab.p, flt);
       }
     });
@@ -1567,10 +1571,10 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   EnumBuffers &E = h->ebuf;
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
-  if (WIDTH == 7 && !(L.list_ready && list_of_current(h))) {
+  if (WIDTH == 7 && !list_is_current(h, false)) {
     uint32_t count = 0;
     if ((rc = run_filter7(h, L, 0, 1, &count)) != SBG_OK) return rc;
-    set_list(h, L, count, true, L.slot);
+    install_list(h, L.slot, count);
   } else {
     L.seq++;
     if ((rc = enqueue_begin(h, L, flags, begin_in, 0)) != SBG_OK) return rc;
@@ -1578,7 +1582,8 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   // this part's tickets: its deal blocks (the last one may be cut short)
   const int n = h->slots[L.slot].n;
   const uint64_t B = enum_block_size(WIDTH);
-  const uint64_t items = WIDTH == 3 ? h_binom[n][2] : WIDTH == 5 ? h_binom[n - 2][3] : L.list_count;
+  const uint64_t items = WIDTH == 3 ? h_binom[n][2] : WIDTH == 5 ? h_binom[n - 2][3]
+      : h->list7.count;
   const uint64_t blocks = (items + B - 1) / B;
   const uint64_t tickets = deal_share(blocks, part, nparts) * B;
   if ((rc = E.d_ectl.grow(h, L.stream, 1)) != SBG_OK) return rc;
@@ -1629,14 +1634,14 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
     c.in = in;
     c.tickets = tickets;
     c.total = ec.carry;
-    c.list_count = L.list_count;
+    c.list_count = h->list7.count;
     c.blocks = blocks;
     c.global = false;
   }
   if (total != nullptr) *total = ec.carry;
   if (feasible != nullptr) {
     // width 3: every feasible triple is a match (the filtered form counts them apart)
-    *feasible = WIDTH == 7 ? (uint64_t)L.list_count
+    *feasible = WIDTH == 7 ? (uint64_t)h->list7.count
         : WIDTH == 3 && in.form == kFormPlain ? ec.total : ec.feasible;
   }
   return SBG_OK;
@@ -1728,9 +1733,8 @@ int check_cursor(sbg_handle *h) {
     return fail(h, SBG_ERR_STATE, "no enumeration cursor: fetch and pick follow a counted "
         "sbg_enum3 / sbg_enum5 / sbg_enum7 call with nothing in between");
   }
-  const sbg_lane &L = h->lane[0];
-  if (L.slot != c.slot || h->ebuf.d_ecount.cap < c.tickets
-      || (c.width == 7 && L.list_count != c.list_count)) {
+  if (h->lane[0].slot != c.slot || h->ebuf.d_ecount.cap < c.tickets
+      || (c.width == 7 && h->list7.count != c.list_count)) {
     return fail(h, SBG_ERR_STATE, "internal: enumeration cursor out of step with its buffers");
   }
   return SBG_OK;
@@ -2175,7 +2179,7 @@ int sbg_use_problem(sbg_handle *h, int slot) {
   if (!h->slots[slot].ready) return fail(h, SBG_ERR_STATE, "slot %d holds no problem", slot);
   h->cur_slot = slot;
   h->problem_ready = true;
-  set_list(h, h->lane[0], 0, false);
+  drop_list(h);
   return SBG_OK;
 }
 
@@ -2264,7 +2268,7 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
   uint32_t keep = 0;
-  set_list(h, L, L.list_count, false);
+  drop_list(h);
   if ((rc = run_filter7(h, L, part, nparts, &keep)) != SBG_OK) return rc;
   for (int i = 0; i < 4; i++) h->last_ms[i] = L.ms[i];
   *count = (int)keep;
@@ -2276,7 +2280,11 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   }
   // The part's own ordered list stays on the device; when it is the whole space (nparts == 1) it
   // IS the list, and phase 2 may follow without sbg_set_list7().
-  set_list(h, L, keep, nparts == 1, h->cur_slot);
+  if (nparts == 1) {
+    install_list(h, h->cur_slot, keep);
+  } else {
+    record_part_list(h, h->cur_slot, keep);
+  }
   return SBG_OK;
 }
 
@@ -2284,7 +2292,7 @@ int sbg_list7_device(sbg_handle *h, const uint64_t **list, int *count) {
   if (h == nullptr || list == nullptr || count == nullptr) return SBG_ERR_ARG;
   h->api_seq++;   // ends the enumeration cursor
   *list = h->lane[0].d_sorted.p;
-  *count = list_of_current(h) ? (int)h->lane[0].list_count : 0;
+  *count = list_is_current(h, true) ? (int)h->list7.count : 0;
   return SBG_OK;
 }
 
@@ -2311,7 +2319,7 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
   const cudaError_t e = launch(h, k_merge_runs, grid, 256, 0, L.stream, false, runs,
       (unsigned long long)stride, rcnt, nruns, L.d_sorted.p, (unsigned int)SBG_LIST_CAP, L.d_ctl.p);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_merge_runs: %s", cudaGetErrorString(e));
-  set_list(h, L, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP), true, h->cur_slot);
+  install_list(h, h->cur_slot, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP));
   return SBG_OK;
 }
 
@@ -2368,7 +2376,7 @@ int sbg_allgather_merge7(sbg_handle *const *hs, int nh, int *total) {
   for (int i = 0; i < nh; i++) {
     if (hs[i] == nullptr) return SBG_ERR_ARG;
     hs[i]->api_seq++;   // ends the enumeration cursor
-    counts[i] = (int)hs[i]->lane[0].list_count;
+    counts[i] = (int)hs[i]->list7.count;
     stride = std::max<uint64_t>(stride, (uint64_t)counts[i]);
     *total += counts[i];
   }
@@ -2415,7 +2423,8 @@ int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_o
   h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   sbg_lane &L = h->lane[0];
-  if (!L.list_ready || !list_of_current(h)) {
+  List7 &list = h->list7;
+  if (!list_is_current(h, false)) {
     return fail(h, SBG_ERR_STATE, "no 7-LUT list installed for the current problem");
   }
   if (nparts < 1 || part < 0 || part >= nparts) return fail(h, SBG_ERR_ARG, "bad part %d/%d", part, nparts);
@@ -2426,11 +2435,11 @@ int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_o
   int rc;
   *key = SBG_KEY_NONE;
   h->last_ms[3] = 0.f;
-  if (L.list_count == 0) return SBG_OK;
+  if (list.count == 0) return SBG_OK;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
   // k_decomp7 takes the list's length from the control words, which k_begin keeps here; but the
   // k_begin of a search_5lut or a 5-LUT enumeration since the list was installed has cleared them
-  L.h_ctl->list_count = L.list_count;
+  L.h_ctl->list_count = list.count;
   SBG_CUDA(h, cudaMemcpyAsync(&L.d_ctl.p->list_count, &L.h_ctl->list_count, sizeof(uint32_t),
       cudaMemcpyHostToDevice, L.stream));
   L.seq++;
@@ -2439,16 +2448,16 @@ int sbg_decomp7_part(sbg_handle *h, int part, int nparts, const uint8_t *outer_o
   in.middle = middle_order;
   if ((rc = enqueue_begin(h, L, kBeginSearch7 | kBeginKeepCtl, in, 0)) != SBG_OK) return rc;
   if (h->timing) cudaEventRecord(L.ev[2], L.stream);
-  if ((rc = enqueue_decomp7(h, L, part, nparts, (L.list_count + nparts - 1) / nparts)) != SBG_OK) {
+  if ((rc = enqueue_decomp7(h, L, part, nparts, (list.count + nparts - 1) / nparts)) != SBG_OK) {
     return rc;
   }
   if ((rc = wait_stage(h, L, 2)) != SBG_OK) return rc;
   if (h->timing) h->last_ms[3] = L.ms[3] = elapsed(L.ev[2], L.ev[3]);
   h->d2h_bytes += 64;
   *key = L.h_out->key[2];
-  L.last_tuple = L.h_out->tuple;
-  L.last_tuple_prev = L.h_out->tuple_prev;
-  L.last_key = *key;
+  list.last_tuple = L.h_out->tuple;
+  list.last_tuple_prev = L.h_out->tuple_prev;
+  list.last_key = *key;
   return SBG_OK;
 }
 
@@ -2460,16 +2469,16 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
   h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
   sbg_lane &L = h->lane[0];
-  if (!L.list_ready || !list_of_current(h)) {
+  if (!list_is_current(h, false)) {
     return fail(h, SBG_ERR_STATE, "no 7-LUT list installed for the current problem");
   }
   uint64_t pair[2] = {0, 0};
   if (key != SBG_KEY_NONE) {
     const uint64_t idx = key >> 23;
-    if (idx >= L.list_count) return fail(h, SBG_ERR_STATE, "corrupt 7-LUT key");
-    if (key == L.last_key) {   // this device found it: the tuples came with the result
-      pair[0] = L.last_tuple_prev;
-      pair[1] = L.last_tuple;
+    if (idx >= h->list7.count) return fail(h, SBG_ERR_STATE, "corrupt 7-LUT key");
+    if (key == h->list7.last_key) {   // this device found it: the tuples came with the result
+      pair[0] = h->list7.last_tuple_prev;
+      pair[1] = h->list7.last_tuple;
     } else {                   // another part's key: read the two list entries
       SBG_CUDA(h, cudaSetDevice(h->device));
       const size_t first = idx > 0 ? idx - 1 : 0;
@@ -2481,7 +2490,7 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
       pair[1] = idx > 0 ? tmp[1] : tmp[0];
     }
   }
-  return finish7_slot(h, cur(h), key, outer_order, middle_order, pair[1], pair[0], L.list_count,
+  return finish7_slot(h, cur(h), key, outer_order, middle_order, pair[1], pair[0], h->list7.count,
       h->swept, res);
 }
 
@@ -2503,7 +2512,7 @@ int sbg_search_node(sbg_handle *h, const sbg_job *job, sbg_node_result *res) {
   in.outer = job->outer7;
   in.middle = job->middle7;
   in.gate_order = job->gate_order;
-  set_list(h, L, L.list_count, false);
+  drop_list(h);
   if ((rc = enqueue_chain(h, L, job->flags, in)) != SBG_OK) return rc;
   const double t1 = wall_now();
   if ((rc = collect_chain(h, L, job, res)) != SBG_OK) return rc;
@@ -2560,7 +2569,7 @@ int sbg_search_batch(sbg_handle *h, int njobs, const sbg_job *jobs, sbg_node_res
       in.outer = job.outer7;
       in.middle = job.middle7;
       in.gate_order = job.gate_order;
-      set_list(h, L, L.list_count, false);
+      if (k == 0) drop_list(h);
       rc = enqueue_chain(h, L, job.flags, in);
       L.mark_begun = false;
       if (rc != SBG_OK) {
