@@ -72,7 +72,18 @@ typedef struct {
   uint64_t index;          /* 5-LUT: lexicographic rank of the combination; 7-LUT: list index */
   uint64_t key;            /* the packed minimum key (SBG_KEY_NONE if nothing matched) */
   uint64_t tuples_feasible;/* 5-LUT: feasible combinations met; 7-LUT: length of the hit list */
-  uint64_t tuples_swept;   /* combinations put through the feasibility test by this device */
+  uint64_t tuples_swept;   /* combinations put through the feasibility test by this device,
+                              inbits rejections included: this part's share in a sharded search
+                              (summed over the parts, the whole's).  5-LUT: C(n,5) on a miss, at
+                              least index + 1 on a hit (a match stops the sweep).  7-LUT: the phase-1
+                              sweep behind the installed list, C(n,7) for an uncapped list; one that
+                              reached SBG_LIST_CAP stops between the reference's count (the last
+                              entry's rank + 1) and C(n,7).  sbg_finish5 reports the last
+                              sbg_search5_part's; sbg_finish7 the installed list's: that of the
+                              sbg_filter7_part, sbg_search7 / node / batch or sbg_enum7 phase 1 that
+                              built it, carried over by sbg_set_list7, sbg_set_list7_device and
+                              sbg_allgather_merge7 from this handle's own list of the current
+                              problem (0 where the handle held none) */
 } sbg_result;
 
 /* ---- lifecycle ------------------------------------------------------------------------------ */

@@ -151,6 +151,9 @@ struct sbg_lane {
   bool mark_begun = false;
   cudaEvent_t ev_begun = nullptr;
   uint64_t seq = 0;
+  // what the host adds to the sweep counters of the lane's last search_5lut / phase-1 launch (see
+  // head_skipped)
+  uint64_t skipped5 = 0, skipped7 = 0;
   int slot = -1;                 // problem the lane's chain works on
   bool timed5 = false, timed7 = false;
   float ms[4] = {0, 0, 0, 0};
@@ -163,6 +166,7 @@ struct List7 {
   bool whole = false;   // the problem's full list, which phase 2 may use (else one part's)
   int slot = -1;        // the problem it was built for: a slot and that slot's version (-1: none)
   uint64_t version = 0;
+  uint64_t swept = 0;   // this device's phase-1 sweep behind the list (sbg_finish7's tuples_swept)
   uint64_t last_key = SBG_KEY_NONE;   // sbg_decomp7_part's result and the two list entries behind it
   uint64_t last_tuple = 0, last_tuple_prev = 0;
 };
@@ -263,8 +267,8 @@ struct sbg_handle {
   int cur_slot = 0;
   bool problem_ready = false;
 
-  uint64_t swept = 0;
-  uint64_t feasible = 0;
+  uint64_t swept5 = 0;      // the last sbg_search5_part's work counters, read by sbg_finish5
+  uint64_t feasible5 = 0;
   std::map<std::pair<const void *, size_t>, int> occupancy;  // grid_for's cache
   std::map<const void *, size_t> smem_attr;                  // largest dynamic smem opted into
   // Kernel-form switches, read from the environment when the handle is created.  Each forces one
@@ -546,6 +550,59 @@ ChunkPlan plan_chunks_mode(int n, uint32_t inmask, int mode, uint64_t waves, uin
   return pl;
 }
 
+// The combinations of the P-gate prefixes in front of the first prefix the prefix tickets take
+// (all prefixes when the chunk tickets cover everything) that hold an excluded gate.  The chunk
+// tickets walk the allowed gates only, so no ticket meets these prefixes and no kernel credits
+// them; the reference steps through them one by one (lut.c:174-187, 294-305), so the host adds them
+// to the sweep of part 0.  Each prefix weighs the C(n-1-last, K-P) combinations that complete it.
+template <int P, int K>
+uint64_t head_skipped(int n, uint32_t inmask, const ChunkPlan &pl) {
+  inmask &= 0xffu;
+  if (pl.items == 0 || inmask == 0) return 0;
+  const int nr = n - (K - P);   // prefix gates are < nr
+  const uint64_t end = h_binom[nr][P];
+  const uint64_t t_end = pl.all ? end : pl.t_offset;
+  // the prefix at rank t_end (the first one left to the prefix tickets: made of allowed gates)
+  int t[P];
+  if (t_end < end) {
+    uint64_t r = t_end;
+    int x = 0;
+    for (int pos = 0; pos < P; pos++) {
+      for (;; x++) {
+        const uint64_t cnt = h_binom[nr - x - 1][P - pos - 1];
+        if (r < cnt) break;
+        r -= cnt;
+      }
+      t[pos] = x++;
+    }
+  }
+  // weight of the prefixes below t_end, over all gates (excl = 0) or over the allowed ones:
+  // f[r][v] = the weight of the r more gates above v (gates above v allowed), summed
+  auto below = [&](uint32_t excl) {
+    static thread_local uint64_t f[P][SBG_MAX_GATES + 1];
+    for (int v = nr - 1; v >= 0; v--) f[0][v] = h_binom[n - 1 - v][K - P];
+    for (int r = 1; r < P; r++) {
+      uint64_t acc = 0;
+      for (int v = nr - 1; v >= 0; v--) {
+        f[r][v] = acc;
+        if (!(v < 8 && ((excl >> v) & 1u))) acc += f[r - 1][v];
+      }
+    }
+    uint64_t w = 0;
+    int lo = 0;
+    for (int pos = 0; pos < P; pos++) {
+      const int hi = t_end < end ? t[pos] : nr;
+      for (int u = lo; u < hi; u++) {
+        if (!(u < 8 && ((excl >> u) & 1u))) w += f[P - 1 - pos][u];
+      }
+      if (t_end >= end) break;
+      lo = t[pos] + 1;
+    }
+    return w;
+  };
+  return below(0) - below(inmask);
+}
+
 sbg_handle::HostProblem &cur(sbg_handle *h) { return h->slots[h->cur_slot]; }
 
 // ---- lane resources (allocated on first need: most graphs never run a large 7-LUT search) ------
@@ -688,6 +745,7 @@ int enqueue_search5(sbg_handle *h, sbg_lane &L, int part, int nparts, bool two, 
   if (!two && head && h->opt_head != 0 && n >= kHeadAlwaysMinGates) {
     pl = plan_chunks_mode<P, P + 2>(n, hp.inmask, 1, kHeadWaves5, h_binom[n - 3][2]);
   }
+  L.skipped5 = part == 0 ? head_skipped<P, P + 2>(n, hp.inmask, pl) : 0;
   const uint64_t tickets = pl.all ? 0 : (total - pl.t_offset + nparts - 1) / nparts;
   const uint64_t chunk_tickets = (pl.items + kDeal * nparts - 1) / (kDeal * nparts) * kDeal;
   if (h->timing) cudaEventRecord(L.ev[6], L.stream);
@@ -896,6 +954,9 @@ int launch_filter7_pm_p(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int pa
 int enqueue_filter7(sbg_handle *h, sbg_lane &L, const FilterPlan &fp, int part, int nparts,
     bool build_sieve3) {
   int rc;
+  const sbg_handle::HostProblem &hp = h->slots[L.slot];
+  L.skipped7 = part != 0 ? 0 : fp.five ? head_skipped<5, 7>(hp.n, hp.inmask, fp.pl)
+                                       : head_skipped<4, 7>(hp.n, hp.inmask, fp.pl);
   if (h->timing) cudaEventRecord(L.ev[0], L.stream);
   const unsigned long long room = (unsigned long long)SBG_LIST_CAP - fp.list_base;
   rc = fp.five ? launch_filter7_pm_p<5>(h, L, fp, part, nparts, room, build_sieve3)
@@ -968,9 +1029,10 @@ bool valid_order(const uint8_t *order) {
 // Runs phase 1 of this part to completion on lane L and leaves the ordered list (<= SBG_LIST_CAP)
 // in L.d_sorted, its length in *count_out.  Handles the hit buffer overflowing (grow once, then the
 // bounded-parallelism retry) and sweeps with more tickets than the ticket table holds (several
-// launches, each appending to the list: later tickets only hold larger tuples).
+// launches, each appending to the list: later tickets only hold larger tuples).  *swept_out = the
+// combinations the part's sweep put through the feasibility test, summed over the segments.
 int run_filter7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint32_t *count_out,
-    bool overflowed_already = false) {
+    uint64_t *swept_out, bool overflowed_already = false) {
   sbg_handle::HostProblem &hp = h->slots[L.slot];
   int rc;
   bool retry = false;
@@ -1027,7 +1089,7 @@ int run_filter7(sbg_handle *h, sbg_lane &L, int part, int nparts, uint32_t *coun
     L.ms[2] = ms_order;
     L.ms[3] = 0.f;
   }
-  h->swept = swept;
+  *swept_out = swept + L.skipped7;
   *count_out = list_base;
   return SBG_OK;
 }
@@ -1210,6 +1272,7 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
   sbg_handle::HostProblem &hp = h->slots[L.slot];
   int rc;
   L.seq++;
+  L.skipped5 = L.skipped7 = 0;
   uint32_t flags = 0;
   if ((what & kDoScan3) && hp.n >= 3) flags |= kBeginScan3;
   if ((what & kDoSearch5) && hp.n >= 5) flags |= kBeginSearch5;
@@ -1253,11 +1316,12 @@ int enqueue_chain(sbg_handle *h, sbg_lane &L, int what, const CallInputs &in) {
 // part's list of it (sbg_filter7_part with nparts > 1), or no list.  Each replaces the whole record:
 // the key and list entries the last sbg_decomp7_part left behind belong to the list it searched
 // (sbg_finish7 would otherwise decode an equal key of a new list with the old list's entries).
-void install_list(sbg_handle *h, int slot, uint32_t count) {
-  h->list7 = {count, true, slot, h->slots[slot].version};
+// `swept` is this device's phase-1 sweep behind the list, which sbg_finish7 reports.
+void install_list(sbg_handle *h, int slot, uint32_t count, uint64_t swept) {
+  h->list7 = {count, true, slot, h->slots[slot].version, swept};
 }
-void record_part_list(sbg_handle *h, int slot, uint32_t count) {
-  h->list7 = {count, false, slot, h->slots[slot].version};
+void record_part_list(sbg_handle *h, int slot, uint32_t count, uint64_t swept) {
+  h->list7 = {count, false, slot, h->slots[slot].version, swept};
 }
 void drop_list(sbg_handle *h) { h->list7 = {}; }
 
@@ -1317,12 +1381,13 @@ int redo_search5_fused(sbg_handle *h, sbg_lane &L, const uint8_t *order5) {
 }
 
 // search_7lut of the lane's problem through the step-by-step path (overflow handling, segments).
+// *swept = its phase-1 sweep.
 int redo_search7_steps(sbg_handle *h, sbg_lane &L, const uint8_t *outer, const uint8_t *middle,
-    bool hit_buffer_overflowed) {
+    bool hit_buffer_overflowed, uint64_t *swept) {
   int rc;
   uint32_t keep = 0;
-  if ((rc = run_filter7(h, L, 0, 1, &keep, hit_buffer_overflowed)) != SBG_OK) return rc;
-  if (&L == &h->lane[0]) install_list(h, L.slot, keep);
+  if ((rc = run_filter7(h, L, 0, 1, &keep, swept, hit_buffer_overflowed)) != SBG_OK) return rc;
+  if (&L == &h->lane[0]) install_list(h, L.slot, keep, *swept);
   L.seq++;
   CallInputs in;
   in.outer = outer;
@@ -1342,6 +1407,7 @@ int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, sbg_node_resul
   const HostOut *o = L.h_out;
   int rc;
   bool redone7 = false;
+  uint64_t swept7 = 0;   // the redone phase 1's sweep
   memset(res, 0, sizeof(*res));
   res->key3 = SBG_KEY_NONE;
   res->r5.key = SBG_KEY_NONE;
@@ -1363,28 +1429,30 @@ int collect_chain(sbg_handle *h, sbg_lane &L, const sbg_job *job, sbg_node_resul
       if ((rc = redo_search5_fused(h, L, job->order5)) != SBG_OK) return rc;
       redone = true;
     }
-    if ((rc = finish5_slot(h, hp, o->key[1], job->order5, o->feasible[1], o->swept[1],
-        &res->r5)) != SBG_OK) return rc;
+    if ((rc = finish5_slot(h, hp, o->key[1], job->order5, o->feasible[1],
+        o->swept[1] + L.skipped5, &res->r5)) != SBG_OK) return rc;
     if (res->r5.found) {
       res->found_stage = 5;
       return SBG_OK;
     }
     if (redone && (job->flags & kDoSearch7) && hp.n >= 7) {
       // the chain's 7-LUT stage was cancelled together with the incomplete 5-LUT stage
-      if ((rc = redo_search7_steps(h, L, job->outer7, job->middle7, false)) != SBG_OK) return rc;
+      if ((rc = redo_search7_steps(h, L, job->outer7, job->middle7, false, &swept7)) != SBG_OK) {
+        return rc;
+      }
       redone7 = true;
     }
   }
   if ((job->flags & kDoSearch7) && hp.n >= 7) {
     if ((rc = wait_stage(h, L, 2)) != SBG_OK) return rc;
     h->d2h_bytes += 64;
-    uint64_t swept7 = o->swept[2];
     if (o->overflow[2] != 0 || redone7) {
       if (!redone7 && (rc = redo_search7_steps(h, L, job->outer7, job->middle7,
-          o->overflow[2] == 1)) != SBG_OK) return rc;
-      swept7 = h->swept;
+          o->overflow[2] == 1, &swept7)) != SBG_OK) return rc;
+    } else {
+      swept7 = o->swept[2] + L.skipped7;
     }
-    if (&L == &h->lane[0]) install_list(h, L.slot, (uint32_t)o->feasible[2]);
+    if (&L == &h->lane[0]) install_list(h, L.slot, (uint32_t)o->feasible[2], swept7);
     if ((rc = finish7_slot(h, hp, o->key[2], job->outer7, job->middle7, o->tuple, o->tuple_prev,
         o->feasible[2], swept7, &res->r7)) != SBG_OK) return rc;
     if (res->r7.found) res->found_stage = 7;
@@ -1573,8 +1641,9 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
   if (WIDTH == 7 && !list_is_current(h, false)) {
     uint32_t count = 0;
-    if ((rc = run_filter7(h, L, 0, 1, &count)) != SBG_OK) return rc;
-    install_list(h, L.slot, count);
+    uint64_t swept = 0;
+    if ((rc = run_filter7(h, L, 0, 1, &count, &swept)) != SBG_OK) return rc;
+    install_list(h, L.slot, count, swept);
   } else {
     L.seq++;
     if ((rc = enqueue_begin(h, L, flags, begin_in, 0)) != SBG_OK) return rc;
@@ -2237,8 +2306,8 @@ int sbg_search5_part(sbg_handle *h, int part, int nparts, const uint8_t *func_or
   collect_times(h, L);
   h->last_ms[0] = L.ms[0];
   h->d2h_bytes += 48;
-  h->swept = L.h_out->swept[1];
-  h->feasible = L.h_out->feasible[1];
+  h->swept5 = L.h_out->swept[1] + L.skipped5;
+  h->feasible5 = L.h_out->feasible[1];
   *key = L.h_out->key[1];
   return SBG_OK;
 }
@@ -2247,7 +2316,7 @@ int sbg_finish5(sbg_handle *h, uint64_t key, const uint8_t *func_order, sbg_resu
   if (h == nullptr || res == nullptr || func_order == nullptr) return SBG_ERR_ARG;
   h->api_seq++;   // ends the enumeration cursor
   if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
-  return finish5_slot(h, cur(h), key, func_order, h->feasible, h->swept, res);
+  return finish5_slot(h, cur(h), key, func_order, h->feasible5, h->swept5, res);
 }
 
 int sbg_search5(sbg_handle *h, const uint8_t *func_order, sbg_result *res) {
@@ -2268,8 +2337,9 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
   uint32_t keep = 0;
+  uint64_t swept = 0;
   drop_list(h);
-  if ((rc = run_filter7(h, L, part, nparts, &keep)) != SBG_OK) return rc;
+  if ((rc = run_filter7(h, L, part, nparts, &keep, &swept)) != SBG_OK) return rc;
   for (int i = 0; i < 4; i++) h->last_ms[i] = L.ms[i];
   *count = (int)keep;
   if (list != nullptr && keep > 0) {
@@ -2281,9 +2351,9 @@ int sbg_filter7_part(sbg_handle *h, int part, int nparts, uint64_t *list, int *c
   // The part's own ordered list stays on the device; when it is the whole space (nparts == 1) it
   // IS the list, and phase 2 may follow without sbg_set_list7().
   if (nparts == 1) {
-    install_list(h, h->cur_slot, keep);
+    install_list(h, h->cur_slot, keep, swept);
   } else {
-    record_part_list(h, h->cur_slot, keep);
+    record_part_list(h, h->cur_slot, keep, swept);
   }
   return SBG_OK;
 }
@@ -2314,12 +2384,15 @@ int sbg_set_list7_device(sbg_handle *h, const uint64_t *runs, uint64_t stride, c
     total += (uint64_t)counts[r];
   }
   if (total > 0 && runs == nullptr) return SBG_ERR_ARG;
+  // the merged list's sweep on this device: the part's that this handle's own phase 1 left for the
+  // current problem (what an all-gather of the parts' lists follows), else none
+  const uint64_t swept = list_is_current(h, true) ? h->list7.swept : 0;
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((total + 255) / 256,
       (uint64_t)h->sm_count * 8));
   const cudaError_t e = launch(h, k_merge_runs, grid, 256, 0, L.stream, false, runs,
       (unsigned long long)stride, rcnt, nruns, L.d_sorted.p, (unsigned int)SBG_LIST_CAP, L.d_ctl.p);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_merge_runs: %s", cudaGetErrorString(e));
-  install_list(h, h->cur_slot, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP));
+  install_list(h, h->cur_slot, (uint32_t)std::min<uint64_t>(total, SBG_LIST_CAP), swept);
   return SBG_OK;
 }
 
@@ -2491,7 +2564,7 @@ int sbg_finish7(sbg_handle *h, uint64_t key, const uint8_t *outer_order,
     }
   }
   return finish7_slot(h, cur(h), key, outer_order, middle_order, pair[1], pair[0], h->list7.count,
-      h->swept, res);
+      h->list7.swept, res);
 }
 
 // ---- one call per node / per batch of nodes -----------------------------------------------------
@@ -2524,7 +2597,6 @@ int sbg_search_node(sbg_handle *h, const sbg_job *job, sbg_node_result *res) {
     collect_times(h, L);
     for (int i = 0; i < 4; i++) h->last_ms[i] = L.ms[i];
   }
-  h->swept = res->r7.tuples_swept;
   return SBG_OK;
 }
 

@@ -107,13 +107,16 @@ class Model:
     slots: slot -> pool index of the staged state; version: slot -> changes staged so far (an
     identical restage is no change); cur: the current slot (None: no problem); lst: (slot, version,
     what) of lane 0's list, what = ("whole",) for the phase-1 list or ("part", p, k) for a part's
-    list of sbg_filter7_part(p, k > 1), or None.  changed / rows: a slot's change not yet applied
-    on the device (a lazy load) / its position-major rows built."""
+    list of sbg_filter7_part(p, k > 1), or None.  lst_parts: the parts of the phase 1 behind the
+    whole list (1, or k for sbg_filter7_part(p, k) of every part merged by sbg_set_list7*, whose
+    sweep is part k-1's).  changed / rows: a slot's change not yet applied on the device (a lazy
+    load) / its position-major rows built."""
 
     def __init__(self, pool):
         self.pool = pool
         self.slots, self.version = {}, {}
         self.cur, self.lst = None, None
+        self.lst_parts = 1
         self.changed, self.rows = {}, {}
         self.filter_n = None
 
@@ -142,8 +145,9 @@ class Model:
         if rows:
             self.rows[slot] = True
 
-    def _whole(self, slot):
+    def _whole(self, slot, parts=1):
         self.lst = (slot, self.version[slot], ("whole",))
+        self.lst_parts = parts
 
     def apply(self, op, stages=None):
         """Advances the model by one operation that succeeded.  stages: the found_stage of each job
@@ -179,7 +183,7 @@ class Model:
                     self._whole(slot)
         elif kind == "filter":
             self._begin(self.cur, True)
-            self._whole(self.cur)
+            self._whole(self.cur, op[1])
         elif kind == "enum" and op[1] == 7:
             if self.list_of_current() != ("whole",):
                 self._begin(self.cur, True)

@@ -290,12 +290,14 @@ def _free_port():
     return port
 
 
-def _spawn(world, backend):
+def _spawn(world, backend, worker=_dist_worker):
+    """Runs worker(rank, world, port, backend, queue) in `world` processes; returns what each put
+    on the queue."""
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()
-    procs = [ctx.Process(target=_dist_worker, args=(r, world, port, backend, q))
+    procs = [ctx.Process(target=worker, args=(r, world, port, backend, q))
              for r in range(world)]
     for p in procs:
         p.start()

@@ -32,9 +32,6 @@ NONE = E.NONE
 SCAN3, SEARCH5, SEARCH7 = H.SCAN3, H.SEARCH5, H.SEARCH7
 FULL = np.full(4, np.uint64(2**64 - 1), dtype=np.uint64)
 FUNCS = [0x96, 0xE8, 0xCA, 0xD8, 0x1B, 0x6A, 0xB4, 0x78, 0x3C, 0xA6]
-# sbg_finish7's tuples_swept is the handle's last phase-1 sweep, whichever call ran it (a standalone
-# decomp7_part + finish7 on `ref` follows its own filter7_part)
-SWEEP = ("tuples_swept",)
 
 
 def state_error(code):
@@ -528,13 +525,20 @@ class Runner:
                     eng.finish7(0, o["outer"], o["middle"])
                 return True
 
+            # finish7's sweep is that of the phase 1 behind the installed list: the whole space's,
+            # or the last part's where the parts' lists were merged
+            parts = self.model.lst_parts
+
             def calls(r):
-                r.filter7_part(0, 1)
+                if parts == 1:
+                    r.filter7_part(0, 1)
+                else:
+                    r.set_list7(np.concatenate([r.filter7_part(p, parts) for p in range(parts)]))
                 k = r.decomp7_part(0, 1, o["outer"], o["middle"])
-                return k, result_fields(r.finish7(k, o["outer"], o["middle"]), 7, SWEEP)
+                return k, result_fields(r.finish7(k, o["outer"], o["middle"]), 7)
             k = eng.decomp7_part(0, 1, o["outer"], o["middle"])
-            got = (k, result_fields(eng.finish7(k, o["outer"], o["middle"]), 7, SWEEP))
-            want = self.want(st, ("decomp", seed), calls)
+            got = (k, result_fields(eng.finish7(k, o["outer"], o["middle"]), 7))
+            want = self.want(st, ("decomp", seed, parts), calls)
             assert got[0] == want[0], ("decomp7_part", hex(got[0]), hex(want[0]))
             assert_same(got[1], want[1], "finish7")
             return True
