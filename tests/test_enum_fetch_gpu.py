@@ -8,6 +8,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import _enum_reference as R
 import _enum_support as E
 import _fetch_support as F
 import _support as S
@@ -147,23 +148,27 @@ def test_fetch_and_pick_on_the_long_7lut_list(engine):
     e = engine.enumerate7(outer, middle, 0)
     assert (e.total, e.feasible) == (251_784, 71_023)
     whole = engine.enumerate7(outer, middle, e.total).matches
+    assert R.check_realises(whole, tabs, tgt, mask) == e.total
     _check_against_whole(engine, 7, 40, whole, np.random.RandomState(40))
     engine.enumerate7(outer, middle, 0)
     assert np.array_equal(engine.fetch_matches(0, e.total), whole)
 
 
-def _check_closed(engine, total, record, rs, picks):
-    """First page, pages across rank 2**24, the last page, deep random pages, seeded picks."""
+def _check_closed(engine, total, record, rs, picks, state):
+    """First page, pages across rank 2**24, the last page, deep random pages, seeded picks; every
+    record fetched or picked realises the target of `state` (tables, target, mask)."""
     firsts = [0, (1 << 24) - 2048, (1 << 24) - 1, 1 << 24, total - 4096] + \
         [int(x) for x in rs.randint(0, total - 600, 4)]
     for first in firsts:
         count = 4096 if first in (0, total - 4096) else 600
         got = engine.fetch_matches(first, count)
         assert len(got) == min(count, total - first)
+        assert R.check_realises(got, *state, what=first) == len(got)
         for j in sorted({0, len(got) - 1} | {int(x) for x in rs.randint(0, len(got), 40)}):
             assert F.as_tuple(got[j]) == record(first + j), (first, j)
     ranks = np.random.default_rng(int(rs.randint(1 << 30))).choice(total, picks, replace=False)
     got = engine.pick_matches(ranks)
+    assert R.check_realises(got, *state, what="picks") == len(got)
     for r, rec in zip(ranks, got):
         assert F.as_tuple(rec) == record(int(r)), int(r)
 
@@ -179,7 +184,7 @@ def test_3lut_n500_closed_form(engine, p):
     e = engine.enumerate3(order, 0)
     assert e.total == F.total3(n) == 20_708_500
     _check_closed(engine, e.total, lambda r: F.record3(r, tabs, tgt, mask, order),
-                  np.random.RandomState(3), 10_000)
+                  np.random.RandomState(3), 10_000, (tabs, tgt, mask))
 
 
 @pytest.mark.parametrize("n,inb,p", [(40, [], None), (40, [0, 2, 5], None), (64, [], None),
@@ -194,7 +199,7 @@ def test_5lut_closed_form(engine, n, inb, p):
     e = engine.enumerate5(order, 0)
     assert e.total == F.total5(n, inb) > (1 << 24)
     _check_closed(engine, e.total, lambda r: F.record5(r, tabs, tgt, mask, inb, order, rows5),
-                  np.random.RandomState(n), 10_000)
+                  np.random.RandomState(n), 10_000, (tabs, tgt, mask))
 
 
 @pytest.mark.parametrize("p", [None, 33])
@@ -211,7 +216,7 @@ def test_7lut_n40_closed_form(engine, p):
     assert e.total == 458_752_000_000
     _check_closed(engine, e.total,
                   lambda r: F.record7(r, tabs, tgt, mask, outer, middle, rows7, 100_000),
-                  np.random.RandomState(7), 10_000 if p is None else 2_000)
+                  np.random.RandomState(7), 10_000 if p is None else 2_000, (tabs, tgt, mask))
 
 
 def _raw_fetch(engine, first, count, out=True, n_out=True):

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 import torch
 
+import _enum_reference as R
 import _enum_support as E
 import _fetch_support as F
 import _support as S
@@ -97,6 +98,7 @@ def test_global_fetch_and_pick_equal_the_whole(engine, shares, case, P):
         # every rank once: its owner, and the block seams where the owner changes
         full = [e.fetch_matches(0, total) for e in engs]
         assert np.array_equal(_summed(full), whole)
+        assert R.check_realises(_summed(full), tabs, tgt, mask) == total
         owner = np.argmax(np.stack([f["width"] for f in full]) != 0, axis=0)
         seams = [int(r) for r in np.nonzero(np.diff(owner))[0] + 1]
         for s in seams[:5] + seams[-3:]:
@@ -124,14 +126,19 @@ def test_global_fetch_and_pick_equal_the_whole(engine, shares, case, P):
         assert np.array_equal(_summed([m for _, m in got]), m_whole)
 
 
-def _check_closed(engs, total, record, rs, picks):
+def _check_closed(engs, total, record, rs, picks, state):
+    """Pages and picks of the summed shares against the closed form; every record realises the
+    target of `state` (tables, target, mask)."""
     for first in (0, total // 2 - 300, total // 2, total - 4096):
         got = _fetch(engs, first, 600 if first else 4096)
         assert len(got) == min(600 if first else 4096, total - first)
+        assert R.check_realises(got, *state, what=first) == len(got)
         for j in sorted({0, len(got) - 1} | {int(x) for x in rs.randint(0, len(got), 30)}):
             assert F.as_tuple(got[j]) == record(first + j), (first, j)
     ranks = np.random.default_rng(int(rs.randint(1 << 30))).choice(total, picks, replace=False)
-    for r, rec in zip(ranks, _pick(engs, ranks)):
+    got = _pick(engs, ranks)
+    assert R.check_realises(got, *state, what="picks") == len(got)
+    for r, rec in zip(ranks, got):
         assert F.as_tuple(rec) == record(int(r)), int(r)
 
 
@@ -147,7 +154,7 @@ def test_5lut_empty_mask_closed_form(shares, n, want):
     assert total == F.total5(n, []) == want   # n = 64: past 2^32
     rows5 = S.order5_rows()
     _check_closed(shares, total, lambda r: F.record5(r, tabs, tgt, mask, [], order, rows5),
-                  np.random.RandomState(5), 1000)
+                  np.random.RandomState(5), 1000, (tabs, tgt, mask))
 
 
 def test_7lut_n40_past_2_32(shares):
@@ -164,7 +171,7 @@ def test_7lut_n40_past_2_32(shares):
     rows7 = S.order7_rows()
     _check_closed(engs, total,
                   lambda r: F.record7(r, tabs, tgt, mask, outer, middle, rows7, 100_000),
-                  np.random.RandomState(7), 1000)
+                  np.random.RandomState(7), 1000, (tabs, tgt, mask))
 
 
 def test_3lut_n500(shares):
@@ -178,7 +185,7 @@ def test_3lut_n500(shares):
     total = _count_global(shares, 3, [order])
     assert total == F.total3(n)
     _check_closed(shares, total, lambda r: F.record3(r, tabs, tgt, mask, order),
-                  np.random.RandomState(3), 1000)
+                  np.random.RandomState(3), 1000, (tabs, tgt, mask))
 
 
 def _raw_set_global(eng, sums, stride, counts, nparts=None):

@@ -8,6 +8,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 
+import _enum_reference as R
 import _enum_support as E
 import _support as S
 import sboxgates_b200 as sb
@@ -68,6 +69,7 @@ def _keys(e):
 
 
 def _check_records(which, e, tabs, tgt, mask, order, middle=None, tuples=None):
+    assert R.check_realises(e.matches, tabs, tgt, mask) == len(e.matches)
     for rec in e.matches[:60]:
         key = int(rec["key"])
         t7 = tuples[key >> 23] if which == 7 else None

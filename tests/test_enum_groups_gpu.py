@@ -11,6 +11,7 @@ import socket
 import numpy as np
 import pytest
 
+import _enum_reference as R
 import _enum_support as E
 import _fetch_support as F
 import _support as S
@@ -255,6 +256,7 @@ def test_long_7lut_list(engine):
     unf = _run(engine, 7, orders, 0)
     full = engine.fetch_matches(0, unf.total)
     assert len(full) == 251_784
+    assert R.check_realises(full, tabs, tgt, mask) == len(full)
     for g in GROUPINGS:
         want = _grouped(full, 7, g)
         assert len(want) == len(np.unique(_group_ids(full["key"], 7, g)))

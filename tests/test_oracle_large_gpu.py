@@ -19,6 +19,7 @@ import re
 import numpy as np
 import pytest
 
+import _enum_reference as R
 import _enum_support as E
 import _support as S
 import sboxgates_b200 as sb
@@ -405,6 +406,7 @@ def test_enum7_long_list_matches_oracle(engine):
     assert e.total == total and len(e.matches) == total
     keys = e.matches["key"].astype(np.uint64)
     assert np.all(keys[1:] > keys[:-1])
+    assert R.check_realises(e.matches, tabs, tgt, mask) == total
     lst = E.unpack_list(engine.filter7_part(0, 1))
     assert len(lst) == count
     idx = (keys >> np.uint64(23)).astype(np.int64)
