@@ -301,7 +301,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
        given), sbg_decomp7_part, sbg_finish7 or sbg_alu_peak ends it, whatever the call returns;
      - sbg_last_error, sbg_launch_count, sbg_transfer_stats, sbg_host_seconds, sbg_last_kernel_ms,
        sbg_set_timing, sbg_set_stream, sbg_enum_fetch, sbg_enum_pick, sbg_enum_block_sums,
-       sbg_enum_set_global and sbg_enum_depth_counts keep it;
+       sbg_enum_set_global, sbg_enum_depth_counts and sbg_enum_group_sizes keep it;
      - sbg_enum_set_depth ends it, whatever the call returns.
      - sbg_enum_set_functions ends it, whatever the call returns.
      - sbg_enum_set_grouping ends it, whatever the call returns.
@@ -425,13 +425,29 @@ int sbg_inner_table(const uint64_t *inner, uint8_t *out);
    the phase-1 list, and searches never read the setting.  sbg_enum_depth_counts bins each group
    once, at the depth of its record: every match of a shape has the same depth, but a gate set's
    record is its first match, which need not be its shallowest (a histogram by shallowest gate set
-   needs no grouping or shape grouping).  How many matches a group holds is not reported. */
+   needs no grouping or shape grouping).  How many matches a group holds: sbg_enum_group_sizes. */
 #define SBG_GROUP_NONE 0    /* every match (the default) */
 #define SBG_GROUP_SHAPE 1   /* one per (gates, ordering row) */
 #define SBG_GROUP_TUPLE 2   /* one per gate set */
 /* Sets the grouping of the later sbg_enum3 / sbg_enum5 / sbg_enum7 calls on the handle.  Any other
    value: SBG_ERR_ARG, with the setting left as it was.  The call ends the cursor. */
 int sbg_enum_set_grouping(sbg_handle *h, int grouping);
+/* sizes[i] = the number of matches in the group at rank ranks[i] of the cursor, i < nranks <=
+   SBG_ENUM_MAX_MATCHES: the matches the ungrouped enumeration, under the cursor's depth and
+   function filters, would count with that group's id (match_group).  5-LUT shape: the outer
+   functions that survive for that (tuple, row); 5-LUT tuple: their sum over the tuple's rows within
+   the depth bound; 7-LUT shape: the (outer, middle) pairs of that (entry, row) that pass the
+   filters; 7-LUT tuple: their sum over the entry's rows.  Every size is at least 1 and at most
+   2,560 (5-LUT tuple) or 70 * 65,536 = 4,587,520 (7-LUT tuple); the sizes of all ranks add up to
+   the ungrouped total.  On an ungrouped cursor, or at width 3, every size is 1.  The ranks may
+   come in any order and repeat.  A rank >= total: SBG_ERR_ARG and nothing written; ranks or sizes
+   NULL with nranks > 0: SBG_ERR_ARG; no cursor: SBG_ERR_STATE.  Keeps the cursor, and changes
+   neither the problem, the installed 7-LUT list nor the depth histogram.  On a global cursor each
+   share writes the sizes of the ranks it owns and 0 at every other slot, so the shares' arrays,
+   summed, are the whole's sizes.  Cost: the grouped pick's walk of every ticket holding a wanted
+   rank, plus, per wanted group, the ungrouped count of its rows (a tuple group: its whole ticket's
+   count; a 7-LUT count with a restricted inner set visits every (outer, middle) pair). */
+int sbg_enum_group_sizes(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, uint64_t *sizes);
 
 /* ---- helpers shared with the host side ------------------------------------------------------ */
 /* Test hook, no device needed: how a sweep's work is cut into tickets (DESIGN.md section 2, "Dense

@@ -2691,13 +2691,19 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
 //   kEnumRange  ranks [sel.lo, max_out) to out[rank - sel.lo];
 //   kEnumPick   one warp per ticket of sel.tickets, writing each rank of its slice of sel.ranks to
 //               out[sel.slots[...]] (duplicate ranks: every slot that asked for it).
-// The kernels keep one parameter list for all modes; sel reaches the range and pick forms in the
-// lane's EnumCtl block.
-enum EnumMode : int { kEnumCount = 0, kEnumFirst = 1, kEnumRange = 2, kEnumPick = 3 };
+//   kEnumSizes  pick's walk over the same selection, grouped form only: at a requested group it
+//               writes the number of the group's matches to EnumCtl::sizes[slot] instead of a
+//               record (see "grouping" below).
+// The kernels keep one parameter list for all modes; sel reaches the range, pick and sizes forms in
+// the lane's EnumCtl block.
+enum EnumMode : int { kEnumCount = 0, kEnumFirst = 1, kEnumRange = 2, kEnumPick = 3, kEnumSizes = 4 };
+
+// The passes that run over pick's selection (EnumSel::ranks, slots, tickets, first).
+__host__ __device__ constexpr bool by_rank(int mode) { return mode == kEnumPick || mode == kEnumSizes; }
 
 struct EnumSel {
   unsigned long long lo;                  // kEnumRange: first rank of the window
-  const unsigned long long *ranks;        // kEnumPick: the requested ranks, ascending, duplicates kept
+  const unsigned long long *ranks;        // pick / sizes: the requested ranks, ascending, duplicates kept
   const unsigned int *slots;              //   the output slot of each of them
   const unsigned long long *tickets;      //   the distinct tickets holding them, ascending
   const unsigned int *first;              //   ticket j's ranks: ranks[first[j] .. first[j+1]-1]
@@ -2709,20 +2715,20 @@ struct EnumTicket {
   unsigned long long max_out;    // first / range: the end of the wanted ranks
   unsigned long long base;       // emit: rank of the ticket's first match
   uint32_t count;                // matches met so far (count pass: the ticket's count)
-  unsigned int req, req_end;     // pick: the ticket's requests not yet met
+  unsigned int req, req_end;     // pick / sizes: the ticket's requests not yet met
 };
 
 // One ballot of a sweep: the lanes with hit hold the next matches of the ticket, in lane order.  The
 // ballot covers ranks [step_end - popc(ballot), step_end), the lane's own match has rank `at`, and
-// write(i) writes the lane's match to out[i].  Pick: the requests of this step are consumed in
-// order from req, each written by the lane that holds its rank.  Returns whether the ticket has
-// nothing more to emit (never in the count pass).
+// write(i) writes the lane's match to out[i].  Pick and sizes: the requests of this step are
+// consumed in order from req, each written by the lane that holds its rank (write(slot)).  Returns
+// whether the ticket has nothing more to emit (never in the count pass).
 template <int MODE, class Write>
 __device__ __forceinline__ bool emit_step(bool hit, EnumTicket &tk, Write write) {
   const uint32_t bal = __ballot_sync(kFull, hit);
   const unsigned long long at = tk.base + tk.count + __popc(bal & lanemask_lt());
   const unsigned long long step_end = tk.base + tk.count + __popc(bal);
-  if (MODE == kEnumPick) {
+  if (by_rank(MODE)) {
     for (; tk.req < tk.req_end; tk.req++) {
       const unsigned long long r = tk.sel.ranks[tk.req];
       if (r >= step_end) break;
@@ -2734,7 +2740,26 @@ __device__ __forceinline__ bool emit_step(bool hit, EnumTicket &tk, Write write)
   }
   tk.count += __popc(bal);
   if (MODE == kEnumCount) return false;
-  return MODE == kEnumPick ? tk.req >= tk.req_end : tk.base + tk.count >= tk.max_out;
+  return by_rank(MODE) ? tk.req >= tk.req_end : tk.base + tk.count >= tk.max_out;
+}
+
+// The sizes pass's state in a ticket's walk: the size of the group met last, and whether it is a
+// wanted tuple group whose later rows still add to its size before its step.  The other passes get
+// an empty stand-in, so that they carry no state of it.
+struct SizeWalk {
+  unsigned long long size = 0;
+  bool sizing = false;
+};
+struct NoSizeWalk {
+  static constexpr bool sizing = false;
+};
+template <int MODE>
+using SizeWalkOf = std::conditional_t<MODE == kEnumSizes, SizeWalk, NoSizeWalk>;
+
+// Sizes pass: whether the ticket's next group (rank tk.base + tk.count) is requested.  The ranks a
+// ticket holds are all met in its walk, so the next request is never below that rank.
+__device__ __forceinline__ bool size_wanted(const EnumTicket &tk) {
+  return tk.req < tk.req_end && tk.sel.ranks[tk.req] == tk.base + tk.count;
 }
 
 // The layout of sbg_match (include/sboxgates_b200.h; sbg_api.cu checks that the two agree).
@@ -2753,11 +2778,12 @@ struct EnumCtl {
   EnumSel sel;                  // range / pick emit: what to emit (set by the host before the pass)
   unsigned long long gtotal;    // k_enum_globalize: the whole's total
   unsigned int gbad;            //   1 if the share's own row of block sums differs from its own
+  unsigned long long *sizes;    // sizes pass: the group sizes, indexed by sel.slots
 };
 
-// The ticket loop of the enumeration kernels: one warp per ticket of t_begin .. t_end-1 (pick: per
-// entry j of sel.tickets, ticket sel.tickets[j]); the emit passes skip the tickets that hold no
-// wanted rank.  sweep(t, tk, feasible) sweeps ticket t, passing every ballot of matches to
+// The ticket loop of the enumeration kernels: one warp per ticket of t_begin .. t_end-1 (pick and
+// sizes: per entry j of sel.tickets, ticket sel.tickets[j]); the emit passes skip the tickets that
+// hold no wanted rank.  sweep(t, tk, feasible) sweeps ticket t, passing every ballot of matches to
 // emit_step.  In the count pass it leaves the ticket's matches in tk.count (and the 5-LUT sweep adds
 // the feasible tuples it met to feasible); the tickets' counts and both sums are written back here.
 template <int MODE, class Sweep>
@@ -2765,7 +2791,7 @@ __device__ __forceinline__ void enum_tickets(EnumCtl *__restrict__ ectl,
     uint32_t *__restrict__ counts, const unsigned long long *__restrict__ offsets,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, Sweep sweep) {
   EnumTicket tk = {};
-  if (MODE == kEnumRange || MODE == kEnumPick) tk.sel = ectl->sel;
+  if (MODE == kEnumRange || by_rank(MODE)) tk.sel = ectl->sel;
   tk.max_out = max_out;
   const int lane = threadIdx.x & 31;
   const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
@@ -2773,11 +2799,11 @@ __device__ __forceinline__ void enum_tickets(EnumCtl *__restrict__ ectl,
   for (unsigned long long j = t_begin + (unsigned long long)blockIdx.x * kWarpsPerCta
            + (threadIdx.x >> 5);
        j < t_end; j += nwarps) {
-    const unsigned long long t = MODE == kEnumPick ? tk.sel.tickets[j] : j;
+    const unsigned long long t = by_rank(MODE) ? tk.sel.tickets[j] : j;
     if (MODE != kEnumCount) {
-      if (MODE != kEnumPick && (counts[t] == 0 || offsets[t] >= max_out)) continue;
+      if (!by_rank(MODE) && (counts[t] == 0 || offsets[t] >= max_out)) continue;
       if (MODE == kEnumRange && offsets[t] + counts[t] <= tk.sel.lo) continue;
-      if (MODE == kEnumPick) {
+      if (by_rank(MODE)) {
         tk.req = tk.sel.first[j];
         tk.req_end = tk.sel.first[j + 1];
       }
@@ -3033,6 +3059,12 @@ __device__ __forceinline__ bool inner_ok7(const uint32_t *s_fn, const uint32_t *
 // key.  A key prefix names a 3-gate prefix ticket's tuple (5-LUT) or a list entry (7-LUT), so no
 // group crosses a ticket, and the count and emit passes stop at the same first match of a group.
 // The kind, EnumFilter::grouping, is warp-uniform.
+// The sizes pass (kEnumSizes, sbg_enum_group_sizes) walks a ticket's groups as the grouped pick
+// does, in key order through emit_step, so it meets them at the same ranks.  At a requested group
+// it counts the group's matches with the ungrouped count pass's arithmetic, the same tests at the
+// same points: a shape group its own row, a tuple group every row of its tuple or entry within the
+// depth bound.  A group's matches lie in its ticket, as the group does, so the count never leaves
+// the ticket either.
 
 // The 5-LUT sweep of one part, tickets t_begin .. t_end-1 of it: the warp's prefix, its (d,e) pairs
 // 32 at a time with the feasibility test of k_sweep (mixed prefix cells split by d and e), then per
@@ -3165,6 +3197,7 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
 #pragma unroll
             for (int i = 0; i < 5; i++) d5[i] = s_dep[g5[i]];
           }
+          [[maybe_unused]] SizeWalkOf<MODE> sw;
           for (int k = 0; k < 10 && !done; k++) {
             int kd = 0;
             if constexpr (FILTER) {
@@ -3186,9 +3219,26 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
                   surv &= __ballot_sync(kFull, inner_ok5(s_fn, rr[hi], rr0));
                 }
               }
-              if constexpr (GR) c |= surv;   // only whether the set is empty
+              if constexpr (GR && MODE != kEnumSizes) c |= surv;   // only whether the set is empty
               else c += __popc(surv);
               if (lane == hi) surv_mine = surv;
+            }
+            if constexpr (MODE == kEnumSizes) {
+              if (sw.sizing) {
+                sw.size += c;
+                continue;
+              }
+              if (c == 0) continue;
+              sw.size = c;
+              if (flt.grouping == kGroupTuple && size_wanted(tk)) {
+                sw.sizing = true;   // the tuple's later rows add to it; its step follows them
+                continue;
+              }
+              done = emit_step<MODE>(lane == 0, tk, [&](unsigned long long s) {
+                ectl->sizes[s] = sw.size;
+              });
+              if (flt.grouping == kGroupTuple) break;
+              continue;
             }
             if constexpr (GR) {
               if (MODE == kEnumCount) {
@@ -3232,6 +3282,13 @@ __device__ __forceinline__ void enum5_body(const DevProblem *__restrict__ prob,
               if (flt.grouping == kGroupTuple) break;
             }
           }
+          if constexpr (MODE == kEnumSizes) {
+            if (sw.sizing) {
+              done = emit_step<MODE>(lane == 0, tk, [&](unsigned long long s) {
+                ectl->sizes[s] = sw.size;
+              });
+            }
+          }
         }
       }
     }
@@ -3271,6 +3328,77 @@ __device__ __forceinline__ void cube_union(const uint32_t (*hv)[4], const bool (
       }
     }
   }
+}
+
+// Whether middle function fm lies in one cube set (see middle_cubes): fm's bit of cube_union.
+__device__ __forceinline__ bool in_cubes(const uint32_t (*hv)[4], const bool (*hok)[4], uint32_t S,
+    uint32_t ov, uint32_t fm) {
+  bool hit = false;
+#pragma unroll
+  for (int c0 = 0; c0 < 4; c0++) {
+#pragma unroll
+    for (int c1 = 0; c1 < 4; c1++) {
+      hit |= hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0
+          && (fm & S) == (hv[0][c0] | hv[1][c1]);
+    }
+  }
+  return hit;
+}
+
+// The outer functions of a warp's survivor words (lane hi holds word hi) to fo_list, ascending;
+// returns how many.
+__device__ __forceinline__ int outer_list7(uint32_t surv_mine, uint8_t *fo_list, int lane) {
+  int ns = 0;
+  __syncwarp();
+#pragma unroll
+  for (int hi = 0; hi < 8; hi++) {
+    const uint32_t sv = __shfl_sync(kFull, surv_mine, hi);
+    if ((sv >> lane) & 1u) fo_list[ns + __popc(sv & lanemask_lt())] = (uint8_t)(hi * 32 + lane);
+    ns += __popc(sv);
+  }
+  __syncwarp();
+  return ns;
+}
+
+// The sizes pass's count of one 7-LUT row: the matches of ordering row k among the outer functions
+// fo_list[0 .. ns-1], summed over the warp, as the ungrouped filtered count pass counts them.  With
+// every inner function allowed, one lane per outer function and the popcount of its cube union
+// ANDed with the middle set; with a restricted inner set (slow), every (fo, fm) of the union
+// through inner_ok7, lanes over fm.
+__device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, int ns,
+    const uint32_t *W, int k, const uint32_t *s_fn, bool slow, int lane) {
+  unsigned long long size = 0;
+#pragma unroll 1
+  for (int i0 = 0; i0 < ns; i0 += slow ? 1 : 32) {
+    const bool have = slow || i0 + lane < ns;
+    const int fo = slow ? fo_list[i0] : have ? fo_list[i0 + lane] : 0;
+    uint32_t r1 = 0, r0 = 0;
+#pragma unroll
+    for (int u = 0; u < 8; u++) {
+      if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
+    }
+    uint32_t hv[2][4], S, ov;
+    bool hok[2][4];
+    middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
+    if (!slow) {
+      uint32_t bits[8], c = 0;
+      cube_union(hv, hok, S, ov, bits);
+#pragma unroll
+      for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd] & s_fn[8 + wd]);
+      size += __reduce_add_sync(kFull, have ? c : 0u);
+      continue;
+    }
+    uint32_t AB[4];
+    inner_cells7(r1, r0, c_row_b[k], AB);
+#pragma unroll 1
+    for (int w = 0; w < 8; w++) {
+      const uint32_t fm = 32u * w + lane;
+      const bool hit = in_cubes(hv, hok, S, ov, fm) && in_set(s_fn + 8, fm)
+          && inner_ok7(s_fn, AB, fm);
+      size += __popc(__ballot_sync(kFull, hit));
+    }
+  }
+  return size;
 }
 
 // The 7-LUT sweep of one part over the list, tickets t_begin .. t_end-1 of it (entry idx = t *
@@ -3352,6 +3480,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
       tuple_summary<NW>(s_tabs, npad, g, T, M, lane, sH);
       const uint32_t pass_j = triples_with_colourings(sH, lane);
       bool done = false;
+      [[maybe_unused]] SizeWalkOf<MODE> sw;
       for (int j = 0; j < 25 && !done; j++) {
         if (((pass_j >> j) & 1u) == 0) continue;
         if constexpr (FILTER) {
@@ -3372,16 +3501,10 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
         if (any == 0) continue;
         const int k0 = c_j_first_k[j];
         const int nrows = c_j_rows[j];
+        [[maybe_unused]] int ns_sizes = 0;   // sizes pass: the survivors in fo_list
+        if constexpr (MODE == kEnumSizes) ns_sizes = outer_list7(surv_mine, fo_list, lane);
         if (!EMIT && !slow) {
-          int ns = 0;
-          __syncwarp();
-#pragma unroll
-          for (int hi = 0; hi < 8; hi++) {
-            const uint32_t sv = __shfl_sync(kFull, surv_mine, hi);
-            if ((sv >> lane) & 1u) fo_list[ns + __popc(sv & lanemask_lt())] = (uint8_t)(hi * 32 + lane);
-            ns += __popc(sv);
-          }
-          __syncwarp();
+          const int ns = outer_list7(surv_mine, fo_list, lane);
           if constexpr (GR) {
 #pragma unroll 1
             for (int row = 0; row < nrows; row++) {
@@ -3456,6 +3579,12 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
         for (int row = 0; (EMIT || slow) && row < nrows && !done; row++) {
           const int k = k0 + row;
           if (FILTER && depth7(d7, k) > B) continue;
+          if constexpr (MODE == kEnumSizes) {
+            if (sw.sizing) {
+              sw.size += row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
+              continue;
+            }
+          }
           [[maybe_unused]] const uint32_t row_start = tk.count;
           [[maybe_unused]] bool row_hit = false;   // grouped: the row's group is emitted
 #pragma unroll 1
@@ -3477,15 +3606,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
             for (int w = 0; w < 8; w++) {
               const uint32_t pm = 32u * w + lane;
               const uint32_t fm = s_ord[1][pm];
-              bool hit = false;
-#pragma unroll
-              for (int c0 = 0; c0 < 4; c0++) {
-#pragma unroll
-                for (int c1 = 0; c1 < 4; c1++) {
-                  hit |= hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0
-                      && (fm & S) == (hv[0][c0] | hv[1][c1]);
-                }
-              }
+              bool hit = in_cubes(hv, hok, S, ov, fm);
               if constexpr (FILTER) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
               if constexpr (GR) {
                 // the group's record: the first hit of the row
@@ -3494,9 +3615,23 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
                 hit = hit && (bal & lanemask_lt()) == 0;
                 row_hit = true;
               }
-              done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
-                write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
-              });
+              if constexpr (MODE == kEnumSizes) {
+                // the row's group; a wanted tuple group goes on through the entry's later rows
+                // and takes its step after them
+                if (size_wanted(tk)) {
+                  sw.size = row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
+                  sw.sizing = flt.grouping == kGroupTuple;
+                }
+                if (!sw.sizing) {
+                  done = emit_step<MODE>(hit, tk, [&](unsigned long long s) {
+                    ectl->sizes[s] = sw.size;
+                  });
+                }
+              } else {
+                done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
+                  write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
+                });
+              }
               if (GR && row_hit) break;
             }
             if (GR && row_hit) break;
@@ -3508,8 +3643,14 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
             }
           }
           if constexpr (GR) {
-            if (row_hit && flt.grouping == kGroupTuple) done = true;   // the entry is the group
+            // the entry is the group (unless the sizes pass is summing its rows)
+            if (row_hit && flt.grouping == kGroupTuple && !sw.sizing) done = true;
           }
+        }
+      }
+      if constexpr (MODE == kEnumSizes) {
+        if (sw.sizing) {
+          emit_step<MODE>(lane == 0, tk, [&](unsigned long long s) { ectl->sizes[s] = sw.size; });
         }
       }
     }

@@ -265,6 +265,22 @@ class DistributedLutSearch:
             return recs
         return self._sum_records(recs)
 
+    def group_sizes(self, ranks):
+        """The whole's group sizes at the given ranks (LutEngine.group_sizes), in their order, the
+        same on every rank: one all-reduce(SUM) of the shares' arrays (each share's sizes at the
+        ranks it owns, 0 elsewhere)."""
+        local = self.engine.group_sizes(ranks)
+        if self.world == 1 or local.shape[0] == 0:
+            return local
+        t0 = time.perf_counter()
+        t = torch.from_numpy(local.view(np.int64).copy()).to(self.device)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        self.collectives += 1
+        out = t.cpu().numpy().view(np.uint64).copy()
+        self.collective_ms += 1e3 * (time.perf_counter() - t0)
+        assert not np.any(out == 0), "a rank of the whole is owned by no share"
+        return out
+
     def sample_matches(self, enumeration, k, seed=None):
         """k distinct matches drawn uniformly from the whole (lut.sample_matches); every rank draws
         the same ranks from the same seed."""

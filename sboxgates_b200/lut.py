@@ -73,6 +73,19 @@ def _u64(a):
     return a, a.ctypes.data_as(native.u64p)
 
 
+def _rank_array(ranks):
+    """The ranks of a pick or group-sizes call, checked: a contiguous 1-D uint64 array of at most
+    SBG_ENUM_MAX_MATCHES non-negative integers."""
+    r = np.asarray(ranks)
+    if r.ndim != 1 or (r.size > 0 and r.dtype.kind not in "iu"):
+        raise ValueError("ranks must be a 1-D integer array")
+    if r.shape[0] > SBG_ENUM_MAX_MATCHES:
+        raise ValueError("at most %d ranks per call" % SBG_ENUM_MAX_MATCHES)
+    if r.size > 0 and r.dtype.kind == "i" and int(r.min()) < 0:
+        raise ValueError("ranks must not be negative")
+    return np.ascontiguousarray(r, dtype=np.uint64)
+
+
 def _order_ptr(order):
     buf = (C.c_uint8 * 256).from_buffer_copy(bytes(order))
     return buf
@@ -426,17 +439,25 @@ class LutEngine:
         On a global cursor (enum_set_global) the ranks are ranks of the whole, below the whole's
         total: this share's records at the ranks it owns, all-zero records (width 0) at every other
         slot.  Summing the shares' outputs as 64-bit words gives the whole's records."""
-        r = np.asarray(ranks)
-        if r.ndim != 1 or (r.size > 0 and r.dtype.kind not in "iu"):
-            raise ValueError("ranks must be a 1-D integer array")
-        if r.shape[0] > SBG_ENUM_MAX_MATCHES:
-            raise ValueError("at most %d ranks per pick" % SBG_ENUM_MAX_MATCHES)
-        if r.size > 0 and r.dtype.kind == "i" and int(r.min()) < 0:
-            raise ValueError("ranks must not be negative")
-        r = np.ascontiguousarray(r, dtype=np.uint64)
+        r = _rank_array(ranks)
         out = np.zeros(max(r.shape[0], 1), dtype=MATCH_DTYPE)
         self._check(self.lib.sbg_enum_pick(self._h, r.ctypes.data_as(native.u64p), r.shape[0],
                                            out.ctypes.data_as(C.c_void_p)))
+        return out[:r.shape[0]].copy()
+
+    def group_sizes(self, ranks):
+        """The number of matches in the group at each of the given ranks of the last counted
+        enumeration, as a numpy uint64 array in the order of `ranks` (checked as pick_matches
+        checks them): the matches the ungrouped enumeration, under the same depth and function
+        filters, counts with that group's match_group id.  All ones on an ungrouped cursor and for
+        enumerate3.  Nothing is counted again but the wanted groups' own matches.
+
+        On a global cursor (enum_set_global): this share's sizes at the ranks it owns, 0 at every
+        other slot.  Summing the shares' outputs gives the whole's sizes."""
+        r = _rank_array(ranks)
+        out = np.zeros(max(r.shape[0], 1), dtype=np.uint64)
+        self._check(self.lib.sbg_enum_group_sizes(self._h, r.ctypes.data_as(native.u64p),
+                                                  r.shape[0], out.ctypes.data_as(native.u64p)))
         return out[:r.shape[0]].copy()
 
     # -- global ranks across shares (the cursor of a sharded count) -----------------------------

@@ -119,6 +119,7 @@ SIGNATURES = {
     "sbg_enum_set_functions": (C.c_int, [C.c_void_p, u64p, u64p, u64p]),
     "sbg_inner_table": (C.c_int, [u64p, C.POINTER(C.c_uint8)]),
     "sbg_enum_set_grouping": (C.c_int, [C.c_void_p, C.c_int]),
+    "sbg_enum_group_sizes": (C.c_int, [C.c_void_p, u64p, C.c_uint64, u64p]),
 }
 
 _lib = None
