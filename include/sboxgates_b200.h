@@ -267,6 +267,27 @@ int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, ui
 int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
     uint64_t *total, uint64_t *feasible);
+/* The matches sbg_enum7 would return if phase 1 had no list cap: every 7-combination of the current
+   problem that has no gate excluded by inbits and passes check_n_lut_possible(7), decided on the
+   true gate tables with the same ordering rows, orders and inner solve as sbg_enum7 (the stale
+   outer cache is not reproduced either).  Key rank<<23 | k<<16 | po<<8 | pm, rank being the
+   combination's lexicographic rank among all C(n,7) (as for the 5-LUT key and sbg_result::index;
+   below 2^30 at n <= 64), so decode_key7 and the grouping key prefixes read it as they read a list
+   index.  Records are byte-identical to the ones sbg_enum7 emits for the same combination, row and
+   positions; only the key differs.  *feasible = the share's feasible 7-combinations (under a depth
+   filter: those with an ordering within the bound, as for sbg_enum5) -- at width 7 the number the
+   list cap hides.  part/nparts, max_matches, the count-free first K, the cursor (fetch, pick, group
+   sizes, depth counts, global ranks) and the depth, function and grouping settings behave as for
+   the other widths; a share's tickets are 6-gate prefixes dealt in blocks of 16.  The call builds
+   no list: an installed 7-LUT list and what sbg_search7 / sbg_enum7 see of it stay as they were.
+   The count buffers take 12 bytes per 6-gate prefix, C(n-1, 6) of them (815 MB at n = 64).
+   SBG_ERR_ARG: n < 7, n > SBG_ENUM7_ALL_MAX_GATES, an order that is not a permutation, or a depth
+   filter of another n; SBG_ERR_STATE: no problem loaded.  The call ends the cursor, whatever it
+   returns. */
+#define SBG_ENUM7_ALL_MAX_GATES 64
+int sbg_enum7_all(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
+    const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
+    uint64_t *total, uint64_t *feasible);
 /* The matches of lut_search's 3-LUT scan (lut.c:501-523) over the caller's shuffled gate order
    (n entries): the position triples i < k < m whose gates gate_order[i], gate_order[k],
    gate_order[m] pass check_n_lut_possible(3, ...) under the mask (get_lut_function then cannot
@@ -307,8 +328,9 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
      - sbg_enum_set_grouping ends it, whatever the call returns.
    Without a cursor both calls return SBG_ERR_STATE.
    A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
-   a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT) or a list
-   entry (7-LUT, up to 70 * 65,536 matches), so one deep rank can cost a whole ticket's sweep. */
+   a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT), a list
+   entry (7-LUT, up to 70 * 65,536 matches) or a 6-gate prefix (sbg_enum7_all, up to n - 7
+   combinations of that many), so one deep rank can cost a whole ticket's sweep. */
 /* The matches at ranks first .. min(first + count, total) - 1, in key order, to out[0..]; *n_out =
    how many (0 when first >= total).  count <= SBG_ENUM_MAX_MATCHES; out may be NULL iff count ==
    0. */
@@ -320,10 +342,10 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
 
 /* ---- global ranks across shares --------------------------------------------------------------- */
 /* A share's tickets fall into deal blocks, in the order the parts are dealt them: blocks of 16
-   position pairs (3-LUT) or 3-gate prefixes (5-LUT), local block j being the whole's block
-   j * nparts + part; or single list entries (7-LUT), local entry t being list entry
-   t * nparts + part.  The whole's blocks are in key order, so from every share's block sums each
-   share can turn its ranks into ranks of the whole (a global cursor):
+   position pairs (3-LUT), 3-gate prefixes (5-LUT) or 6-gate prefixes (sbg_enum7_all), local block j
+   being the whole's block j * nparts + part; or single list entries (sbg_enum7), local entry t
+   being list entry t * nparts + part.  The whole's blocks are in key order, so from every share's
+   block sums each share can turn its ranks into ranks of the whole (a global cursor):
      1. every share counts (sbg_enum* with part = its part, nparts, total != NULL);
      2. sbg_enum_block_sums on each; the rows are gathered in part order;
      3. sbg_enum_set_global on each with all the rows;

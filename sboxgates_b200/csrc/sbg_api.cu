@@ -192,12 +192,14 @@ struct EnumBuffers {
 };
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
-// (widths 5 and 7) or the gate order (width 3), the kernel form (EnumForm) and, for the filtered and
-// grouped forms, the filter block (take_filter; its histogram pointer is the lane's, set at launch).
+// (widths 5 and 7) or the gate order (width 3), the kernel form (EnumForm), the 7-LUT ticket source
+// (Enum7Source; kSrcList at the other widths) and, for the filtered and grouped forms, the filter
+// block (take_filter; its histogram pointer is the lane's, set at launch).
 struct EnumInputs {
   EnumOrders ord;
   EnumGateOrder gates;
   int form;
+  int source;
   EnumFilter filter;
 };
 
@@ -226,7 +228,7 @@ struct EnumCursor {
   int width = 0, part = 0, nparts = 1, slot = -1;
   EnumInputs in;
   uint64_t tickets = 0, total = 0;
-  uint32_t list_count = 0;   // width 7
+  uint32_t list_count = 0;   // width 7 over the list
   uint64_t blocks = 0;       // the whole's deal blocks (every part's)
   bool global = false;       // sbg_enum_set_global ran: offsets and total are the whole's
 };
@@ -355,6 +357,12 @@ template <int NW>
 size_t decomp_smem(int n) {
   const int npad = (n + 3) & ~3;
   return sizeof(uint32_t) * (size_t)(NW * npad);
+}
+
+// k_enum7_all: the tables and each warp's prefix cells.
+template <int NW>
+size_t enum7_all_smem(int n) {
+  return decomp_smem<NW>(n) + sizeof(uint32_t) * (size_t)(kWarpsPerCta * kPrefix7Cells * NW);
 }
 
 // Kernels whose dynamic shared memory can exceed the 48 KB default opt in once per size class.
@@ -1556,6 +1564,8 @@ static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
 // most 128 bytes of pointers and scalars, within the 4 KB kernel-parameter limit.
 static_assert(sizeof(EnumGateOrder) + sizeof(EnumFilter) + 128 <= 4096,
     "the filtered k_enum3's parameters fit in 4 KB");
+static_assert(kEnum7AllMaxGates == SBG_ENUM7_ALL_MAX_GATES,
+    "one limit of the whole-space 7-LUT sweep");
 
 // Count-free windows start at this many tickets and double: a first-match search then costs a few
 // windows of work past the first match, a search without one about twice the counting sweep's
@@ -1563,6 +1573,9 @@ static_assert(sizeof(EnumGateOrder) + sizeof(EnumFilter) + 128 <= 4096,
 constexpr uint64_t kEnumWindow3 = kNominalWarps;
 constexpr uint64_t kEnumWindow5 = kNominalWarps;
 constexpr uint64_t kEnumWindow7 = kNominalWarps / 4;
+// A whole-space ticket is a 6-gate prefix, up to n - 7 combinations: a window's work past the first
+// match stays near a list window's with fewer tickets per window.
+constexpr uint64_t kEnumWindow7All = kNominalWarps / 16;
 
 // The first n emitted records to the caller's out.
 int copy_matches(sbg_handle *h, sbg_lane &L, sbg_match *out, uint64_t n) {
@@ -1609,6 +1622,11 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
             E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, h->d_tab.p,
             flt);
       } else {
+        if (in.source == kSrcWhole) {
+          return run(k_enum7_all<NW, MODE, FORM>, enum7_all_smem<NW>(n), prob, E.d_ectl.p,
+              in.ord, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts,
+              h->d_tab.p, flt);
+        }
         return run(k_enum7<NW, MODE, FORM>, decomp_smem<NW>(n), prob, E.d_ectl.p, in.ord,
             L.d_sorted.p, h->list7.count, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b,
             part, nparts, h->d_tab.p, flt);
@@ -1630,15 +1648,17 @@ uint64_t deal_share(uint64_t blocks, int q, int nparts) {
   return blocks > (uint64_t)q ? (blocks - q + nparts - 1) / nparts : 0;
 }
 
-// Tickets per deal block of an enumeration of `width`: kDeal position pairs or 3-gate prefixes, or
-// one 7-LUT list entry.
-unsigned int enum_block_size(int width) { return width == 7 ? 1u : (unsigned)kDeal; }
+// Tickets per deal block of an enumeration of `width` from `source` (Enum7Source): kDeal position
+// pairs, 3-gate prefixes or 6-gate prefixes, or one 7-LUT list entry.
+unsigned int enum_block_size(int width, int source) {
+  return width == 7 && source == kSrcList ? 1u : (unsigned)kDeal;
+}
 
-// sbg_enum3 / sbg_enum5 / sbg_enum7 once their arguments are checked.  Lane 0 takes the current
-// problem slot, and k_begin (flags, begin_in) brings its problem block up to date; a 7-LUT
-// enumeration without an installed list runs phase 1 instead, which does that and installs the
-// list.  Then the part's tickets are counted (in windows when only the first max_matches are
-// wanted), their offsets taken, and the first max_matches emitted and copied out.
+// sbg_enum3 / sbg_enum5 / sbg_enum7 / sbg_enum7_all once their arguments are checked.  Lane 0
+// takes the current problem slot, and k_begin (flags, begin_in) brings its problem block up to date;
+// a 7-LUT enumeration over the list without an installed one runs phase 1 instead, which does that
+// and installs the list.  Then the part's tickets are counted (in windows when only the first
+// max_matches are wanted), their offsets taken, and the first max_matches emitted and copied out.
 template <int WIDTH>
 int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const EnumInputs &in,
     int part, int nparts, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
@@ -1648,7 +1668,8 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   EnumBuffers &E = h->ebuf;
   int rc;
   if ((rc = lane_uses_slot(h, L, h->cur_slot)) != SBG_OK) return rc;
-  if (WIDTH == 7 && !list_is_current(h, false)) {
+  const bool whole = WIDTH == 7 && in.source == kSrcWhole;
+  if (WIDTH == 7 && !whole && !list_is_current(h, false)) {
     uint32_t count = 0;
     uint64_t swept = 0;
     if ((rc = run_filter7(h, L, 0, 1, &count, &swept)) != SBG_OK) return rc;
@@ -1659,9 +1680,9 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   }
   // this part's tickets: its deal blocks (the last one may be cut short)
   const int n = h->slots[L.slot].n;
-  const uint64_t B = enum_block_size(WIDTH);
+  const uint64_t B = enum_block_size(WIDTH, in.source);
   const uint64_t items = WIDTH == 3 ? h_binom[n][2] : WIDTH == 5 ? h_binom[n - 2][3]
-      : h->list7.count;
+      : whole ? h_binom[n - 1][6] : h->list7.count;
   const uint64_t blocks = (items + B - 1) / B;
   const uint64_t tickets = deal_share(blocks, part, nparts) * B;
   if ((rc = E.d_ectl.grow(h, L.stream, 1)) != SBG_OK) return rc;
@@ -1675,7 +1696,8 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   }
   const bool count_all = total != nullptr;
   uint64_t window = count_all ? tickets
-      : (WIDTH == 3 ? kEnumWindow3 : WIDTH == 5 ? kEnumWindow5 : kEnumWindow7);
+      : (WIDTH == 3 ? kEnumWindow3 : WIDTH == 5 ? kEnumWindow5
+         : whole ? kEnumWindow7All : kEnumWindow7);
   uint64_t done = 0;
   EnumCtl ec;
   memset(&ec, 0, sizeof(ec));
@@ -1719,7 +1741,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   if (total != nullptr) *total = ec.carry;
   if (feasible != nullptr) {
     // width 3: every feasible triple is a match (the filtered form counts them apart)
-    *feasible = WIDTH == 7 ? (uint64_t)h->list7.count
+    *feasible = WIDTH == 7 && !whole ? (uint64_t)h->list7.count
         : WIDTH == 3 && in.form == kFormPlain ? ec.total : ec.feasible;
   }
   return SBG_OK;
@@ -1812,7 +1834,7 @@ int check_cursor(sbg_handle *h) {
         "sbg_enum3 / sbg_enum5 / sbg_enum7 call with nothing in between");
   }
   if (h->lane[0].slot != c.slot || h->ebuf.d_ecount.cap < c.tickets
-      || (c.width == 7 && h->list7.count != c.list_count)) {
+      || (c.width == 7 && c.in.source == kSrcList && h->list7.count != c.list_count)) {
     return fail(h, SBG_ERR_STATE, "internal: enumeration cursor out of step with its buffers");
   }
   return SBG_OK;
@@ -1843,7 +1865,8 @@ int block_sums(sbg_handle *h, sbg_lane &L, uint64_t nblocks) {
   const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nblocks + 255) / 256,
       (uint64_t)h->sm_count * 8));
   const cudaError_t e = launch(h, k_enum_block_sums, grid, 256, 0, L.stream, false,
-      (const uint32_t *)E.d_ecount.p, (unsigned long long)nblocks, enum_block_size(h->cursor.width),
+      (const uint32_t *)E.d_ecount.p, (unsigned long long)nblocks,
+      enum_block_size(h->cursor.width, h->cursor.in.source),
       E.d_bsums.p);
   if (e != cudaSuccess) return fail(h, SBG_ERR_CUDA, "k_enum_block_sums: %s", cudaGetErrorString(e));
   return SBG_OK;
@@ -2815,6 +2838,7 @@ int sbg_enum5(sbg_handle *h, int part, int nparts, const uint8_t *func_order, ui
   EnumInputs in5;
   memcpy(in5.ord.order[0], func_order, 256);
   memset(in5.ord.order[1], 0, 256);
+  in5.source = kSrcList;
   if ((rc = take_filter(h, 5, in5)) != SBG_OK) return rc;
   return run_enum<5>(h, kBeginSearch5, in, in5, part, nparts, max_matches, out, n_out, total,
       feasible);
@@ -2832,8 +2856,33 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
   EnumInputs in7;
   memcpy(in7.ord.order[0], outer_order, 256);
   memcpy(in7.ord.order[1], middle_order, 256);
+  in7.source = kSrcList;
   if ((rc = take_filter(h, 7, in7)) != SBG_OK) return rc;
   // the installed list: only bring the problem block up to date
+  return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
+      total, feasible);
+}
+
+int sbg_enum7_all(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
+    const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
+    uint64_t *total, uint64_t *feasible) {
+  int rc;
+  if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
+  const int n = cur(h).n;
+  if (n < 7 || n > SBG_ENUM7_ALL_MAX_GATES) {
+    return fail(h, SBG_ERR_ARG, "the whole-space 7-LUT enumeration needs 7 <= n <= %d, not %d",
+        SBG_ENUM7_ALL_MAX_GATES, n);
+  }
+  if (!valid_order(outer_order) || !valid_order(middle_order)) {
+    return fail(h, SBG_ERR_ARG, "function order is not a permutation");
+  }
+  EnumInputs in7;
+  memcpy(in7.ord.order[0], outer_order, 256);
+  memcpy(in7.ord.order[1], middle_order, 256);
+  in7.source = kSrcWhole;
+  if ((rc = take_filter(h, 7, in7)) != SBG_OK) return rc;
+  // no list: only bring the problem block up to date, so an installed list and its control words
+  // stay as they are
   return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
       total, feasible);
 }
@@ -2964,7 +3013,7 @@ int sbg_enum_block_sums(sbg_handle *h, uint64_t *out, uint64_t *nblocks) {
   int rc;
   if ((rc = check_cursor(h)) != SBG_OK) return rc;
   const EnumCursor &c = h->cursor;
-  const uint64_t nb = c.tickets / enum_block_size(c.width);
+  const uint64_t nb = c.tickets / enum_block_size(c.width, c.in.source);
   *nblocks = nb;
   if (out == nullptr || nb == 0) return SBG_OK;
   SBG_CUDA(h, cudaSetDevice(h->device));
@@ -3005,7 +3054,7 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
   EnumBuffers &E = h->ebuf;
-  const unsigned int B = enum_block_size(c.width);
+  const unsigned int B = enum_block_size(c.width, c.in.source);
   const uint64_t nb = c.tickets / B;
   uint64_t whole = 0;
   if (c.blocks > 0) {

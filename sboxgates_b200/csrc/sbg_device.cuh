@@ -167,7 +167,7 @@ __device__ __forceinline__ void stage_tables(uint32_t *s_tabs, const DevProblem 
   __syncthreads();
 }
 
-// C(a, r) for 0 <= a <= 512, r <= 5, by arithmetic (exact at every step: a product of k consecutive
+// C(a, r) for 0 <= a <= 512, r <= 7, by arithmetic (exact at every step: a product of k consecutive
 // integers is divisible by k!).  r is a compile-time constant wherever this is called from an
 // unrolled loop, the chain below then folds to the one case.  The table c_binom sits in constant
 // memory, which serves one address per warp at a time -- lanes that each need a different entry
@@ -181,7 +181,11 @@ __device__ __forceinline__ uint64_t binom_arith(uint32_t a, int r) {
   if (r == 3) return c3;
   const uint64_t c4 = ((uint64_t)c3 * (uint64_t)(a - 3u)) >> 2;
   if (r == 4) return c4;                                   // (a < r: some factor above is zero)
-  return (c4 * (uint64_t)(a - 4u)) / 5ull;
+  const uint64_t c5 = (c4 * (uint64_t)(a - 4u)) / 5ull;
+  if (r == 5) return c5;
+  const uint64_t c6 = (c5 * (uint64_t)(a - 5u)) / 6ull;   // <= C(512, 6) * 507 < 2^64
+  if (r == 6) return c6;
+  return (c6 * (uint64_t)(a - 6u)) / 7ull;
 }
 
 // Work item t of the P-element prefixes of K-combinations over n gates, lexicographic order, and
@@ -194,7 +198,7 @@ __device__ __forceinline__ uint64_t binom_arith(uint32_t a, int r) {
 template <int P, int K, bool RANK>
 __device__ __forceinline__ void unrank_prefix_warp(uint64_t t64, int n, int *pre, uint64_t &base_rank,
     int lane) {
-  static_assert(P <= 5 && (!RANK || K <= 5), "binom_arith covers r <= 5");
+  static_assert(P <= 6 && (!RANK || K <= 7), "binom_arith covers r <= 7");
   // the number of P-prefixes fits 32 bits up to P = 4 (C(509, 4) = 2.77e9)
   using T = typename std::conditional<(P <= 4), uint32_t, uint64_t>::type;
   const int np = n - (K - P);
@@ -2718,6 +2722,14 @@ struct EnumTicket {
   unsigned int req, req_end;     // pick / sizes: the ticket's requests not yet met
 };
 
+// Whether the ticket has nothing more to emit: the first / range pass has reached max_out, the pick
+// or sizes pass has met the ticket's last request (never in the count pass).
+template <int MODE>
+__device__ __forceinline__ bool ticket_over(const EnumTicket &tk) {
+  if (MODE == kEnumCount) return false;
+  return by_rank(MODE) ? tk.req >= tk.req_end : tk.base + tk.count >= tk.max_out;
+}
+
 // One ballot of a sweep: the lanes with hit hold the next matches of the ticket, in lane order.  The
 // ballot covers ranks [step_end - popc(ballot), step_end), the lane's own match has rank `at`, and
 // write(i) writes the lane's match to out[i].  Pick and sizes: the requests of this step are
@@ -2739,8 +2751,7 @@ __device__ __forceinline__ bool emit_step(bool hit, EnumTicket &tk, Write write)
     write(MODE == kEnumRange ? at - tk.sel.lo : at);
   }
   tk.count += __popc(bal);
-  if (MODE == kEnumCount) return false;
-  return by_rank(MODE) ? tk.req >= tk.req_end : tk.base + tk.count >= tk.max_out;
+  return ticket_over<MODE>(tk);
 }
 
 // The sizes pass's state in a ticket's walk: the size of the group met last, and whether it is a
@@ -3401,21 +3412,42 @@ __device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, 
   return size;
 }
 
-// The 7-LUT sweep of one part over the list, tickets t_begin .. t_end-1 of it (entry idx = t *
-// nparts + part), one warp per entry: the summary and stage-1 filter of k_decomp7 on the TRUE gate
-// tables (no stale outer cache), then per surviving outer function and ordering row the union of
-// the middle-function cubes.  Count: one lane per outer function; emit: positions in ascending
-// order, outer position in the loop, middle position across the lanes.  Filtered and grouped
-// forms: the depth filter (see depth7); an entry without an ordering within the bound is skipped,
-// and so is every row above it.  The function filter: the outer set cuts the survivors, the middle
-// set the cube union.  A restricted inner set depends on the whole of fm, not only on its cube, so
-// the count pass then runs the emit loop (positions over the lanes) in place of the popcounts, and
-// both passes apply inner_ok7 to each lane's (fo, fm).  Grouped form (see "grouping" above
-// enum5_body): the count pass takes a row once when some surviving outer function leaves a
-// non-empty cube union (rows outer, outer functions inner, stopping at the first); the emit loop
-// emits a row's first hit (first po, lowest pm) and moves to the next row.  Under kGroupTuple both
-// end the entry at its first row with a match.
-template <int NW, int MODE, int FORM>
+// Where the 7-LUT enumeration takes its combinations from (template parameter SRC of enum7_body):
+//   kSrcList   the installed phase-1 list (sbg_enum7): ticket t of the part is list entry
+//              idx = t * nparts + part, and the key's high field is idx;
+//   kSrcWhole  every 7-combination (sbg_enum7_all, n <= kEnum7AllMaxGates): a ticket is a 6-gate
+//              prefix a < ... < f <= n - 2 in lexicographic order, dealt to the parts in blocks of
+//              kDeal as k_enum5 deals its 3-gate prefixes; the lanes take the last gate g, and the
+//              feasible (a..f, g) go through the per-combination part below in ascending g, with
+//              the combination's rank in C(n,7) order as the key's high field.  A ticket holds at
+//              most (n - 6) * 70 * 65,536 < 2^32 matches (a 5-gate prefix could hold more than
+//              2^32 at n >= 49), so the u32 per-ticket counts and the scans serve it unchanged.
+//              Feasibility is k_sweep's test with a 6-gate prefix: every mixed prefix cell (masked
+//              1s and 0s of the target) must be split by g into a part without a masked 0 and a
+//              part without a masked 1.  Gates excluded by inbits drop out as in phase 1; under
+//              the depth filter a prefix, or a lane's g, that no ordering within the bound can
+//              use is dropped before the feasibility work, and `feasible` counts the feasible
+//              combinations with such an ordering.
+enum Enum7Source : int { kSrcList = 0, kSrcWhole = 1 };
+constexpr int kEnum7AllMaxGates = 64;   // SBG_ENUM7_ALL_MAX_GATES: C(63, 6) tickets of 12 bytes
+constexpr int kPrefix7Cells = 64;       // cells of a 6-gate prefix
+
+// The 7-LUT sweep of one part, tickets t_begin .. t_end-1 of it, one warp per ticket; per
+// combination (a list entry, or a feasible tuple of a prefix): the summary and stage-1 filter of
+// k_decomp7 on the TRUE gate tables (no stale outer cache), then per surviving outer function and
+// ordering row the union of the middle-function cubes.  Count: one lane per outer function; emit:
+// positions in ascending order, outer position in the loop, middle position across the lanes.
+// Filtered and grouped forms: the depth filter (see depth7); a combination without an ordering
+// within the bound is skipped, and so is every row above it.  The function filter: the outer set
+// cuts the survivors, the middle set the cube union.  A restricted inner set depends on the whole
+// of fm, not only on its cube, so the count pass then runs the emit loop (positions over the lanes)
+// in place of the popcounts, and both passes apply inner_ok7 to each lane's (fo, fm).  Grouped form
+// (see "grouping" above enum5_body): the count pass takes a row once when some surviving outer
+// function leaves a non-empty cube union (rows outer, outer functions inner, stopping at the
+// first); the emit loop emits a row's first hit (first po, lowest pm) and moves to the next row.
+// Under kGroupTuple both end the combination at its first row with a match.  A group never leaves
+// its combination, so it never crosses a ticket under either source.
+template <int NW, int MODE, int FORM, int SRC>
 __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders &ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
@@ -3456,205 +3488,295 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
   uint32_t *sH = s_H[warp];
   uint8_t *fo_list = s_fo[warp];
 
-  enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
-      [&](unsigned long long t, EnumTicket &tk, unsigned long long &) {
-    const uint64_t idx = t * (uint64_t)nparts + (uint64_t)part;
-    if (idx < list_count) {
-      const uint64_t cur = list[idx];
-      int g[7];
+  // One combination g (tuple order), whose keys are idx << 23 | k << 16 | po << 8 | pm: its
+  // matches in key order through emit_step.
+  auto tuple7 = [&](const int *g, unsigned long long idx, EnumTicket &tk) {
+    int d7[7];
+    if constexpr (FILTER) {
+      // no gate of depth >= B, and at most one of depth B - 1 (it must be the last input)
+      int deep = 0;
+      bool over = false;
 #pragma unroll
-      for (int i = 0; i < 7; i++) g[i] = (int)((cur >> (9 * (6 - i))) & 0x1ffu);
-      int d7[7];
-      if constexpr (FILTER) {
-        // no gate of depth >= B, and at most one of depth B - 1 (it must be the last input)
-        int deep = 0;
-        bool over = false;
-#pragma unroll
-        for (int i = 0; i < 7; i++) {
-          d7[i] = s_dep[g[i]];
-          over |= d7[i] >= B;
-          deep += d7[i] >= B - 1;
-        }
-        if (over || deep > 1) return;
+      for (int i = 0; i < 7; i++) {
+        d7[i] = s_dep[g[i]];
+        over |= d7[i] >= B;
+        deep += d7[i] >= B - 1;
       }
-      tuple_summary<NW>(s_tabs, npad, g, T, M, lane, sH);
-      const uint32_t pass_j = triples_with_colourings(sH, lane);
-      bool done = false;
-      [[maybe_unused]] SizeWalkOf<MODE> sw;
-      for (int j = 0; j < 25 && !done; j++) {
-        if (((pass_j >> j) & 1u) == 0) continue;
-        if constexpr (FILTER) {
-          bool fits = false;
-          for (int row = 0; row < c_j_rows[j]; row++) fits |= depth7(d7, c_j_first_k[j] + row) <= B;
-          if (!fits) continue;
-        }
-        uint32_t W[8], ok[8];
-        outer_ok7(sH, s_src7[j * 32 + lane], lane, W, ok);
-        uint32_t any = 0, surv_mine = 0;
+      if (over || deep > 1) return;
+    }
+    tuple_summary<NW>(s_tabs, npad, g, T, M, lane, sH);
+    const uint32_t pass_j = triples_with_colourings(sH, lane);
+    bool done = false;
+    [[maybe_unused]] SizeWalkOf<MODE> sw;
+    for (int j = 0; j < 25 && !done; j++) {
+      if (((pass_j >> j) & 1u) == 0) continue;
+      if constexpr (FILTER) {
+        bool fits = false;
+        for (int row = 0; row < c_j_rows[j]; row++) fits |= depth7(d7, c_j_first_k[j] + row) <= B;
+        if (!fits) continue;
+      }
+      uint32_t W[8], ok[8];
+      outer_ok7(sH, s_src7[j * 32 + lane], lane, W, ok);
+      uint32_t any = 0, surv_mine = 0;
 #pragma unroll
-        for (int hi = 0; hi < 8; hi++) {
-          uint32_t sv = ok[hi] & __brev(ok[7 - hi]);
-          if constexpr (FILTER) sv &= s_fn[hi];
-          any |= sv;
-          if (lane == hi) surv_mine = sv;
-        }
-        if (any == 0) continue;
-        const int k0 = c_j_first_k[j];
-        const int nrows = c_j_rows[j];
-        [[maybe_unused]] int ns_sizes = 0;   // sizes pass: the survivors in fo_list
-        if constexpr (MODE == kEnumSizes) ns_sizes = outer_list7(surv_mine, fo_list, lane);
-        if (!EMIT && !slow) {
-          const int ns = outer_list7(surv_mine, fo_list, lane);
-          if constexpr (GR) {
+      for (int hi = 0; hi < 8; hi++) {
+        uint32_t sv = ok[hi] & __brev(ok[7 - hi]);
+        if constexpr (FILTER) sv &= s_fn[hi];
+        any |= sv;
+        if (lane == hi) surv_mine = sv;
+      }
+      if (any == 0) continue;
+      const int k0 = c_j_first_k[j];
+      const int nrows = c_j_rows[j];
+      [[maybe_unused]] int ns_sizes = 0;   // sizes pass: the survivors in fo_list
+      if constexpr (MODE == kEnumSizes) ns_sizes = outer_list7(surv_mine, fo_list, lane);
+      if (!EMIT && !slow) {
+        const int ns = outer_list7(surv_mine, fo_list, lane);
+        if constexpr (GR) {
 #pragma unroll 1
-            for (int row = 0; row < nrows; row++) {
-              const int rd = depth7(d7, k0 + row);
-              if (rd > B) continue;
-              bool found = false;
-              for (int i0 = 0; i0 < ns && !found; i0 += 32) {
-                const bool have = i0 + lane < ns;
-                const int fo = have ? fo_list[i0 + lane] : 0;
-                uint32_t r1 = 0, r0 = 0;
+          for (int row = 0; row < nrows; row++) {
+            const int rd = depth7(d7, k0 + row);
+            if (rd > B) continue;
+            bool found = false;
+            for (int i0 = 0; i0 < ns && !found; i0 += 32) {
+              const bool have = i0 + lane < ns;
+              const int fo = have ? fo_list[i0 + lane] : 0;
+              uint32_t r1 = 0, r0 = 0;
 #pragma unroll
-                for (int u = 0; u < 8; u++) {
-                  if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
-                }
-                uint32_t hv[2][4], S, ov, bits[8], nz = 0;
-                bool hok[2][4];
-                middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
-                cube_union(hv, hok, S, ov, bits);
-#pragma unroll
-                for (int wd = 0; wd < 8; wd++) nz |= bits[wd] & s_fn[8 + wd];
-                found = __any_sync(kFull, have && nz != 0);
+              for (int u = 0; u < 8; u++) {
+                if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
               }
-              if (!found) continue;
-              tk.count++;
-              if (flt.hist_on && lane == 0) hist_add(rd, 1);
-              if (flt.grouping == kGroupTuple) {
-                done = true;   // the entry is the group
-                break;
-              }
-            }
-            continue;
-          }
-          for (int i0 = 0; i0 < ns; i0 += 32) {
-            const bool have = i0 + lane < ns;
-            const int fo = have ? fo_list[i0 + lane] : 0;
-            uint32_t r1 = 0, r0 = 0;
-#pragma unroll
-            for (int u = 0; u < 8; u++) {
-              if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
-            }
-            uint32_t c = 0;
-#pragma unroll 1
-            for (int row = 0; row < nrows; row++) {
-              int rd = 0;
-              if constexpr (FILTER) {
-                rd = depth7(d7, k0 + row);
-                if (rd > B) continue;
-              }
-              const uint32_t c_before = c;
-              uint32_t hv[2][4], S, ov, bits[8];
+              uint32_t hv[2][4], S, ov, bits[8], nz = 0;
               bool hok[2][4];
               middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
               cube_union(hv, hok, S, ov, bits);
-              if constexpr (FILTER) {
 #pragma unroll
-                for (int wd = 0; wd < 8; wd++) bits[wd] &= s_fn[8 + wd];
-              }
+              for (int wd = 0; wd < 8; wd++) nz |= bits[wd] & s_fn[8 + wd];
+              found = __any_sync(kFull, have && nz != 0);
+            }
+            if (!found) continue;
+            tk.count++;
+            if (flt.hist_on && lane == 0) hist_add(rd, 1);
+            if (flt.grouping == kGroupTuple) {
+              done = true;   // the entry is the group
+              break;
+            }
+          }
+          continue;
+        }
+        for (int i0 = 0; i0 < ns; i0 += 32) {
+          const bool have = i0 + lane < ns;
+          const int fo = have ? fo_list[i0 + lane] : 0;
+          uint32_t r1 = 0, r0 = 0;
 #pragma unroll
-              for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd]);
-              if constexpr (FILTER) {
-                if (flt.hist_on) {
-                  // rows differ in depth: each row's matches go to its own bin
-                  const uint32_t s = __reduce_add_sync(kFull, have ? c - c_before : 0u);
-                  if (lane == 0 && s != 0) hist_add(rd, s);
-                }
+          for (int u = 0; u < 8; u++) {
+            if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
+          }
+          uint32_t c = 0;
+#pragma unroll 1
+          for (int row = 0; row < nrows; row++) {
+            int rd = 0;
+            if constexpr (FILTER) {
+              rd = depth7(d7, k0 + row);
+              if (rd > B) continue;
+            }
+            const uint32_t c_before = c;
+            uint32_t hv[2][4], S, ov, bits[8];
+            bool hok[2][4];
+            middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
+            cube_union(hv, hok, S, ov, bits);
+            if constexpr (FILTER) {
+#pragma unroll
+              for (int wd = 0; wd < 8; wd++) bits[wd] &= s_fn[8 + wd];
+            }
+#pragma unroll
+            for (int wd = 0; wd < 8; wd++) c += __popc(bits[wd]);
+            if constexpr (FILTER) {
+              if (flt.hist_on) {
+                // rows differ in depth: each row's matches go to its own bin
+                const uint32_t s = __reduce_add_sync(kFull, have ? c - c_before : 0u);
+                if (lane == 0 && s != 0) hist_add(rd, s);
               }
             }
-            tk.count += __reduce_add_sync(kFull, have ? c : 0u);
+          }
+          tk.count += __reduce_add_sync(kFull, have ? c : 0u);
+        }
+      }
+#pragma unroll 1
+      for (int row = 0; (EMIT || slow) && row < nrows && !done; row++) {
+        const int k = k0 + row;
+        if (FILTER && depth7(d7, k) > B) continue;
+        if constexpr (MODE == kEnumSizes) {
+          if (sw.sizing) {
+            sw.size += row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
+            continue;
           }
         }
+        [[maybe_unused]] const uint32_t row_start = tk.count;
+        [[maybe_unused]] bool row_hit = false;   // grouped: the row's group is emitted
 #pragma unroll 1
-        for (int row = 0; (EMIT || slow) && row < nrows && !done; row++) {
-          const int k = k0 + row;
-          if (FILTER && depth7(d7, k) > B) continue;
-          if constexpr (MODE == kEnumSizes) {
-            if (sw.sizing) {
-              sw.size += row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
-              continue;
-            }
-          }
-          [[maybe_unused]] const uint32_t row_start = tk.count;
-          [[maybe_unused]] bool row_hit = false;   // grouped: the row's group is emitted
-#pragma unroll 1
-          for (int po = 0; po < 256 && !done; po++) {
-            const uint32_t fo = s_ord[0][po];
-            if (((__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u) == 0) continue;
-            uint32_t r1 = 0, r0 = 0;
+        for (int po = 0; po < 256 && !done; po++) {
+          const uint32_t fo = s_ord[0][po];
+          if (((__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u) == 0) continue;
+          uint32_t r1 = 0, r0 = 0;
 #pragma unroll
-            for (int u = 0; u < 8; u++) {
-              if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
-            }
-            uint32_t hv[2][4], S, ov;
-            bool hok[2][4];
-            middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
-            [[maybe_unused]] uint32_t AB[4] = {0, 0, 0, 0};
-            if (FILTER && slow) inner_cells7(r1, r0, c_row_b[k], AB);
-            const unsigned long long key_hi = (idx << 23) | ((uint64_t)k << 16) | ((uint64_t)po << 8);
+          for (int u = 0; u < 8; u++) {
+            if ((fo >> u) & 1) r1 |= W[u]; else r0 |= W[u];
+          }
+          uint32_t hv[2][4], S, ov;
+          bool hok[2][4];
+          middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
+          [[maybe_unused]] uint32_t AB[4] = {0, 0, 0, 0};
+          if (FILTER && slow) inner_cells7(r1, r0, c_row_b[k], AB);
+          const unsigned long long key_hi = (idx << 23) | ((uint64_t)k << 16) | ((uint64_t)po << 8);
 #pragma unroll 1
-            for (int w = 0; w < 8; w++) {
-              const uint32_t pm = 32u * w + lane;
-              const uint32_t fm = s_ord[1][pm];
-              bool hit = in_cubes(hv, hok, S, ov, fm);
-              if constexpr (FILTER) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
-              if constexpr (GR) {
-                // the group's record: the first hit of the row
-                const uint32_t bal = __ballot_sync(kFull, hit);
-                if (bal == 0) continue;
-                hit = hit && (bal & lanemask_lt()) == 0;
-                row_hit = true;
+          for (int w = 0; w < 8; w++) {
+            const uint32_t pm = 32u * w + lane;
+            const uint32_t fm = s_ord[1][pm];
+            bool hit = in_cubes(hv, hok, S, ov, fm);
+            if constexpr (FILTER) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
+            if constexpr (GR) {
+              // the group's record: the first hit of the row
+              const uint32_t bal = __ballot_sync(kFull, hit);
+              if (bal == 0) continue;
+              hit = hit && (bal & lanemask_lt()) == 0;
+              row_hit = true;
+            }
+            if constexpr (MODE == kEnumSizes) {
+              // the row's group; a wanted tuple group goes on through the entry's later rows
+              // and takes its step after them
+              if (size_wanted(tk)) {
+                sw.size = row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
+                sw.sizing = flt.grouping == kGroupTuple;
               }
-              if constexpr (MODE == kEnumSizes) {
-                // the row's group; a wanted tuple group goes on through the entry's later rows
-                // and takes its step after them
-                if (size_wanted(tk)) {
-                  sw.size = row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
-                  sw.sizing = flt.grouping == kGroupTuple;
-                }
-                if (!sw.sizing) {
-                  done = emit_step<MODE>(hit, tk, [&](unsigned long long s) {
-                    ectl->sizes[s] = sw.size;
-                  });
-                }
-              } else {
-                done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
-                  write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
+              if (!sw.sizing) {
+                done = emit_step<MODE>(hit, tk, [&](unsigned long long s) {
+                  ectl->sizes[s] = sw.size;
                 });
               }
-              if (GR && row_hit) break;
+            } else {
+              done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
+                write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
+              });
             }
             if (GR && row_hit) break;
           }
-          if constexpr (FILTER && MODE == kEnumCount) {
-            // the slow count pass: this row's matches to its depth's bin
-            if (flt.hist_on && lane == 0 && tk.count != row_start) {
-              hist_add(depth7(d7, k), tk.count - row_start);
-            }
-          }
-          if constexpr (GR) {
-            // the entry is the group (unless the sizes pass is summing its rows)
-            if (row_hit && flt.grouping == kGroupTuple && !sw.sizing) done = true;
+          if (GR && row_hit) break;
+        }
+        if constexpr (FILTER && MODE == kEnumCount) {
+          // the slow count pass: this row's matches to its depth's bin
+          if (flt.hist_on && lane == 0 && tk.count != row_start) {
+            hist_add(depth7(d7, k), tk.count - row_start);
           }
         }
-      }
-      if constexpr (MODE == kEnumSizes) {
-        if (sw.sizing) {
-          emit_step<MODE>(lane == 0, tk, [&](unsigned long long s) { ectl->sizes[s] = sw.size; });
+        if constexpr (GR) {
+          // the entry is the group (unless the sizes pass is summing its rows)
+          if (row_hit && flt.grouping == kGroupTuple && !sw.sizing) done = true;
         }
       }
     }
-  });
+    if constexpr (MODE == kEnumSizes) {
+      if (sw.sizing) {
+        emit_step<MODE>(lane == 0, tk, [&](unsigned long long s) { ectl->sizes[s] = sw.size; });
+      }
+    }
+  };
+
+  if constexpr (SRC == kSrcList) {
+    enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
+        [&](unsigned long long t, EnumTicket &tk, unsigned long long &) {
+      const uint64_t idx = t * (uint64_t)nparts + (uint64_t)part;
+      if (idx < list_count) {
+        const uint64_t cur = list[idx];
+        int g[7];
+#pragma unroll
+        for (int i = 0; i < 7; i++) g[i] = (int)((cur >> (9 * (6 - i))) & 0x1ffu);
+        tuple7(g, idx, tk);
+      }
+    });
+  } else {
+    // per prefix cell (first prefix gate = most significant bit): its masked positions, NW words
+    uint32_t *cells = smem + NW * npad + warp * (kPrefix7Cells * NW);
+    const uint32_t inmask = prob->inmask;
+    const uint64_t prefixes = c_binom[n - 1][6];
+    enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
+        [&](unsigned long long t, EnumTicket &tk, unsigned long long &feasible) {
+      const uint64_t dealt = dealt_item(t, part, nparts);   // as k_enum5 deals its prefixes
+      if (dealt >= prefixes) return;
+      int pre[6];
+      uint64_t base_rank;   // rank of (pre, pre[5] + 1)
+      unrank_prefix_warp<6, 7, true>(dealt, n, pre, base_rank, lane);
+      bool rejected = false;
+#pragma unroll
+      for (int i = 0; i < 6; i++) rejected |= (pre[i] < 8) && ((inmask >> pre[i]) & 1u);
+      int pre_deep = 0;   // prefix gates of depth B - 1 (at most one gate of a match may have it)
+      if constexpr (FILTER) {
+#pragma unroll
+        for (int i = 0; i < 6; i++) {
+          rejected |= s_dep[pre[i]] >= B;
+          pre_deep += s_dep[pre[i]] >= B - 1;
+        }
+        rejected |= pre_deep > 1;
+      }
+      if (rejected) return;
+      uint32_t mixed[2];   // prefix cells 32 * h + lane with a masked 1 and a masked 0
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int cell = 32 * h + lane;
+        uint32_t ones = 0, zeros = 0;
+#pragma unroll
+        for (int w = 0; w < NW; w++) {
+          uint32_t tt = M[w];
+#pragma unroll
+          for (int i = 0; i < 6; i++) {
+            const uint32_t tv = s_tabs[w * npad + pre[i]];
+            tt &= ((cell >> (5 - i)) & 1) ? tv : ~tv;
+          }
+          cells[cell * NW + w] = tt;
+          ones |= tt & T[w];
+          zeros |= tt & ~T[w];
+        }
+        mixed[h] = __ballot_sync(kFull, ones != 0 && zeros != 0);
+      }
+      __syncwarp();
+      const int last = pre[5];
+      bool over = false;
+      for (int g0 = last + 1; g0 < n && !over; g0 += 32) {
+        // lane's last gate: it must split every mixed prefix cell into a part without a masked 0
+        // and a part without a masked 1 (k_sweep's test)
+        const int gl = g0 + lane;
+        bool alive = gl < n && !(gl < 8 && ((inmask >> gl) & 1u));
+        if constexpr (FILTER) {
+          if (alive) {
+            const int dg = s_dep[gl];
+            alive = dg < B && pre_deep + (dg >= B - 1) <= 1;
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          for (uint32_t mc = mixed[h]; mc != 0 && alive; mc &= mc - 1) {
+            const int cj = 32 * h + __ffs(mc) - 1;
+            uint32_t a1 = 0, b1 = 0, a0 = 0, b0 = 0;
+#pragma unroll
+            for (int w = 0; w < NW; w++) {
+              const uint32_t tg = s_tabs[w * npad + gl], tt = cells[cj * NW + w];
+              const uint32_t c1 = tt & T[w], c0 = tt & ~T[w];
+              a1 |= c1 & tg; b1 |= c0 & tg;
+              a0 |= c1 & ~tg; b0 |= c0 & ~tg;
+            }
+            if ((a1 && b1) || (a0 && b0)) alive = false;
+          }
+        }
+        for (uint32_t fb = __ballot_sync(kFull, alive); fb != 0 && !over; fb &= fb - 1) {
+          const int src = __ffs(fb) - 1;
+          const int g[7] = {pre[0], pre[1], pre[2], pre[3], pre[4], pre[5], g0 + src};
+          feasible++;
+          tuple7(g, base_rank + (uint64_t)(g0 + src - last - 1), tk);
+          over = ticket_over<MODE>(tk);
+        }
+      }
+    });
+  }
   flush_hist<MODE, FORM>(flt);
 }
 
@@ -3665,8 +3787,21 @@ __global__ void __launch_bounds__(kThreads) k_enum7(const DevProblem *__restrict
     const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
-  enum7_body<NW, MODE, FORM>(prob, ectl, ord, list, list_count, counts, offsets, out, max_out,
-      t_begin, t_end, part, nparts, tab, flt);
+  enum7_body<NW, MODE, FORM, kSrcList>(prob, ectl, ord, list, list_count, counts, offsets, out,
+      max_out, t_begin, t_end, part, nparts, tab, flt);
+}
+
+// The whole-space form (kSrcWhole).  Dynamic shared memory: the tables, then per warp the prefix
+// cells (kPrefix7Cells * NW words), so that with the filter block's static shared memory every
+// form stays within the 48 KB a launch may use without opting in.
+template <int NW, int MODE, int FORM>
+__global__ void __launch_bounds__(kThreads) k_enum7_all(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
+  enum7_body<NW, MODE, FORM, kSrcWhole>(prob, ectl, ord, nullptr, 0u, counts, offsets, out,
+      max_out, t_begin, t_end, part, nparts, tab, flt);
 }
 
 

@@ -250,6 +250,13 @@ class DistributedLutSearch:
             lambda k, part, nparts: self.engine.enumerate7(outer, middle, k, True, part, nparts),
             max_matches, list_length=count)
 
+    def enumerate7_all(self, outer, middle, max_matches):
+        """The same over every 7-combination (LutEngine.enumerate7_all): no list is installed, and
+        `feasible` is the whole's feasible combinations, summed over the ranks."""
+        return self._enumerate(
+            lambda k, part, nparts: self.engine.enumerate7_all(outer, middle, k, True, part, nparts),
+            max_matches)
+
     def fetch_matches(self, first, count):
         """The whole's matches at ranks first .. min(first + count, total) - 1 (the last
         enumerate* call's), the same on every rank."""

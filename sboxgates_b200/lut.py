@@ -15,7 +15,8 @@ import numpy as np
 from . import native
 from .native import (SbgResult, SbgJob, SbgNodeResult, NativeLibraryError, SBG_KEY_NONE,
                      SBG_LIST_CAP, SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7, MATCH_DTYPE,
-                     SBG_ENUM_MAX_MATCHES, SBG_MAX_GATES, SBG_MAX_DEPTH, SBG_DEPTH_BINS)
+                     SBG_ENUM_MAX_MATCHES, SBG_MAX_GATES, SBG_MAX_DEPTH, SBG_DEPTH_BINS,
+                     SBG_ENUM7_ALL_MAX_GATES)
 
 NO_GATE = 0xFFFF  # state.h:30
 
@@ -400,6 +401,15 @@ class LutEngine:
         return self._enumerate(self.lib.sbg_enum7, [outer_order, middle_order], max_matches, count,
                                part, nparts)
 
+    def enumerate7_all(self, outer_order, middle_order, max_matches, count=True, part=0,
+                       nparts=1):
+        """The same over every 7-combination of the problem instead of the phase-1 list
+        (sbg_enum7_all, 7 <= n <= SBG_ENUM7_ALL_MAX_GATES): keys rank << 23 | k << 16 | po << 8 | pm
+        with the combination's rank among all C(n, 7), records as enumerate7's, and `feasible` =
+        the feasible combinations, which the list's cap hides.  The installed list stays."""
+        return self._enumerate(self.lib.sbg_enum7_all, [outer_order, middle_order], max_matches,
+                               count, part, nparts)
+
     def enumerate3(self, gate_order, max_matches, count=True, part=0, nparts=1):
         """Every match of lut_search's 3-LUT scan over `gate_order` (a permutation of the current
         problem's gates): the feasible position triples, keys i << 18 | k << 9 | m."""
@@ -637,7 +647,7 @@ def match_depth(record, depth):
     raise ValueError("not a match record (width %d)" % width)
 
 
-def shallowest_matches(engine, width, orders, depth, max_matches):
+def shallowest_matches(engine, width, orders, depth, max_matches, whole=False):
     """The shallowest realisations of the current problem by the width-3, 5 or 7 enumeration:
     one count with the loosest bound gives the depth histogram, a second counts at its first
     non-empty depth.  `orders` are the enumerate call's order arguments: (gate_order,),
@@ -646,10 +656,14 @@ def shallowest_matches(engine, width, orders, depth, max_matches):
     depth, so the engine's cursor serves the shallowest set (fetch_matches, pick_matches).
     `engine` is a LutEngine or a DistributedLutSearch.  Use it with no grouping or with "shape"
     grouping: under "tuple" grouping a gate set is binned at the depth of its first match, which
-    need not be its shallowest."""
+    need not be its shallowest.  whole=True (width 7 only) searches every 7-combination
+    (enumerate7_all) instead of the phase-1 list, so the result is the state's shallowest 7-LUT
+    realisation, not the list's."""
     if width not in (3, 5, 7):
         raise ValueError("width must be 3, 5 or 7")
-    run = getattr(engine, "enumerate%d" % width)
+    if whole and width != 7:
+        raise ValueError("whole=True applies to width 7 only")
+    run = getattr(engine, "enumerate7_all" if whole else "enumerate%d" % width)
     engine.set_depth_filter(depth, SBG_DEPTH_BINS - 1)
     run(*orders, 0)
     hist = engine.depth_counts()
@@ -886,7 +900,8 @@ def decode_key5(key):
 
 
 def decode_key7(key):
-    """7-LUT key -> (list index, ordering k, outer position, middle position)."""
+    """7-LUT key -> (list index, or the combination's rank for enumerate7_all, ordering k, outer
+    position, middle position)."""
     key = int(key)
     return key >> 23, (key >> 16) & 0x7F, (key >> 8) & 0xFF, key & 0xFF
 
@@ -909,6 +924,17 @@ def enumerate_7lut(engine, tables, target, mask, inbits, outer, middle, max_matc
         raise ValueError("search_7lut needs at least 7 gates (lut.c:259)")
     engine.load(tables, target, mask, inbits)
     return engine.enumerate7(outer, middle, max_matches, count, part, nparts)
+
+
+def enumerate_7lut_all(engine, tables, target, mask, inbits, outer, middle, max_matches,
+                       count=True, part=0, nparts=1):
+    """The same over every feasible 7-combination of the state, not only the phase-1 list
+    (LutEngine.enumerate7_all; at most SBG_ENUM7_ALL_MAX_GATES gates)."""
+    if not 7 <= len(tables) <= SBG_ENUM7_ALL_MAX_GATES:
+        raise ValueError("the whole-space 7-LUT enumeration takes 7..%d gates"
+                         % SBG_ENUM7_ALL_MAX_GATES)
+    engine.load(tables, target, mask, inbits)
+    return engine.enumerate7_all(outer, middle, max_matches, count, part, nparts)
 
 
 def enumerate_3lut(engine, tables, target, mask, inbits, gate_order, max_matches, count=True,

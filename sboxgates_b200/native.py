@@ -54,6 +54,7 @@ MATCH_DTYPE = np.dtype([("key", "<u8"), ("gates", "<u2", (7,)), ("func_outer", "
                         ("func_middle", "u1"), ("func_inner", "u1"), ("inner_seen", "u1"),
                         ("width", "u1"), ("pad", "u1", (5,))])
 SBG_ENUM_MAX_MATCHES = 1 << 24
+SBG_ENUM7_ALL_MAX_GATES = 64   # largest n of the whole-space 7-LUT enumeration (sbg_enum7_all)
 SBG_MAX_GATES = 500
 SBG_MAX_DEPTH = 1020      # largest gate depth of a depth filter
 SBG_DEPTH_BINS = 1024     # bins of the depth histogram
@@ -108,6 +109,8 @@ SIGNATURES = {
                             u64p]),
     "sbg_enum7": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, C.c_uint64, C.c_void_p, u64p,
                             u64p, u64p]),
+    "sbg_enum7_all": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, C.c_uint64, C.c_void_p,
+                                u64p, u64p, u64p]),
     "sbg_enum3": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint16), C.c_uint64,
                             C.c_void_p, u64p, u64p, u64p]),
     "sbg_enum_fetch": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, u64p]),
