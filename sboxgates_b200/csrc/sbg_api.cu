@@ -433,8 +433,9 @@ auto with_nw(int nw, F &&f) {
 
 // f(form_c) with the enumeration kernel form (EnumForm) as the compile-time constant
 // decltype(form_c)::value.  Width 3 has no grouped form (take_filter never picks it there).  The
-// sizes pass (MODE kEnumSizes) runs on grouped cursors of widths 5 and 7 only, so it has the grouped
-// form alone.
+// count, range and pick passes (MODE kEnumCount, kEnumRange, kEnumPick) run in every form of the
+// width; the sizes pass (kEnumSizes) runs on grouped cursors of widths 5 and 7 only, so it has the
+// grouped form alone.
 template <int WIDTH, int MODE, class F>
 auto with_form(int form, F &&f) {
   static_assert(MODE != kEnumSizes || WIDTH != 3, "width 3 has no sizes pass");
@@ -1586,7 +1587,7 @@ int copy_matches(sbg_handle *h, sbg_lane &L, sbg_match *out, uint64_t n) {
   return SBG_OK;
 }
 
-// One enumeration pass (MODE: count, first-K, range or pick emit, or sizes) of width 3, 5 or 7 over
+// One enumeration pass (MODE: count, range or pick emit, or sizes) of width 3, 5 or 7 over
 // tickets [a, b) of the lane's problem (pick and sizes: entries [a, b) of the ticket list in
 // EnumCtl::sel).
 template <int WIDTH, int MODE>
@@ -1689,6 +1690,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   const uint64_t room = std::max<uint64_t>(tickets, 1);
   if ((rc = E.d_ecount.grow(h, L.stream, room)) != SBG_OK) return rc;
   if ((rc = E.d_eoffset.grow(h, L.stream, room)) != SBG_OK) return rc;
+  // also sets EnumCtl::sel.lo = 0, which the first-K range pass below relies on
   SBG_CUDA(h, cudaMemsetAsync(E.d_ectl.p, 0, sizeof(EnumCtl), L.stream));
   if (in.form != kFormPlain) {
     if ((rc = E.d_ehist.grow(h, L.stream, (uint64_t)kDepthBins)) != SBG_OK) return rc;
@@ -1718,7 +1720,9 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   const uint64_t emit = std::min<uint64_t>(max_matches, ec.carry);
   if (emit > 0) {
     if ((rc = E.d_ematch.grow(h, L.stream, emit)) != SBG_OK) return rc;
-    if ((rc = launch_enum<WIDTH, kEnumFirst>(h, L, in, part, nparts, emit, 0, done)) != SBG_OK) return rc;
+    // ranks [0, emit): the range pass with sel.lo = 0 from the memset above (not emit_sel, which
+    // needs the cursor a count-free call does not set)
+    if ((rc = launch_enum<WIDTH, kEnumRange>(h, L, in, part, nparts, emit, 0, done)) != SBG_OK) return rc;
     if ((rc = copy_matches(h, L, out, emit)) != SBG_OK) return rc;
   }
   *n_out = emit;

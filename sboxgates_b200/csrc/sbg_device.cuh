@@ -2691,8 +2691,8 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
 // (sbg_enum_fetch / sbg_enum_pick): the emit pass of the same sweep, run over the tickets that hold
 // the wanted ranks only (k_enum_locate finds them).  The pass's mode (template parameter MODE):
 //   kEnumCount  the count pass;
-//   kEnumFirst  the first K (max_out = K), ranks [0, K) to out[rank];
-//   kEnumRange  ranks [sel.lo, max_out) to out[rank - sel.lo];
+//   kEnumRange  ranks [sel.lo, max_out) to out[rank - sel.lo]; with sel.lo = 0 and max_out = K,
+//               the first K;
 //   kEnumPick   one warp per ticket of sel.tickets, writing each rank of its slice of sel.ranks to
 //               out[sel.slots[...]] (duplicate ranks: every slot that asked for it).
 //   kEnumSizes  pick's walk over the same selection, grouped form only: at a requested group it
@@ -2700,13 +2700,13 @@ __global__ void __launch_bounds__(kThreads) k_decomp7(const DevProblem *__restri
 //               record (see "grouping" below).
 // The kernels keep one parameter list for all modes; sel reaches the range, pick and sizes forms in
 // the lane's EnumCtl block.
-enum EnumMode : int { kEnumCount = 0, kEnumFirst = 1, kEnumRange = 2, kEnumPick = 3, kEnumSizes = 4 };
+enum EnumMode : int { kEnumCount = 0, kEnumRange = 2, kEnumPick = 3, kEnumSizes = 4 };
 
 // The passes that run over pick's selection (EnumSel::ranks, slots, tickets, first).
 __host__ __device__ constexpr bool by_rank(int mode) { return mode == kEnumPick || mode == kEnumSizes; }
 
 struct EnumSel {
-  unsigned long long lo;                  // kEnumRange: first rank of the window
+  unsigned long long lo;                  // kEnumRange: first rank of the window (0: the first K)
   const unsigned long long *ranks;        // pick / sizes: the requested ranks, ascending, duplicates kept
   const unsigned int *slots;              //   the output slot of each of them
   const unsigned long long *tickets;      //   the distinct tickets holding them, ascending
@@ -2716,13 +2716,13 @@ struct EnumSel {
 // Where a pass stands in the ticket a warp sweeps (warp-uniform).
 struct EnumTicket {
   EnumSel sel;                   // range / pick: what to emit
-  unsigned long long max_out;    // first / range: the end of the wanted ranks
+  unsigned long long max_out;    // range: the end of the wanted ranks
   unsigned long long base;       // emit: rank of the ticket's first match
   uint32_t count;                // matches met so far (count pass: the ticket's count)
   unsigned int req, req_end;     // pick / sizes: the ticket's requests not yet met
 };
 
-// Whether the ticket has nothing more to emit: the first / range pass has reached max_out, the pick
+// Whether the ticket has nothing more to emit: the range pass has reached max_out, the pick
 // or sizes pass has met the ticket's last request (never in the count pass).
 template <int MODE>
 __device__ __forceinline__ bool ticket_over(const EnumTicket &tk) {
@@ -2746,9 +2746,8 @@ __device__ __forceinline__ bool emit_step(bool hit, EnumTicket &tk, Write write)
       if (r >= step_end) break;
       if (hit && at == r) write((unsigned long long)tk.sel.slots[tk.req]);
     }
-  } else if (MODE != kEnumCount && hit && at < tk.max_out
-             && (MODE != kEnumRange || at >= tk.sel.lo)) {
-    write(MODE == kEnumRange ? at - tk.sel.lo : at);
+  } else if (MODE == kEnumRange && hit && at < tk.max_out && at >= tk.sel.lo) {
+    write(at - tk.sel.lo);
   }
   tk.count += __popc(bal);
   return ticket_over<MODE>(tk);
@@ -2786,7 +2785,8 @@ struct EnumCtl {
   unsigned long long total;     // matches counted so far (all windows of the call)
   unsigned long long feasible;  // 5-LUT: feasible tuples met
   unsigned long long carry;     // k_enum_scan: matches in front of the next window
-  EnumSel sel;                  // range / pick emit: what to emit (set by the host before the pass)
+  EnumSel sel;                  // range / pick emit: what to emit (set by the host before the pass;
+                                //   the first K reads the zeros run_enum clears it to)
   unsigned long long gtotal;    // k_enum_globalize: the whole's total
   unsigned int gbad;            //   1 if the share's own row of block sums differs from its own
   unsigned long long *sizes;    // sizes pass: the group sizes, indexed by sel.slots
@@ -2802,7 +2802,7 @@ __device__ __forceinline__ void enum_tickets(EnumCtl *__restrict__ ectl,
     uint32_t *__restrict__ counts, const unsigned long long *__restrict__ offsets,
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, Sweep sweep) {
   EnumTicket tk = {};
-  if (MODE == kEnumRange || by_rank(MODE)) tk.sel = ectl->sel;
+  if (MODE != kEnumCount) tk.sel = ectl->sel;
   tk.max_out = max_out;
   const int lane = threadIdx.x & 31;
   const unsigned long long nwarps = (unsigned long long)gridDim.x * kWarpsPerCta;
