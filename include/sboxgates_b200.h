@@ -245,8 +245,12 @@ typedef struct {
   uint8_t func_inner;      /* 24: solved bits only; don't-care bits are 0 (3-LUT: the LUT) */
   uint8_t inner_seen;      /* 25: bit c set = inner cell c occurs under the mask */
   uint8_t width;           /* 26: 3, 5 or 7 */
-  uint8_t pad[5];          /* 27: 0 */
+  uint8_t shape;           /* 27: how a 7-LUT match wires its LUTs, SBG_SHAPE_TREE (every call but
+                              sbg_enum7_chain, and widths 3 and 5) or SBG_SHAPE_CHAIN */
+  uint8_t pad[4];          /* 28: 0 */
 } sbg_match;
+#define SBG_SHAPE_TREE 0    /* L3(L1(a,b,c), L2(d,e,f), g): search_7lut's wiring */
+#define SBG_SHAPE_CHAIN 1   /* L3(L2(L1(a,b,c), d, e), f, g) */
 #define SBG_ENUM_MAX_MATCHES (1u << 24)   /* largest max_matches of one call */
 
 /* Enumerates the matches of the current problem in this part's share of the work (part/nparts as
@@ -288,6 +292,25 @@ int sbg_enum7(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
 int sbg_enum7_all(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
     uint64_t *total, uint64_t *feasible);
+/* The 7-LUT realisations search_7lut never tries: three LUTs wired as a chain,
+   L3(L2(L1(a,b,c), d, e), f, g), over the 7-combinations sbg_enum7_all takes (no gate excluded by
+   inbits, check_n_lut_possible(7) passed; *feasible as there, under a depth filter the ones with a
+   chain row within the bound).  Row k = 6 j + q (sbg_chain_row): j = the lexicographic index of
+   L1's position triple among the 3-subsets of 0..6 of the ascending combination, q = that of the
+   pair {d, e} among the 2-subsets of the four other positions; f, g = the other two.  Inside each
+   LUT the inputs are in ascending position, the first the cell's high bit: L2's cells are
+   x1<<2 | d<<1 | e, L3's x2<<2 | f<<1 | g.  A match is (combination, k, po, pm) with L1 =
+   outer_order[po] and L2 = middle_order[pm] for which L3 is solvable without a random fill,
+   decided on the true gate tables.  Key rank<<24 | k<<16 | po<<8 | pm (rank as for sbg_enum7_all).
+   Record: width 7, shape SBG_SHAPE_CHAIN, gates a..g in row order, func_outer = L1, func_middle
+   = L2, func_inner / inner_seen = L3's solved bits and seen cells.  Depth (sbg_enum_set_depth)
+   1 + max(1 + max(1 + max(Da, Db, Dc), Dd, De), Df, Dg); function filter: outer = L1, middle = L2,
+   inner = L3; groupings: SBG_GROUP_SHAPE key >> 16, SBG_GROUP_TUPLE key >> 24.  Arguments, limits,
+   tickets, deal blocks, the cursor and its calls, the count buffers and the errors are those of
+   sbg_enum7_all; the call builds no list and leaves an installed one alone. */
+int sbg_enum7_chain(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
+    const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
+    uint64_t *total, uint64_t *feasible);
 /* The matches of lut_search's 3-LUT scan (lut.c:501-523) over the caller's shuffled gate order
    (n entries): the position triples i < k < m whose gates gate_order[i], gate_order[k],
    gate_order[m] pass check_n_lut_possible(3, ...) under the mask (get_lut_function then cannot
@@ -307,7 +330,8 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
     uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible);
 
 /* ---- matches at any rank: the enumeration cursor ---------------------------------------------- */
-/* The cursor is the last sbg_enum3 / sbg_enum5 / sbg_enum7 call on the handle that counted
+/* The cursor is the last sbg_enum3 / sbg_enum5 / sbg_enum7 / sbg_enum7_all / sbg_enum7_chain call
+   on the handle that counted
    (total != NULL; max_matches may be 0).  Ranks are positions in that call's share (part/nparts),
    in ascending key order: 0 .. total-1.  The device keeps what that count found (matches per
    ticket and where each ticket's matches start), so a fetch or pick emits the matches of the
@@ -330,7 +354,8 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
    A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
    a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT), a list
    entry (7-LUT, up to 70 * 65,536 matches) or a 6-gate prefix (sbg_enum7_all, up to n - 7
-   combinations of that many), so one deep rank can cost a whole ticket's sweep. */
+   combinations of that many; sbg_enum7_chain, of 210 * 65,536), so one deep rank can cost a whole
+   ticket's sweep. */
 /* The matches at ranks first .. min(first + count, total) - 1, in key order, to out[0..]; *n_out =
    how many (0 when first >= total).  count <= SBG_ENUM_MAX_MATCHES; out may be NULL iff count ==
    0. */
@@ -342,7 +367,8 @@ int sbg_enum_pick(sbg_handle *h, const uint64_t *ranks, uint64_t nranks, sbg_mat
 
 /* ---- global ranks across shares --------------------------------------------------------------- */
 /* A share's tickets fall into deal blocks, in the order the parts are dealt them: blocks of 16
-   position pairs (3-LUT), 3-gate prefixes (5-LUT) or 6-gate prefixes (sbg_enum7_all), local block j
+   position pairs (3-LUT), 3-gate prefixes (5-LUT) or 6-gate prefixes (sbg_enum7_all,
+   sbg_enum7_chain), local block j
    being the whole's block j * nparts + part; or single list entries (sbg_enum7), local entry t
    being list entry t * nparts + part.  The whole's blocks are in key order, so from every share's
    block sums each share can turn its ranks into ranks of the whole (a global cursor):
@@ -378,7 +404,8 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
    gates in reference order:
      3-LUT a,b,c:     1 + max(Da, Db, Dc);
      5-LUT a..e:      1 + max(1 + max(Da, Db, Dc), Dd, De)            (outer LUT over a,b,c);
-     7-LUT a..g:      1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df), Dg).
+     7-LUT a..g:      1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df), Dg);
+     7-LUT chain a..g: 1 + max(1 + max(1 + max(Da, Db, Dc), Dd, De), Df, Dg) (sbg_enum7_chain).
    Under a filter the matches of sbg_enum3 / sbg_enum5 / sbg_enum7 are exactly the unfiltered
    matches of depth <= max_depth: keys, key order and records are unchanged, only the set shrinks,
    and ranks are ranks within it.  The 7-LUT list is still the phase-1 list (the first
@@ -388,7 +415,7 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
    under, so fetch, pick, sbg_enum_block_sums and sbg_enum_set_global serve the filtered set.
    Searches (sbg_search*, sbg_search_node / batch, the *_part and finish calls) never read it. */
 #define SBG_MAX_DEPTH 1020     /* largest gate depth of a filter */
-#define SBG_DEPTH_BINS 1024    /* bins of the depth histogram (a match is at most 1,022 deep) */
+#define SBG_DEPTH_BINS 1024    /* bins of the depth histogram (a match is at most 1,023 deep) */
 /* Installs the filter (n depths, host memory) for the later sbg_enum3 / sbg_enum5 / sbg_enum7
    calls on the handle; depth == NULL clears it.  SBG_ERR_ARG, with the filter left as it was: n
    outside 1..SBG_MAX_GATES or a depth above SBG_MAX_DEPTH.  An sbg_enum* call whose problem does
@@ -437,7 +464,7 @@ int sbg_inner_table(const uint64_t *inner, uint8_t *out);
    grouping, sbg_enum3 / sbg_enum5 / sbg_enum7 enumerate groups of matches instead: the matches
    sharing a key prefix,
      SBG_GROUP_SHAPE: the gates and the ordering row (the wiring): 5-LUT key >> 8, 7-LUT key >> 16;
-     SBG_GROUP_TUPLE: the gate set: 5-LUT key >> 12, 7-LUT key >> 23.
+     SBG_GROUP_TUPLE: the gate set: 5-LUT key >> 12, 7-LUT key >> 23 (chain: key >> 24).
    A 3-LUT key already is its gate set and wiring, so at width 3 every grouping is the identity.
    The total is the number of groups holding at least one match (after the depth and function
    filters); each group has one record, its first match (smallest key), byte-identical to the
@@ -460,7 +487,8 @@ int sbg_enum_set_grouping(sbg_handle *h, int grouping);
    functions that survive for that (tuple, row); 5-LUT tuple: their sum over the tuple's rows within
    the depth bound; 7-LUT shape: the (outer, middle) pairs of that (entry, row) that pass the
    filters; 7-LUT tuple: their sum over the entry's rows.  Every size is at least 1 and at most
-   2,560 (5-LUT tuple) or 70 * 65,536 = 4,587,520 (7-LUT tuple); the sizes of all ranks add up to
+   2,560 (5-LUT tuple) or 70 * 65,536 = 4,587,520 (7-LUT tuple; chain: 65,536 for a shape and
+   210 * 65,536 for a tuple); the sizes of all ranks add up to
    the ungrouped total.  On an ungrouped cursor, or at width 3, every size is 1.  The ranks may
    come in any order and repeat.  A rank >= total: SBG_ERR_ARG and nothing written; ranks or sizes
    NULL with nranks > 0: SBG_ERR_ARG; no cursor: SBG_ERR_STATE.  Keeps the cursor, and changes
@@ -492,6 +520,8 @@ int sbg_weighted_tickets(int n, uint32_t group_pairs, uint32_t *out);
 
 /* Row k of the ordering tables (lut.c:189-229 for width 5, lut.c:396-415 for width 7). */
 int sbg_ordering_row(int width, int k, int *row);
+/* Chain row k < 210 of sbg_enum7_chain: the seven positions in record order a..g. */
+int sbg_chain_row(int k, int *row);
 /* Closed form of get_lut_function without the random fill (lut.c:79-103): returns 1 and the
    solved function / seen mask, or 0 on conflict. */
 int sbg_solve_inner(const uint64_t *in1, const uint64_t *in2, const uint64_t *in3,

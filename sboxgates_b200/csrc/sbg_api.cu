@@ -25,6 +25,7 @@ namespace {
 
 uint64_t h_binom[501][8];
 int h_rows7[70][7];
+int h_rows7c[210][7];
 int h_rows5[10][5];
 bool g_tables_ready = false;
 
@@ -69,6 +70,23 @@ void build_host_tables() {
       h_rows7[k][3] = mid[0]; h_rows7[k][4] = mid[1]; h_rows7[k][5] = mid[2];
       h_rows7[k][6] = rest[skip];
       k++;
+    }
+  }
+  // chain rows (sbg_chain_row): k = 6 j + q, j = the outer triple's lexicographic index, q = that
+  // of the pair {d, e} among the four other positions; f, g = the other two, ascending.
+  k = 0;
+  for (int a = 0; a < 7; a++) for (int b = a + 1; b < 7; b++) for (int c = b + 1; c < 7; c++) {
+    int rest[4], r = 0;
+    for (int i = 0; i < 7; i++) {
+      if (i != a && i != b && i != c) rest[r++] = i;
+    }
+    for (int d = 0; d < 4; d++) for (int e = d + 1; e < 4; e++) {
+      int *row = h_rows7c[k++];
+      row[0] = a; row[1] = b; row[2] = c; row[3] = rest[d]; row[4] = rest[e];
+      int w = 5;
+      for (int i = 0; i < 4; i++) {
+        if (i != d && i != e) row[w++] = rest[i];
+      }
     }
   }
   g_tables_ready = true;
@@ -193,13 +211,15 @@ struct EnumBuffers {
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
 // (widths 5 and 7) or the gate order (width 3), the kernel form (EnumForm), the 7-LUT ticket source
-// (Enum7Source; kSrcList at the other widths) and, for the filtered and grouped forms, the filter
-// block (take_filter; its histogram pointer is the lane's, set at launch).
+// (Enum7Source; kSrcList at the other widths), the 7-LUT shape (Enum7Shape; the chain with kSrcWhole
+// only) and, for the filtered and grouped forms, the filter block (take_filter; its histogram
+// pointer is the lane's, set at launch).
 struct EnumInputs {
   EnumOrders ord;
   EnumGateOrder gates;
   int form;
   int source;
+  int shape = kShapeTree;
   EnumFilter filter;
 };
 
@@ -359,7 +379,7 @@ size_t decomp_smem(int n) {
   return sizeof(uint32_t) * (size_t)(NW * npad);
 }
 
-// k_enum7_all: the tables and each warp's prefix cells.
+// k_enum7_all and k_enum7_chain: the tables and each warp's prefix cells.
 template <int NW>
 size_t enum7_all_smem(int n) {
   return decomp_smem<NW>(n) + sizeof(uint32_t) * (size_t)(kWarpsPerCta * kPrefix7Cells * NW);
@@ -1560,7 +1580,8 @@ static_assert(sizeof(sbg_match) == 32 && sizeof(DevMatch) == sizeof(sbg_match)
     && offsetof(sbg_match, gates) == offsetof(DevMatch, gates)
     && offsetof(sbg_match, func_outer) == offsetof(DevMatch, func_outer)
     && offsetof(sbg_match, inner_seen) == offsetof(DevMatch, inner_seen)
-    && offsetof(sbg_match, width) == offsetof(DevMatch, width), "sbg_match and DevMatch agree");
+    && offsetof(sbg_match, width) == offsetof(DevMatch, width)
+    && offsetof(sbg_match, shape) == offsetof(DevMatch, pad), "sbg_match and DevMatch agree");
 // The largest enumeration form, the filtered k_enum3: the gate order and the filter block, plus at
 // most 128 bytes of pointers and scalars, within the 4 KB kernel-parameter limit.
 static_assert(sizeof(EnumGateOrder) + sizeof(EnumFilter) + 128 <= 4096,
@@ -1623,6 +1644,11 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
             E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, h->d_tab.p,
             flt);
       } else {
+        if (in.shape == kShapeChain) {
+          return run(k_enum7_chain<NW, MODE, FORM>, enum7_all_smem<NW>(n), prob, E.d_ectl.p,
+              in.ord, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts,
+              h->d_tab.p, flt);
+        }
         if (in.source == kSrcWhole) {
           return run(k_enum7_all<NW, MODE, FORM>, enum7_all_smem<NW>(n), prob, E.d_ectl.p,
               in.ord, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts,
@@ -1655,7 +1681,7 @@ unsigned int enum_block_size(int width, int source) {
   return width == 7 && source == kSrcList ? 1u : (unsigned)kDeal;
 }
 
-// sbg_enum3 / sbg_enum5 / sbg_enum7 / sbg_enum7_all once their arguments are checked.  Lane 0
+// sbg_enum3 / sbg_enum5 / sbg_enum7 / sbg_enum7_all / sbg_enum7_chain once their arguments are checked.  Lane 0
 // takes the current problem slot, and k_begin (flags, begin_in) brings its problem block up to date;
 // a 7-LUT enumeration over the list without an installed one runs phase 1 instead, which does that
 // and installs the list.  Then the part's tickets are counted (in windows when only the first
@@ -2075,6 +2101,13 @@ int sbg_ordering_row(int width, int k, int *row) {
   return SBG_ERR_ARG;
 }
 
+int sbg_chain_row(int k, int *row) {
+  build_host_tables();
+  if (row == nullptr || k < 0 || k >= 210) return SBG_ERR_ARG;
+  for (int i = 0; i < 7; i++) row[i] = h_rows7c[k][i];
+  return SBG_OK;
+}
+
 void sbg_lut_table(uint8_t func, const uint64_t *in1, const uint64_t *in2, const uint64_t *in3,
     uint64_t *out) {
   for (int v = 0; v < 4; v++) {
@@ -2237,6 +2270,23 @@ int sbg_create(sbg_handle **out, int device) {
       return fail(h, SBG_ERR_STATE, "internal: %d outer triples (expected 25)", nj);
     }
     memcpy(host_tab->src7, src7, sizeof(src7));
+    // the chain's other 10 outer triples (positions 2..6), in src7's layout
+    for (int j = 0; j < 10; j++) {
+      const int *o = h_rows7c[6 * (25 + j)];
+      for (int lane = 0; lane < 32; lane++) {
+        const int u0 = lane >> 4, v4 = lane & 15;
+        uint32_t packed = 0;
+        for (int t4 = 0; t4 < 4; t4++) {
+          int c = 0;
+          c |= ((t4 >> 1) & 1) << cb[o[0]];
+          c |= (t4 & 1) << cb[o[1]];
+          c |= u0 << cb[o[2]];
+          for (int m = 0; m < 4; m++) c |= ((v4 >> (3 - m)) & 1) << cb[o[3 + m]];
+          packed |= (uint32_t)c << (8 * t4);
+        }
+        host_tab->src7x[j][lane] = packed;
+      }
+    }
     // minpos3 entries by number of unconstrained bits (k_begin)
     {
       int fill = 0;
@@ -2275,6 +2325,9 @@ int sbg_create(sbg_handle **out, int device) {
     for (int k = 0; k < 70; k++) for (int i = 0; i < 7; i++) rows7[k][i] = (uint8_t)h_rows7[k][i];
     SBG_CUDA(h, cudaMemcpyToSymbol(c_rows5, rows5, sizeof(rows5)));
     SBG_CUDA(h, cudaMemcpyToSymbol(c_rows7, rows7, sizeof(rows7)));
+    uint8_t rows7c[210][7];
+    for (int k = 0; k < 210; k++) for (int i = 0; i < 7; i++) rows7c[k][i] = (uint8_t)h_rows7c[k][i];
+    SBG_CUDA(h, cudaMemcpyToSymbol(c_rows7c, rows7c, sizeof(rows7c)));
   }
 
   if ((rc = h->d_slots.grow(h, h->lane[0].stream, kSlots)) != SBG_OK) return rc;
@@ -2887,6 +2940,30 @@ int sbg_enum7_all(sbg_handle *h, int part, int nparts, const uint8_t *outer_orde
   if ((rc = take_filter(h, 7, in7)) != SBG_OK) return rc;
   // no list: only bring the problem block up to date, so an installed list and its control words
   // stay as they are
+  return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
+      total, feasible);
+}
+
+int sbg_enum7_chain(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
+    const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
+    uint64_t *total, uint64_t *feasible) {
+  int rc;
+  if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
+  const int n = cur(h).n;
+  if (n < 7 || n > SBG_ENUM7_ALL_MAX_GATES) {
+    return fail(h, SBG_ERR_ARG, "the 7-LUT chain enumeration needs 7 <= n <= %d, not %d",
+        SBG_ENUM7_ALL_MAX_GATES, n);
+  }
+  if (!valid_order(outer_order) || !valid_order(middle_order)) {
+    return fail(h, SBG_ERR_ARG, "function order is not a permutation");
+  }
+  EnumInputs in7;
+  memcpy(in7.ord.order[0], outer_order, 256);
+  memcpy(in7.ord.order[1], middle_order, 256);
+  in7.source = kSrcWhole;
+  in7.shape = kShapeChain;
+  if ((rc = take_filter(h, 7, in7)) != SBG_OK) return rc;
+  // as sbg_enum7_all: no list is built or touched
   return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
       total, feasible);
 }

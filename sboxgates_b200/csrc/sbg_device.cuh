@@ -115,6 +115,10 @@ struct DevParams7 {
   uint8_t minpos3[kMinpos3 + 3];   // device-built; not part of the upload
 };
 
+// How a 7-LUT match wires its three LUTs (SBG_SHAPE_TREE, SBG_SHAPE_CHAIN): the tree
+// L3(L1(a,b,c), L2(d,e,f), g) of search_7lut, or the chain L3(L2(L1(a,b,c), d, e), f, g).
+enum Enum7Shape : int { kShapeTree = 0, kShapeChain = 1 };
+
 // Lane-indexed lookup tables live in global memory (coalesced, L1-resident): a constant-memory load
 // whose address differs per lane is replayed once per distinct address.
 struct DevTables {
@@ -125,6 +129,9 @@ struct DevTables {
   // else: 3^j of its lowest unconstrained bit j) << 16
   uint32_t m3_info[6561];
   int32_t m3_level[10];
+  // enum7 chain: src7's layout for the 10 outer triples inside positions 2..6 (triples 25..34 in
+  // lexicographic order; triples 0..24 are src7's)
+  uint32_t src7x[10][32];
 };
 
 __constant__ uint64_t c_binom[501][8];   // C(m, r), 0 <= m <= 500, 0 <= r <= 7
@@ -2358,15 +2365,17 @@ __device__ __forceinline__ void outer_ok7(const uint32_t *Hs, uint32_t srcw, int
 // / 0) and one ordering row (b = bit of v4 that is the g input): the middle functions that work are
 // the union, over the (c0, c1) with hok[0][c0] && hok[1][c1] && ((hv[0][c0] ^ hv[1][c1]) & ov) == 0,
 // of the cubes { fm : (fm & S) == (hv[0][c0] | hv[1][c1]) }.
-__device__ __forceinline__ void middle_cubes(uint32_t r1, uint32_t r0, int b, uint32_t (*hv)[4],
-    bool (*hok)[4], uint32_t &S, uint32_t &ov) {
-  // The four inner cells (x, g): A = middle patterns with a masked 1, B = with a masked 0
-  // (both compressed at once: they are the two halves of r1 / r0).
+// The cube combining of middle_cubes, from the four classes' cells cells(ci) (A = the middle cells
+// with a masked 1 in bits 0..7, B = with a masked 0 in bits 16..23): fm works iff in every class it
+// sends A and B to opposite values.
+template <class Cells>
+__device__ __forceinline__ void cubes_of_cells(Cells cells, uint32_t (*hv)[4], bool (*hok)[4],
+    uint32_t &S, uint32_t &ov) {
   // If both are non-empty, fm must send A to one value and B to the other: fm & S in {A, B}.
   uint32_t cs[4], ca[4], cb[4];
 #pragma unroll
   for (int ci = 0; ci < 4; ci++) {
-    const uint32_t AB = compress16x2((ci & 2) ? r1 : r0, b, ci & 1);
+    const uint32_t AB = cells(ci);
     const uint32_t A = AB & 0xffu, B = AB >> 16;
     const bool act = A != 0 && B != 0;
     cs[ci] = act ? (A | B) : 0u;   // inactive: empty support, both choices identical
@@ -2391,6 +2400,70 @@ __device__ __forceinline__ void middle_cubes(uint32_t r1, uint32_t r0, int b, ui
   }
   S = hs[0] | hs[1];
   ov = hs[0] & hs[1];
+}
+
+__device__ __forceinline__ void middle_cubes(uint32_t r1, uint32_t r0, int b, uint32_t (*hv)[4],
+    bool (*hok)[4], uint32_t &S, uint32_t &ov) {
+  // The four inner cells (x, g): A = middle patterns with a masked 1, B = with a masked 0
+  // (both compressed at once: they are the two halves of r1 / r0).
+  cubes_of_cells([&](int ci) { return compress16x2((ci & 2) ? r1 : r0, b, ci & 1); }, hv, hok, S,
+      ov);
+}
+
+// ---- the chain L3(L2(L1(a,b,c), d, e), f, g) --------------------------------------------------
+// Outer triple j (of all 35, lexicographic) leaves r1 / r0 over v4 = r0<<3 | r1<<2 | r2<<1 | r3,
+// the four other positions ascending, as for the tree.  Chain row q (k = 6 j + q) picks {d, e}
+// among them (the q-th pair in lexicographic order); {f, g} are the other two.  L2's cells are
+// x1<<2 | d<<1 | e and L3 decides per class (f, g), so middle_cubes' structure holds with the
+// classes (f, g) and the middle cells (x1, d, e) in place of the tree's (x1, g) and (d, e, f).
+
+// Exchanges index bits i < j of both 16-bit halves of r (sets over v4).
+__device__ __forceinline__ uint32_t swap_v4_bits(uint32_t r, int i, int j) {
+  const uint32_t has_i = i == 0 ? 0xAAAAu : i == 1 ? 0xCCCCu : 0xF0F0u;
+  const uint32_t has_j = j == 1 ? 0xCCCCu : j == 2 ? 0xF0F0u : 0xFF00u;
+  const uint32_t m = (has_i & ~has_j) * 0x10001u;
+  const int d = (1 << j) - (1 << i);
+  const uint32_t t = ((r >> d) ^ r) & m;
+  return r ^ t ^ (t << d);
+}
+
+// The classes of chain row q: cells[ci], ci = f<<1 | g, A (bits 0..7) / B (bits 16..23) = the cells
+// x1<<2 | d<<1 | e with a masked 1 / 0.  The v4 index bits are reordered to f, g, d, e first.
+__device__ __forceinline__ void chain_cells(uint32_t r1, uint32_t r0, int q, uint32_t *cells) {
+  uint32_t p[2] = {r0, r1};
+#pragma unroll
+  for (int x = 0; x < 2; x++) {
+    uint32_t r = p[x];
+    switch (q) {
+      case 0: r = swap_v4_bits(swap_v4_bits(r, 1, 3), 0, 2); break;
+      case 1: r = swap_v4_bits(swap_v4_bits(swap_v4_bits(r, 2, 3), 0, 2), 0, 1); break;
+      case 2: r = swap_v4_bits(swap_v4_bits(r, 2, 3), 1, 2); break;
+      case 3: r = swap_v4_bits(swap_v4_bits(r, 0, 2), 0, 1); break;
+      case 4: r = swap_v4_bits(r, 1, 2); break;
+      default: break;
+    }
+    p[x] = r;
+  }
+#pragma unroll
+  for (int ci = 0; ci < 4; ci++) {
+    cells[ci] = ((p[0] >> (4 * ci)) & 0x000f000fu) | (((p[1] >> (4 * ci)) & 0x000f000fu) << 4);
+  }
+}
+
+// The number of outer triples of either shape, and the cubes of row k (see middle_cubes).
+template <int SHAPE>
+__host__ __device__ constexpr int triples7() { return SHAPE == kShapeChain ? 35 : 25; }
+
+template <int SHAPE>
+__device__ __forceinline__ void row_cubes7(uint32_t r1, uint32_t r0, int k, uint32_t (*hv)[4],
+    bool (*hok)[4], uint32_t &S, uint32_t &ov) {
+  if constexpr (SHAPE == kShapeChain) {
+    uint32_t cells[4];
+    chain_cells(r1, r0, k % 6, cells);
+    cubes_of_cells([&](int ci) { return cells[ci]; }, hv, hok, S, ov);
+  } else {
+    middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
+  }
 }
 
 // Moves index bit b of both 16-bit halves of r to bit 3, bits b+1..3 one place down (the other
@@ -2778,7 +2851,7 @@ struct DevMatch {
   uint16_t gates[7];
   uint8_t func_outer, func_middle, func_inner, inner_seen;
   uint8_t width;
-  uint8_t pad[5];
+  uint8_t pad[5];   // sbg_match's shape (kShapeTree, kShapeChain), then its 4 bytes of padding
 };
 
 struct EnumCtl {
@@ -2839,6 +2912,7 @@ struct EnumOrders {
 
 __constant__ uint8_t c_rows5[10][5];   // ordering rows (lut.c:189,224-229 and lut.c:396-415)
 __constant__ uint8_t c_rows7[70][7];
+__constant__ uint8_t c_rows7c[210][7];   // chain rows (sbg_chain_row): a, b, c, d, e, f, g
 
 // Output of LUT(func; x, y, z) on one table word (state.c:202-230).
 __device__ __forceinline__ uint32_t lut_word(uint32_t func, uint32_t x, uint32_t y, uint32_t z) {
@@ -2852,7 +2926,7 @@ __device__ __forceinline__ uint32_t lut_word(uint32_t func, uint32_t x, uint32_t
 
 // A match's record of width 3, 5 or 7: the first WIDTH gates of G, zeros in the fields the width
 // does not use (func_outer at width 3, func_middle below width 7).
-template <int WIDTH>
+template <int WIDTH, int SHAPE = kShapeTree>
 __device__ __forceinline__ void store_match(DevMatch *__restrict__ dst, unsigned long long key,
     const int *G, uint32_t fo, uint32_t fm, uint32_t inner, uint32_t seen) {
   DevMatch m;
@@ -2865,26 +2939,32 @@ __device__ __forceinline__ void store_match(DevMatch *__restrict__ dst, unsigned
   m.inner_seen = (uint8_t)seen;
   m.width = (uint8_t)WIDTH;
 #pragma unroll
-  for (int i = 0; i < 5; i++) m.pad[i] = 0;
+  for (int i = 0; i < 5; i++) m.pad[i] = i == 0 ? (uint8_t)SHAPE : (uint8_t)0;
   *dst = m;
 }
 
-// A 5- or 7-LUT match's record: gates in reference order (tuple positions of ordering row k),
-// func_inner = solved bits only and inner_seen = cells with a masked position (sbg_solve_inner's
-// closed form, on the compressed tables; a match has no conflicting cell).
-template <int NW, int WIDTH>
+// A 5- or 7-LUT match's record: gates in reference order (tuple positions of ordering row k; a
+// chain: of chain row k), func_inner = solved bits only and inner_seen = cells with a masked
+// position (sbg_solve_inner's closed form, on the compressed tables; a match has no conflicting
+// cell).  The inner LUT's cells are x<<2 | y<<1 | z: the outer LUT, the middle LUT (5-LUT: d) and
+// the last gate for the tree, the middle LUT, f and g for the chain.
+template <int NW, int WIDTH, int SHAPE = kShapeTree>
 __device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned long long key,
     const int *tuple, int k, uint32_t fo, uint32_t fm, const uint32_t *s_tabs, int npad,
     const uint32_t *T, const uint32_t *M) {
+  constexpr bool CHAIN = SHAPE == kShapeChain;
   int G[WIDTH];
 #pragma unroll
-  for (int i = 0; i < WIDTH; i++) G[i] = tuple[WIDTH == 5 ? c_rows5[k][i] : c_rows7[k][i]];
+  for (int i = 0; i < WIDTH; i++) {
+    G[i] = tuple[WIDTH == 5 ? c_rows5[k][i] : CHAIN ? c_rows7c[k][i] : c_rows7[k][i]];
+  }
   uint32_t ones = 0, seen = 0;
 #pragma unroll
   for (int w = 0; w < NW; w++) {
     const uint32_t *t = s_tabs + w * npad;
-    const uint32_t x = lut_word(fo, t[G[0]], t[G[1]], t[G[2]]);
-    const uint32_t y = WIDTH == 7 ? lut_word(fm, t[G[3]], t[G[4]], t[G[5]]) : t[G[3]];
+    const uint32_t l1 = lut_word(fo, t[G[0]], t[G[1]], t[G[2]]);
+    const uint32_t x = CHAIN ? lut_word(fm, l1, t[G[3]], t[G[4]]) : l1;
+    const uint32_t y = CHAIN ? t[G[5]] : WIDTH == 7 ? lut_word(fm, t[G[3]], t[G[4]], t[G[5]]) : t[G[3]];
     const uint32_t z = t[G[WIDTH - 1]];
 #pragma unroll
     for (int c = 0; c < 8; c++) {
@@ -2893,7 +2973,7 @@ __device__ __forceinline__ void write_match(DevMatch *__restrict__ dst, unsigned
       if (in_cell) seen |= 1u << c;
     }
   }
-  store_match<WIDTH>(dst, key, G, fo, fm, ones, seen);
+  store_match<WIDTH, SHAPE>(dst, key, G, fo, fm, ones, seen);
 }
 
 // ---- kernel forms --------------------------------------------------------------------------------
@@ -3010,6 +3090,19 @@ __device__ __forceinline__ int depth7(const int *d7, int k) {
   return max(2 + m6, 1 + dg);
 }
 
+// Depth of a 7-LUT match of row k of either shape; a chain's is 1 + max(1 + max(1 + max(Da, Db,
+// Dc), Dd, De), Df, Dg), gates in record order.
+template <int SHAPE>
+__device__ __forceinline__ int depth7s(const int *d7, int k) {
+  if constexpr (SHAPE == kShapeChain) {
+    const uint8_t *p = c_rows7c[k];
+    return max(max(3 + max(max(d7[p[0]], d7[p[1]]), d7[p[2]]), 2 + max(d7[p[3]], d7[p[4]])),
+        1 + max(d7[p[5]], d7[p[6]]));
+  } else {
+    return depth7(d7, k);
+  }
+}
+
 // ---- function filter (sbg_enum_set_functions) --------------------------------------------------
 // The filtered and grouped forms keep only the matches whose outer LUT lies in the outer set, whose
 // middle LUT lies in the middle set, and whose inner LUT can be completed inside the inner set:
@@ -3046,17 +3139,29 @@ __device__ __forceinline__ void inner_cells7(uint32_t r1, uint32_t r0, int b, ui
   for (int ci = 0; ci < 4; ci++) AB[ci] = compress16x2((ci & 2) ? r1 : r0, b, ci & 1);
 }
 
+// inner_cells7 for row k of either shape (a chain's classes from chain_cells).
+template <int SHAPE>
+__device__ __forceinline__ void row_cells7(uint32_t r1, uint32_t r0, int k, uint32_t *AB) {
+  if constexpr (SHAPE == kShapeChain) chain_cells(r1, r0, k % 6, AB);
+  else inner_cells7(r1, r0, c_row_b[k], AB);
+}
+
 // The 7-LUT inner test of middle function fm: inner cell (x, y, g) holds a masked 1 iff fm sends a
-// pattern of A to y, a masked 0 likewise with B.
+// pattern of A to y, a masked 0 likewise with B.  A chain's inner cells are (x2, f, g), x2 = fm's
+// value, with AB from chain_cells.
+template <int SHAPE = kShapeTree>
 __device__ __forceinline__ bool inner_ok7(const uint32_t *s_fn, const uint32_t *AB, uint32_t fm) {
+  constexpr bool CHAIN = SHAPE == kShapeChain;
+  constexpr uint32_t ybit = CHAIN ? 4u : 2u;   // the inner cell's bit that fm decides
   uint32_t ones = 0, seen = 0;
 #pragma unroll
   for (int ci = 0; ci < 4; ci++) {
-    const uint32_t c0 = (ci & 2) << 1 | (ci & 1);   // cell x<<2 | 0<<1 | g
+    // cell x<<2 | 0<<1 | g (chain: 0<<2 | f<<1 | g)
+    const uint32_t c0 = CHAIN ? (uint32_t)ci : (ci & 2) << 1 | (ci & 1);
     const uint32_t A = AB[ci] & 0xffu, B = AB[ci] >> 16;
-    if (A & fm) ones |= 1u << (c0 | 2);
+    if (A & fm) ones |= 1u << (c0 | ybit);
     if (A & ~fm) ones |= 1u << c0;
-    if ((A | B) & fm) seen |= 1u << (c0 | 2);
+    if ((A | B) & fm) seen |= 1u << (c0 | ybit);
     if ((A | B) & ~fm) seen |= 1u << c0;
   }
   return inner_ok(s_fn, seen, ones);
@@ -3376,6 +3481,7 @@ __device__ __forceinline__ int outer_list7(uint32_t surv_mine, uint8_t *fo_list,
 // every inner function allowed, one lane per outer function and the popcount of its cube union
 // ANDed with the middle set; with a restricted inner set (slow), every (fo, fm) of the union
 // through inner_ok7, lanes over fm.
+template <int SHAPE>
 __device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, int ns,
     const uint32_t *W, int k, const uint32_t *s_fn, bool slow, int lane) {
   unsigned long long size = 0;
@@ -3390,7 +3496,7 @@ __device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, 
     }
     uint32_t hv[2][4], S, ov;
     bool hok[2][4];
-    middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
+    row_cubes7<SHAPE>(r1, r0, k, hv, hok, S, ov);
     if (!slow) {
       uint32_t bits[8], c = 0;
       cube_union(hv, hok, S, ov, bits);
@@ -3400,12 +3506,12 @@ __device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, 
       continue;
     }
     uint32_t AB[4];
-    inner_cells7(r1, r0, c_row_b[k], AB);
+    row_cells7<SHAPE>(r1, r0, k, AB);
 #pragma unroll 1
     for (int w = 0; w < 8; w++) {
       const uint32_t fm = 32u * w + lane;
       const bool hit = in_cubes(hv, hok, S, ov, fm) && in_set(s_fn + 8, fm)
-          && inner_ok7(s_fn, AB, fm);
+          && inner_ok7<SHAPE>(s_fn, AB, fm);
       size += __popc(__ballot_sync(kFull, hit));
     }
   }
@@ -3428,6 +3534,16 @@ __device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, 
 //              the depth filter a prefix, or a lane's g, that no ordering within the bound can
 //              use is dropped before the feasibility work, and `feasible` counts the feasible
 //              combinations with such an ordering.
+// The shape (template parameter SHAPE, kShapeChain with kSrcWhole only) picks the rows: the tree's
+// 70 ordering rows over its 25 outer triples, or the chain's 210 rows k = 6 j + q over all 35
+// (key rank << 24 | k << 16 | po << 8 | pm; a ticket holds at most (n - 6) * 210 * 65,536 < 2^32
+// matches).  Stage 1 (outer_ok7) is the same for both: an outer function must leave a conflict-free
+// 5-input remainder over (x1, the other four gates) either way.  So is triples_with_colourings,
+// which decides exactly whether outer_ok7 leaves a survivor; the chain uses it for triples 0..24
+// and runs outer_ok7 on the other ten.  The depth pruning is the shape's: a tree needs every gate
+// below B and at most one at B - 1 (its g); a chain every gate below B, at most two at B - 1 or
+// deeper (its f, g) and at most four at B - 2 or deeper (its d, e, f, g), which is exact as every
+// split of the seven into (3, 2, 2) is a chain row.
 enum Enum7Source : int { kSrcList = 0, kSrcWhole = 1 };
 constexpr int kEnum7AllMaxGates = 64;   // SBG_ENUM7_ALL_MAX_GATES: C(63, 6) tickets of 12 bytes
 constexpr int kPrefix7Cells = 64;       // cells of a 6-gate prefix
@@ -3447,7 +3563,7 @@ constexpr int kPrefix7Cells = 64;       // cells of a 6-gate prefix
 // first); the emit loop emits a row's first hit (first po, lowest pm) and moves to the next row.
 // Under kGroupTuple both end the combination at its first row with a match.  A group never leaves
 // its combination, so it never crosses a ticket under either source.
-template <int NW, int MODE, int FORM, int SRC>
+template <int NW, int MODE, int FORM, int SRC, int SHAPE = kShapeTree>
 __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
     EnumCtl *__restrict__ ectl, const EnumOrders &ord, const uint64_t *__restrict__ list,
     unsigned int list_count, uint32_t *__restrict__ counts,
@@ -3456,10 +3572,13 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
     int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> &flt) {
   constexpr bool FILTER = FORM != kFormPlain, GR = FORM == kFormGrouped;
   constexpr bool EMIT = MODE != kEnumCount;
+  constexpr bool CHAIN = SHAPE == kShapeChain;
+  constexpr int NJ = triples7<SHAPE>();
+  static_assert(!CHAIN || SRC == kSrcWhole, "the chain is enumerated over the whole space only");
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
   __shared__ uint8_t s_fo[kWarpsPerCta][256];
-  __shared__ uint32_t s_src7[25 * 32];
+  __shared__ uint32_t s_src7[NJ * 32];
   __shared__ uint32_t s_H[kWarpsPerCta][16];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -3468,6 +3587,9 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
   uint32_t *s_tabs = smem;
   stage_tables(s_tabs, prob, NW, npad);
   for (int i = threadIdx.x; i < 25 * 32; i += blockDim.x) s_src7[i] = tab->src7[i >> 5][i & 31];
+  if constexpr (CHAIN) {
+    for (int i = threadIdx.x; i < 10 * 32; i += blockDim.x) s_src7[800 + i] = tab->src7x[i >> 5][i & 31];
+  }
   for (int i = threadIdx.x; i < 512; i += blockDim.x) s_ord[i >> 8][i & 255] = ord.order[i >> 8][i & 255];
   const uint16_t *s_dep = nullptr;
   const uint32_t *s_fn = nullptr;
@@ -3488,31 +3610,39 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
   uint32_t *sH = s_H[warp];
   uint8_t *fo_list = s_fo[warp];
 
-  // One combination g (tuple order), whose keys are idx << 23 | k << 16 | po << 8 | pm: its
-  // matches in key order through emit_step.
+  // One combination g (tuple order), whose keys are idx << 23 | k << 16 | po << 8 | pm (chain:
+  // idx << 24): its matches in key order through emit_step.
   auto tuple7 = [&](const int *g, unsigned long long idx, EnumTicket &tk) {
     int d7[7];
     if constexpr (FILTER) {
-      // no gate of depth >= B, and at most one of depth B - 1 (it must be the last input)
-      int deep = 0;
+      // no gate of depth >= B, and at most one of depth B - 1 (it must be the last input); chain:
+      // at most two of depth >= B - 1 and four of depth >= B - 2
+      int deep = 0, deep2 = 0;
       bool over = false;
 #pragma unroll
       for (int i = 0; i < 7; i++) {
         d7[i] = s_dep[g[i]];
         over |= d7[i] >= B;
         deep += d7[i] >= B - 1;
+        if constexpr (CHAIN) deep2 += d7[i] >= B - 2;
       }
-      if (over || deep > 1) return;
+      if constexpr (CHAIN) {
+        if (over || deep > 2 || deep2 > 4) return;
+      } else {
+        if (over || deep > 1) return;
+      }
     }
     tuple_summary<NW>(s_tabs, npad, g, T, M, lane, sH);
     const uint32_t pass_j = triples_with_colourings(sH, lane);
     bool done = false;
     [[maybe_unused]] SizeWalkOf<MODE> sw;
-    for (int j = 0; j < 25 && !done; j++) {
-      if (((pass_j >> j) & 1u) == 0) continue;
+    for (int j = 0; j < NJ && !done; j++) {
+      if (j < 25 && ((pass_j >> j) & 1u) == 0) continue;
+      const int k0 = CHAIN ? 6 * j : c_j_first_k[j];
+      const int nrows = CHAIN ? 6 : c_j_rows[j];
       if constexpr (FILTER) {
         bool fits = false;
-        for (int row = 0; row < c_j_rows[j]; row++) fits |= depth7(d7, c_j_first_k[j] + row) <= B;
+        for (int row = 0; row < nrows; row++) fits |= depth7s<SHAPE>(d7, k0 + row) <= B;
         if (!fits) continue;
       }
       uint32_t W[8], ok[8];
@@ -3526,8 +3656,6 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
         if (lane == hi) surv_mine = sv;
       }
       if (any == 0) continue;
-      const int k0 = c_j_first_k[j];
-      const int nrows = c_j_rows[j];
       [[maybe_unused]] int ns_sizes = 0;   // sizes pass: the survivors in fo_list
       if constexpr (MODE == kEnumSizes) ns_sizes = outer_list7(surv_mine, fo_list, lane);
       if (!EMIT && !slow) {
@@ -3535,7 +3663,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
         if constexpr (GR) {
 #pragma unroll 1
           for (int row = 0; row < nrows; row++) {
-            const int rd = depth7(d7, k0 + row);
+            const int rd = depth7s<SHAPE>(d7, k0 + row);
             if (rd > B) continue;
             bool found = false;
             for (int i0 = 0; i0 < ns && !found; i0 += 32) {
@@ -3548,7 +3676,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
               }
               uint32_t hv[2][4], S, ov, bits[8], nz = 0;
               bool hok[2][4];
-              middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
+              row_cubes7<SHAPE>(r1, r0, k0 + row, hv, hok, S, ov);
               cube_union(hv, hok, S, ov, bits);
 #pragma unroll
               for (int wd = 0; wd < 8; wd++) nz |= bits[wd] & s_fn[8 + wd];
@@ -3577,13 +3705,13 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
           for (int row = 0; row < nrows; row++) {
             int rd = 0;
             if constexpr (FILTER) {
-              rd = depth7(d7, k0 + row);
+              rd = depth7s<SHAPE>(d7, k0 + row);
               if (rd > B) continue;
             }
             const uint32_t c_before = c;
             uint32_t hv[2][4], S, ov, bits[8];
             bool hok[2][4];
-            middle_cubes(r1, r0, c_row_b[k0 + row], hv, hok, S, ov);
+            row_cubes7<SHAPE>(r1, r0, k0 + row, hv, hok, S, ov);
             cube_union(hv, hok, S, ov, bits);
             if constexpr (FILTER) {
 #pragma unroll
@@ -3605,10 +3733,10 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
 #pragma unroll 1
       for (int row = 0; (EMIT || slow) && row < nrows && !done; row++) {
         const int k = k0 + row;
-        if (FILTER && depth7(d7, k) > B) continue;
+        if (FILTER && depth7s<SHAPE>(d7, k) > B) continue;
         if constexpr (MODE == kEnumSizes) {
           if (sw.sizing) {
-            sw.size += row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
+            sw.size += row_size7<SHAPE>(fo_list, ns_sizes, W, k, s_fn, slow, lane);
             continue;
           }
         }
@@ -3625,16 +3753,19 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
           }
           uint32_t hv[2][4], S, ov;
           bool hok[2][4];
-          middle_cubes(r1, r0, c_row_b[k], hv, hok, S, ov);
+          row_cubes7<SHAPE>(r1, r0, k, hv, hok, S, ov);
           [[maybe_unused]] uint32_t AB[4] = {0, 0, 0, 0};
-          if (FILTER && slow) inner_cells7(r1, r0, c_row_b[k], AB);
-          const unsigned long long key_hi = (idx << 23) | ((uint64_t)k << 16) | ((uint64_t)po << 8);
+          if (FILTER && slow) row_cells7<SHAPE>(r1, r0, k, AB);
+          const unsigned long long key_hi = (idx << (CHAIN ? 24 : 23)) | ((uint64_t)k << 16)
+              | ((uint64_t)po << 8);
 #pragma unroll 1
           for (int w = 0; w < 8; w++) {
             const uint32_t pm = 32u * w + lane;
             const uint32_t fm = s_ord[1][pm];
             bool hit = in_cubes(hv, hok, S, ov, fm);
-            if constexpr (FILTER) hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7(s_fn, AB, fm));
+            if constexpr (FILTER) {
+              hit = hit && in_set(s_fn + 8, fm) && (!slow || inner_ok7<SHAPE>(s_fn, AB, fm));
+            }
             if constexpr (GR) {
               // the group's record: the first hit of the row
               const uint32_t bal = __ballot_sync(kFull, hit);
@@ -3646,7 +3777,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
               // the row's group; a wanted tuple group goes on through the entry's later rows
               // and takes its step after them
               if (size_wanted(tk)) {
-                sw.size = row_size7(fo_list, ns_sizes, W, k, s_fn, slow, lane);
+                sw.size = row_size7<SHAPE>(fo_list, ns_sizes, W, k, s_fn, slow, lane);
                 sw.sizing = flt.grouping == kGroupTuple;
               }
               if (!sw.sizing) {
@@ -3656,7 +3787,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
               }
             } else {
               done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
-                write_match<NW, 7>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
+                write_match<NW, 7, SHAPE>(out + i, key_hi | pm, g, k, fo, fm, s_tabs, npad, T, M);
               });
             }
             if (GR && row_hit) break;
@@ -3666,7 +3797,7 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
         if constexpr (FILTER && MODE == kEnumCount) {
           // the slow count pass: this row's matches to its depth's bin
           if (flt.hist_on && lane == 0 && tk.count != row_start) {
-            hist_add(depth7(d7, k), tk.count - row_start);
+            hist_add(depth7s<SHAPE>(d7, k), tk.count - row_start);
           }
         }
         if constexpr (GR) {
@@ -3709,14 +3840,20 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
       bool rejected = false;
 #pragma unroll
       for (int i = 0; i < 6; i++) rejected |= (pre[i] < 8) && ((inmask >> pre[i]) & 1u);
-      int pre_deep = 0;   // prefix gates of depth B - 1 (at most one gate of a match may have it)
+      // prefix gates of depth >= B - 1 (at most one gate of a tree may have it, two of a chain),
+      // and of depth >= B - 2 (chain: at most four)
+      constexpr int kDeep1 = CHAIN ? 2 : 1;
+      int pre_deep = 0;
+      [[maybe_unused]] int pre_deep2 = 0;
       if constexpr (FILTER) {
 #pragma unroll
         for (int i = 0; i < 6; i++) {
           rejected |= s_dep[pre[i]] >= B;
           pre_deep += s_dep[pre[i]] >= B - 1;
+          if constexpr (CHAIN) pre_deep2 += s_dep[pre[i]] >= B - 2;
         }
-        rejected |= pre_deep > 1;
+        rejected |= pre_deep > kDeep1;
+        if constexpr (CHAIN) rejected |= pre_deep2 > 4;
       }
       if (rejected) return;
       uint32_t mixed[2];   // prefix cells 32 * h + lane with a masked 1 and a masked 0
@@ -3749,7 +3886,8 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
         if constexpr (FILTER) {
           if (alive) {
             const int dg = s_dep[gl];
-            alive = dg < B && pre_deep + (dg >= B - 1) <= 1;
+            alive = dg < B && pre_deep + (dg >= B - 1) <= kDeep1;
+            if constexpr (CHAIN) alive = alive && pre_deep2 + (dg >= B - 2) <= 4;
           }
         }
 #pragma unroll
@@ -3802,6 +3940,18 @@ __global__ void __launch_bounds__(kThreads) k_enum7_all(const DevProblem *__rest
     int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
   enum7_body<NW, MODE, FORM, kSrcWhole>(prob, ectl, ord, nullptr, 0u, counts, offsets, out,
       max_out, t_begin, t_end, part, nparts, tab, flt);
+}
+
+// The chain over the whole space (sbg_enum7_chain): k_enum7_all's sweep and launch shape with the
+// chain's rows.
+template <int NW, int MODE, int FORM>
+__global__ void __launch_bounds__(kThreads) k_enum7_chain(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
+  enum7_body<NW, MODE, FORM, kSrcWhole, kShapeChain>(prob, ectl, ord, nullptr, 0u, counts, offsets,
+      out, max_out, t_begin, t_end, part, nparts, tab, flt);
 }
 
 

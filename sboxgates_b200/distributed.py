@@ -257,6 +257,14 @@ class DistributedLutSearch:
             lambda k, part, nparts: self.engine.enumerate7_all(outer, middle, k, True, part, nparts),
             max_matches)
 
+    def enumerate7_chain(self, outer, middle, max_matches):
+        """The 7-LUT chain realisations (LutEngine.enumerate7_chain), over every 7-combination as
+        enumerate7_all: no list is installed, and `feasible` is summed over the ranks."""
+        return self._enumerate(
+            lambda k, part, nparts: self.engine.enumerate7_chain(outer, middle, k, True, part,
+                                                                 nparts),
+            max_matches)
+
     def fetch_matches(self, first, count):
         """The whole's matches at ranks first .. min(first + count, total) - 1 (the last
         enumerate* call's), the same on every rank."""

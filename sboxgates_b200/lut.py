@@ -16,7 +16,7 @@ from . import native
 from .native import (SbgResult, SbgJob, SbgNodeResult, NativeLibraryError, SBG_KEY_NONE,
                      SBG_LIST_CAP, SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7, MATCH_DTYPE,
                      SBG_ENUM_MAX_MATCHES, SBG_MAX_GATES, SBG_MAX_DEPTH, SBG_DEPTH_BINS,
-                     SBG_ENUM7_ALL_MAX_GATES)
+                     SBG_ENUM7_ALL_MAX_GATES, SBG_SHAPE_TREE, SBG_SHAPE_CHAIN)
 
 NO_GATE = 0xFFFF  # state.h:30
 
@@ -97,6 +97,17 @@ def ordering_row(width, k):
     row = (C.c_int * width)()
     if lib.sbg_ordering_row(width, k, row) != 0:
         raise ValueError("bad ordering (%d, %d)" % (width, k))
+    return [int(x) for x in row]
+
+
+def chain_row(k):
+    """Row k (0..209) of the 7-LUT chain L3(L2(L1(a,b,c), d, e), f, g) (sbg_chain_row): the
+    combination's positions in record order a..g.  k = 6 j + q: j = L1's position triple, q = the
+    pair {d, e} among the other four, both in lexicographic order."""
+    lib = native.load_library()
+    row = (C.c_int * 7)()
+    if lib.sbg_chain_row(int(k), row) != 0:
+        raise ValueError("bad chain row %r" % (k,))
     return [int(x) for x in row]
 
 
@@ -410,6 +421,15 @@ class LutEngine:
         return self._enumerate(self.lib.sbg_enum7_all, [outer_order, middle_order], max_matches,
                                count, part, nparts)
 
+    def enumerate7_chain(self, outer_order, middle_order, max_matches, count=True, part=0,
+                         nparts=1):
+        """The 7-LUT realisations wired as a chain L3(L2(L1(a,b,c), d, e), f, g), which search_7lut
+        never tries (sbg_enum7_chain), over the combinations enumerate7_all takes: keys rank << 24 |
+        k << 16 | po << 8 | pm with k a chain_row, L1 = outer_order[po], L2 = middle_order[pm], and
+        records of shape SBG_SHAPE_CHAIN (see chain_luts).  The installed list stays."""
+        return self._enumerate(self.lib.sbg_enum7_chain, [outer_order, middle_order], max_matches,
+                               count, part, nparts)
+
     def enumerate3(self, gate_order, max_matches, count=True, part=0, nparts=1):
         """Every match of lut_search's 3-LUT scan over `gate_order` (a permutation of the current
         problem's gates): the feasible position triples, keys i << 18 | k << 9 | m."""
@@ -589,25 +609,31 @@ def inner_table(inner=None):
 # -- grouping: the distinct gate sets and wirings that realise a state ---------------------------
 _GROUPINGS = {None: native.SBG_GROUP_NONE, "shape": native.SBG_GROUP_SHAPE,
               "tuple": native.SBG_GROUP_TUPLE}
-# the key bits below a group's id, per (grouping, width): positions (shape), then the ordering row
-_GROUP_SHIFT = {("shape", 5): 8, ("shape", 7): 16, ("tuple", 5): 12, ("tuple", 7): 23}
+# the key bits below a group's id, per (grouping, width, wiring): positions (shape), then the row
+_GROUP_SHIFT = {("shape", 5, "tree"): 8, ("shape", 7, "tree"): 16, ("tuple", 5, "tree"): 12,
+                ("tuple", 7, "tree"): 23, ("shape", 7, "chain"): 16, ("tuple", 7, "chain"): 24}
 
 
-def match_group(key, width, grouping):
+def match_group(key, width, grouping, shape="tree"):
     """The id of the group an enumerated match's key belongs to under a grouping (see
     LutEngine.set_grouping): the key itself for None and for width 3, else key >> 8 / key >> 16
-    (shape, 5- / 7-LUT) or key >> 12 / key >> 23 (tuple).  Matches of one group have equal ids;
-    groups come in ascending id order."""
+    (shape, 5- / 7-LUT) or key >> 12 / key >> 23 (tuple).  shape="chain" reads a key of
+    enumerate7_chain (width 7): key >> 16 (shape) or key >> 24 (tuple).  Matches of one group have
+    equal ids; groups come in ascending id order."""
     if grouping not in _GROUPINGS:
         raise ValueError("grouping must be None, 'shape' or 'tuple', not %r" % (grouping,))
     if width not in (3, 5, 7):
         raise ValueError("width must be 3, 5 or 7")
+    if shape not in ("tree", "chain"):
+        raise ValueError("shape must be 'tree' or 'chain', not %r" % (shape,))
+    if shape == "chain" and width != 7:
+        raise ValueError("a chain is a 7-LUT wiring")
     key = int(key)
     if not 0 <= key < 2**64:
         raise ValueError("key must lie in 0..2**64-1")
     if grouping is None or width == 3:
         return key
-    return key >> _GROUP_SHIFT[(grouping, width)]
+    return key >> _GROUP_SHIFT[(grouping, width, shape)]
 
 
 def _depth_args(depth, max_depth):
@@ -635,19 +661,22 @@ def match_depth(record, depth):
     """The depth of the gate an enumerated match (a MATCH_DTYPE record) would add, given the depth
     of every gate of the problem: 1 + max(Da, Db, Dc) for a 3-LUT; 1 + max(1 + max(Da, Db, Dc),
     Dd, De) for a 5-LUT (outer LUT over a, b, c); 1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df),
-    Dg) for a 7-LUT (outer over a, b, c, middle over d, e, f).  Gates in the record's order."""
+    Dg) for a 7-LUT (outer over a, b, c, middle over d, e, f); 1 + max(1 + max(1 + max(Da, Db, Dc),
+    Dd, De), Df, Dg) for a 7-LUT chain (the record's shape).  Gates in the record's order."""
     width = int(record["width"])
     d = [int(depth[int(g)]) for g in record["gates"][:width]]
     if width == 3:
         return 1 + max(d)
     if width == 5:
         return 1 + max(1 + max(d[:3]), d[3], d[4])
+    if width == 7 and int(record["shape"]) == SBG_SHAPE_CHAIN:
+        return 1 + max(1 + max(1 + max(d[:3]), d[3], d[4]), d[5], d[6])
     if width == 7:
         return 1 + max(1 + max(d[:3]), 1 + max(d[3:6]), d[6])
     raise ValueError("not a match record (width %d)" % width)
 
 
-def shallowest_matches(engine, width, orders, depth, max_matches, whole=False):
+def shallowest_matches(engine, width, orders, depth, max_matches, whole=False, shape="tree"):
     """The shallowest realisations of the current problem by the width-3, 5 or 7 enumeration:
     one count with the loosest bound gives the depth histogram, a second counts at its first
     non-empty depth.  `orders` are the enumerate call's order arguments: (gate_order,),
@@ -658,12 +687,19 @@ def shallowest_matches(engine, width, orders, depth, max_matches, whole=False):
     grouping: under "tuple" grouping a gate set is binned at the depth of its first match, which
     need not be its shallowest.  whole=True (width 7 only) searches every 7-combination
     (enumerate7_all) instead of the phase-1 list, so the result is the state's shallowest 7-LUT
-    realisation, not the list's."""
+    realisation, not the list's.  shape="chain" (width 7 only) takes the chain realisations of
+    enumerate7_chain, which always cover every 7-combination."""
     if width not in (3, 5, 7):
         raise ValueError("width must be 3, 5 or 7")
     if whole and width != 7:
         raise ValueError("whole=True applies to width 7 only")
-    run = getattr(engine, "enumerate7_all" if whole else "enumerate%d" % width)
+    if shape not in ("tree", "chain"):
+        raise ValueError("shape must be 'tree' or 'chain', not %r" % (shape,))
+    if shape == "chain" and width != 7:
+        raise ValueError("shape='chain' applies to width 7 only")
+    name = ("enumerate7_chain" if shape == "chain" else "enumerate7_all" if whole
+            else "enumerate%d" % width)
+    run = getattr(engine, name)
     engine.set_depth_filter(depth, SBG_DEPTH_BINS - 1)
     run(*orders, 0)
     hist = engine.depth_counts()
@@ -870,6 +906,8 @@ def match_to_ret(match, rng):
     get_lut_function would fill them.  A 3-LUT match has no ret[10]: see match_to_lut3."""
     if int(match["width"]) == 3:
         raise ValueError("a 3-LUT match has no ret[10]; use match_to_lut3")
+    if int(match["shape"]) == SBG_SHAPE_CHAIN:
+        raise ValueError("a chain match has no ret[10] (search_7lut's wiring); use chain_luts")
     fi = _fill(match["func_inner"], match["inner_seen"], rng)
     gates = [int(g) for g in match["gates"]]
     if int(match["width"]) == 5:
@@ -885,6 +923,28 @@ def match_to_lut3(match, rng):
         raise ValueError("not a 3-LUT match (width %d)" % int(match["width"]))
     fi = _fill(match["func_inner"], match["inner_seen"], rng)
     return (fi, int(match["gates"][0]), int(match["gates"][1]), int(match["gates"][2]))
+
+
+def chain_luts(match, rng_or_fill):
+    """One enumerated chain match (enumerate7_chain) -> its three LUTs in the order a circuit
+    builder appends them: [(L1, (a, b, c)), (L2, (("new", 0), d, e)), (L3, (("new", 1), f, g))],
+    ("new", k) being the k-th LUT of the list (LutSearchResult's convention).  L3 is filled:
+    rng_or_fill is either an int, a complete function that agrees with the solved bits (see
+    allowed_fill), or an rng whose draw fills the don't-care bits as get_lut_function would (one
+    draw iff a cell is unseen)."""
+    if int(match["width"]) != 7 or int(match["shape"]) != SBG_SHAPE_CHAIN:
+        raise ValueError("not a chain match (width %d, shape %d)"
+                         % (int(match["width"]), int(match["shape"])))
+    if isinstance(rng_or_fill, (int, np.integer)):
+        f3 = int(rng_or_fill)
+        if not 0 <= f3 < 256 or not inner_completes(match["func_inner"], match["inner_seen"], f3):
+            raise ValueError("function %d does not complete the inner LUT" % f3)
+    else:
+        f3 = _fill(match["func_inner"], match["inner_seen"], rng_or_fill)
+    g = [int(x) for x in match["gates"]]
+    return [(int(match["func_outer"]), (g[0], g[1], g[2])),
+            (int(match["func_middle"]), (("new", 0), g[3], g[4])),
+            (f3, (("new", 1), g[5], g[6]))]
 
 
 def decode_key3(key):
@@ -904,6 +964,13 @@ def decode_key7(key):
     position, middle position)."""
     key = int(key)
     return key >> 23, (key >> 16) & 0x7F, (key >> 8) & 0xFF, key & 0xFF
+
+
+def decode_key7_chain(key):
+    """7-LUT chain key (enumerate7_chain) -> (the combination's rank, chain row k, outer position,
+    middle position)."""
+    key = int(key)
+    return key >> 24, (key >> 16) & 0xFF, (key >> 8) & 0xFF, key & 0xFF
 
 
 def enumerate_5lut(engine, tables, target, mask, inbits, order, max_matches, count=True, part=0,
@@ -935,6 +1002,17 @@ def enumerate_7lut_all(engine, tables, target, mask, inbits, outer, middle, max_
                          % SBG_ENUM7_ALL_MAX_GATES)
     engine.load(tables, target, mask, inbits)
     return engine.enumerate7_all(outer, middle, max_matches, count, part, nparts)
+
+
+def enumerate_7lut_chain(engine, tables, target, mask, inbits, outer, middle, max_matches,
+                         count=True, part=0, nparts=1):
+    """The realisations by the 7-LUT chain L3(L2(L1(a,b,c), d, e), f, g), which search_7lut never
+    tries, over every feasible 7-combination (LutEngine.enumerate7_chain; at most
+    SBG_ENUM7_ALL_MAX_GATES gates).  Consumes no RNG; chain_luts applies the fill per match."""
+    if not 7 <= len(tables) <= SBG_ENUM7_ALL_MAX_GATES:
+        raise ValueError("the 7-LUT chain enumeration takes 7..%d gates" % SBG_ENUM7_ALL_MAX_GATES)
+    engine.load(tables, target, mask, inbits)
+    return engine.enumerate7_chain(outer, middle, max_matches, count, part, nparts)
 
 
 def enumerate_3lut(engine, tables, target, mask, inbits, gate_order, max_matches, count=True,

@@ -46,13 +46,13 @@ class SbgMatch(C.Structure):
     """One enumerated match (sbg_match, 32 bytes)."""
     _fields_ = [("key", C.c_uint64), ("gates", C.c_uint16 * 7), ("func_outer", C.c_uint8),
                 ("func_middle", C.c_uint8), ("func_inner", C.c_uint8), ("inner_seen", C.c_uint8),
-                ("width", C.c_uint8), ("pad", C.c_uint8 * 5)]
+                ("width", C.c_uint8), ("shape", C.c_uint8), ("pad", C.c_uint8 * 4)]
 
 
 # The same layout as a numpy structured dtype: enumeration results arrive as one array.
 MATCH_DTYPE = np.dtype([("key", "<u8"), ("gates", "<u2", (7,)), ("func_outer", "u1"),
                         ("func_middle", "u1"), ("func_inner", "u1"), ("inner_seen", "u1"),
-                        ("width", "u1"), ("pad", "u1", (5,))])
+                        ("width", "u1"), ("shape", "u1"), ("pad", "u1", (4,))])
 SBG_ENUM_MAX_MATCHES = 1 << 24
 SBG_ENUM7_ALL_MAX_GATES = 64   # largest n of the whole-space 7-LUT enumeration (sbg_enum7_all)
 SBG_MAX_GATES = 500
@@ -61,6 +61,8 @@ SBG_DEPTH_BINS = 1024     # bins of the depth histogram
 SBG_GROUP_NONE = 0        # enumeration groupings (sbg_enum_set_grouping): every match,
 SBG_GROUP_SHAPE = 1       #   one per (gates, ordering row),
 SBG_GROUP_TUPLE = 2       #   one per gate set
+SBG_SHAPE_TREE = 0        # a 7-LUT record's wiring (sbg_match::shape): L3(L1(a,b,c), L2(d,e,f), g),
+SBG_SHAPE_CHAIN = 1       #   or L3(L2(L1(a,b,c), d, e), f, g) (sbg_enum7_chain)
 
 SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7 = 1, 2, 4
 SBG_LANES = 8
@@ -103,6 +105,7 @@ SIGNATURES = {
     "sbg_decomp7_part": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, u64p]),
     "sbg_finish7": (C.c_int, [C.c_void_p, C.c_uint64, u8p, u8p, C.POINTER(SbgResult)]),
     "sbg_ordering_row": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "sbg_chain_row": (C.c_int, [C.c_int, C.POINTER(C.c_int)]),
     "sbg_solve_inner": (C.c_int, [u64p, u64p, u64p, u64p, u64p, u8p, u8p]),
     "sbg_lut_table": (None, [C.c_uint8, u64p, u64p, u64p, u64p]),
     "sbg_enum5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, C.c_uint64, C.c_void_p, u64p, u64p,
@@ -111,6 +114,8 @@ SIGNATURES = {
                             u64p, u64p]),
     "sbg_enum7_all": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, C.c_uint64, C.c_void_p,
                                 u64p, u64p, u64p]),
+    "sbg_enum7_chain": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, C.c_uint64, C.c_void_p,
+                                  u64p, u64p, u64p]),
     "sbg_enum3": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint16), C.c_uint64,
                             C.c_void_p, u64p, u64p, u64p]),
     "sbg_enum_fetch": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, u64p]),
