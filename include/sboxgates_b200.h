@@ -59,7 +59,8 @@ typedef struct sbg_handle sbg_handle;
    453-462) after applying the random don't-care fill. */
 typedef struct {
   int32_t found;
-  int32_t ordering;        /* k: 0..9 (lut.c:189-229) or 0..69 (lut.c:396-415) */
+  int32_t ordering;        /* k: 0..9 (lut.c:189-229) or 0..69 (lut.c:396-415); sbg_search7_chain:
+                              the chain row, 0..209 (sbg_chain_row) */
   int32_t pos_outer;       /* position of func_outer in the shuffled order */
   int32_t pos_middle;      /* 7-LUT only */
   uint8_t func_outer;
@@ -141,6 +142,25 @@ int sbg_use_problem(sbg_handle *h, int slot);
 int sbg_search5(sbg_handle *h, const uint8_t *func_order /*256*/, sbg_result *res);
 int sbg_search7(sbg_handle *h, const uint8_t *outer_order /*256*/, const uint8_t *middle_order
     /*256*/, sbg_result *res);
+/* The first 7-LUT chain L3(L2(L1(a,b,c), d, e), f, g) (the wiring of sbg_enum7_chain, which
+   search_7lut never tries) over the combinations search_7lut tries: the 7-LUT list of the current
+   problem, taken as sbg_enum7 takes it (the installed list when it belongs to the current problem as
+   staged now, else phase 1 runs here and its list stays installed), so the SBG_LIST_CAP cut applies
+   and any n >= 7 works.  Candidates are those of sbg_enum7_chain: chain row k < 210, L1 =
+   outer_order[po], L2 = middle_order[pm], L3 solvable without a random fill, decided on the true
+   gate tables.  The result is the candidate with the smallest key idx << 24 | k << 16 | po << 8 | pm,
+   idx being the list index; over an uncut list that is sbg_enum7_chain's first match with its rank
+   replaced by the list index.  res: found, key, ordering = k, pos_outer = po, pos_middle = pm,
+   func_outer = L1, func_middle = L2, func_inner / inner_seen = L3's solved bits and seen cells
+   (cells x2<<2 | f<<1 | g), gates a..g in chain-row order, index = idx, stale_outer = 0,
+   tuples_feasible = the list's length, tuples_swept = the installed list's sweep (as sbg_finish7
+   reports it); nothing matched: found = 0, key = SBG_KEY_NONE.  The caller applies L3's random fill
+   and adds L1, then L2 over (L1, d, e), then L3 over (L2, f, g).  The depth, function and grouping
+   settings are not read.  The installed list and the current problem stay as they were, unless
+   phase 1 had to run.  SBG_ERR_ARG: n < 7 or an order that is not a permutation; SBG_ERR_STATE: no
+   problem loaded. */
+int sbg_search7_chain(sbg_handle *h, const uint8_t *outer_order /*256*/,
+    const uint8_t *middle_order /*256*/, sbg_result *res);
 
 /* ---- one call per node, batches of independent nodes ----------------------------------------- */
 /* A job is what lut_search() does for one node (lut.c:489-631): the 3-LUT scan over the caller's
@@ -341,7 +361,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
    it was counted with; the caller's buffers of that call are not read again.  Cursor lifetime:
      - a counted sbg_enum* call replaces it; a count-free one ends it;
      - any call of sbg_load_problem, sbg_stage_problem, sbg_use_problem, sbg_search5, sbg_search7,
-       sbg_search_node, sbg_search_batch, sbg_search5_part, sbg_finish5, sbg_filter7_part,
+       sbg_search7_chain, sbg_search_node, sbg_search_batch, sbg_search5_part, sbg_finish5, sbg_filter7_part,
        sbg_set_list7, sbg_list7_device, sbg_set_list7_device, sbg_allgather_merge7 (every handle
        given), sbg_decomp7_part, sbg_finish7 or sbg_alu_peak ends it, whatever the call returns;
      - sbg_last_error, sbg_launch_count, sbg_transfer_stats, sbg_host_seconds, sbg_last_kernel_ms,

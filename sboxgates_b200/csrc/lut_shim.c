@@ -28,7 +28,13 @@ _Static_assert(offsetof(sbg_options, randomize) == 2019 && offsetof(sbg_options,
    per device around the sbg_*_part calls; minimum key over the devices, per-device hit lists
    gathered and merged on the devices -- the in-process counterpart of the all-reduce(MIN) /
    all-gather that sboxgates_b200/distributed.py does over NCCL); smaller ones run on the first
-   device only. */
+   device only.
+   SBG_LUT_CHAIN=1 (node variant; default off) adds a stage the reference does not have to
+   lut_search: when search_7lut ran and found nothing, the first three-LUT chain
+   L3(L2(L1(a,b,c), d, e), f, g) over the same 7-combinations and function orders
+   (sbg_search7_chain) is built from three add_lut calls, where the reference would go on to
+   multiplexer recursion.  A node without a chain leaves the state and the random stream exactly as
+   without the variable; a node with one takes only L3's don't-care fill from the generator. */
 #define SBG_SHIM_MAX_GPUS 8
 static sbg_handle *g_handles[SBG_SHIM_MAX_GPUS];
 static int g_ngpus = 0;
@@ -38,7 +44,11 @@ static uint64_t g_sharded_calls = 0;
 #define g_handle (g_handles[0])
 static uint64_t g_calls[3] = {0, 0, 0};          /* search_5lut, search_7lut, lut_search */
 static double g_seconds[3] = {0.0, 0.0, 0.0};
-static uint64_t g_node_stage[4] = {0, 0, 0, 0};  /* node calls that ended at: nothing, 3, 5, 7 */
+static uint64_t g_node_stage[5] = {0, 0, 0, 0, 0};  /* node calls that ended at: nothing, 3, 5, 7,
+                                                      the 7-LUT chain */
+static int g_lut_chain = 0;                         /* SBG_LUT_CHAIN */
+static uint64_t g_chain_calls = 0;                  /* sbg_search7_chain calls and their seconds */
+static double g_chain_seconds = 0.0;
 static double g_kernel_ms[4] = {0.0, 0.0, 0.0, 0.0}; /* search5, filter7, ordering, decomp7 */
 static int g_stats = 0;
 
@@ -146,13 +156,18 @@ static void shim_exit(void) {
   if (g_stats) {
     uint64_t tr[5] = {0, 0, 0, 0, 0};
     sbg_transfer_stats(g_handle, tr);
+    char chain_col[64] = "";   /* only with SBG_LUT_CHAIN, so the default line stays as it was */
+    if (g_lut_chain) {
+      snprintf(chain_col, sizeof(chain_col), ", 7-LUT chain %llu",
+          (unsigned long long)g_node_stage[4]);
+    }
     fprintf(stderr, "[sbg] start-up (sbg_create) %.3f s, inside the first call; "
-        "lut_search: %llu calls %.3f s (ended at: 3-LUT %llu, 5-LUT %llu, 7-LUT %llu, nothing %llu); "
+        "lut_search: %llu calls %.3f s (ended at: 3-LUT %llu, 5-LUT %llu, 7-LUT %llu%s, nothing %llu); "
         "search_5lut: %llu calls %.3f s; search_7lut: %llu calls %.3f s; "
         "%llu kernel launches; state changes: %llu bulk copies, %llu as kernel arguments, %llu none; "
         "%llu B host->device, %llu B device->host\n", g_init_seconds,
         (unsigned long long)g_calls[2], g_seconds[2], (unsigned long long)g_node_stage[1],
-        (unsigned long long)g_node_stage[2], (unsigned long long)g_node_stage[3],
+        (unsigned long long)g_node_stage[2], (unsigned long long)g_node_stage[3], chain_col,
         (unsigned long long)g_node_stage[0], (unsigned long long)g_calls[0], g_seconds[0],
         (unsigned long long)g_calls[1], g_seconds[1],
         (unsigned long long)sbg_launch_count(g_handle), (unsigned long long)tr[2],
@@ -167,6 +182,10 @@ static void shim_exit(void) {
     }
     fprintf(stderr, "[sbg] waiting by stage: 3-LUT scan %.3f s, search_5lut %.3f s, search_7lut "
         "%.3f s\n", hs[2], hs[3], hs[4]);
+    if (g_lut_chain) {
+      fprintf(stderr, "[sbg] 7-LUT chain stage: %llu calls %.3f s, %llu nodes took a chain\n",
+          (unsigned long long)g_chain_calls, g_chain_seconds, (unsigned long long)g_node_stage[4]);
+    }
     if (getenv("SBG_TIMING") != NULL) {
       fprintf(stderr, "[sbg] kernel time: search5 %.3f s, filter7 %.3f s, ordering %.3f s, "
           "decomp7 %.3f s\n", 1e-3 * g_kernel_ms[0], 1e-3 * g_kernel_ms[1], 1e-3 * g_kernel_ms[2],
@@ -196,6 +215,7 @@ static sbg_handle *handle(void) {
       want = SBG_SHIM_MAX_GPUS;
     }
     g_stats = getenv("SBG_SHIM_STATS") != NULL;
+    g_lut_chain = getenv("SBG_LUT_CHAIN") != NULL && atoi(getenv("SBG_LUT_CHAIN")) != 0;
     for (int i = 0; i < want; i++) {
       int rc = sbg_create(&g_handles[i], first + i);
       if (rc != SBG_OK) {
@@ -545,6 +565,7 @@ uint16_t lut_search(sbg_state *st, const sbg_ttable target, const sbg_ttable mas
 
   uint16_t out = SBG_SHIM_NO_GATE;
   int stage = 0;
+  bool chained = false;   /* the node took the 7-LUT chain (SBG_LUT_CHAIN) */
   if (nr.found_stage == 3) { /* lut.c:501-523 */
     const uint16_t gi = nr.gates3[0], gk = nr.gates3[1], gm = nr.gates3[2];
     uint8_t func = nr.func3;
@@ -638,12 +659,45 @@ uint16_t lut_search(sbg_state *st, const sbg_ttable target, const sbg_ttable mas
       goto done;
     }
     trace_call(7, st, target, mask, false, NULL);
+    if (g_lut_chain) {
+      /* not in the reference: the first 7-LUT chain over the list search_7lut just tried, which the
+         handle still holds (sbg_search_node / sbg_search7 installed it, or the merge of a sharded
+         phase 1 did on every device) */
+      const double tc = now();
+      sbg_result rc7;
+      rc = sbg_search7_chain(h, outer, middle, &rc7);
+      if (rc != SBG_OK) die("sbg_search7_chain", rc, h);
+      g_chain_calls++;
+      g_chain_seconds += now() - tc;
+      if (rc7.found) {
+        const uint16_t *g = rc7.gates;
+        const uint8_t l1 = rc7.func_outer, l2 = rc7.func_middle;
+        const uint8_t l3 = fill_dont_cares(rc7.func_inner, rc7.inner_seen);
+        if (opt->verbosity >= 1) {
+          printf("[   0]   Selected chain: %02x %02x %02x %3d %3d %3d %3d %3d %3d %3d\n", l1, l2,
+              l3, g[0], g[1], g[2], g[3], g[4], g[5], g[6]);
+        }
+        const sbg_ttable t1 = generate_lut_ttable(l1, st->gates[g[0]].table,
+            st->gates[g[1]].table, st->gates[g[2]].table);
+        const sbg_ttable t2 = generate_lut_ttable(l2, t1, st->gates[g[3]].table,
+            st->gates[g[4]].table);
+        const sbg_ttable t3 = generate_lut_ttable(l3, t2, st->gates[g[5]].table,
+            st->gates[g[6]].table);
+        require(ttable_equals_mask(target, t3, mask), __LINE__);
+        const uint16_t g1 = add_lut(st, l1, t1, g[0], g[1], g[2]);
+        const uint16_t g2 = add_lut(st, l2, t2, g1, g[3], g[4]);
+        out = checked(add_lut(st, l3, t3, g2, g[5], g[6]), st, target, mask, __LINE__);
+        stage = 7;
+        chained = true;
+        goto done;
+      }
+    }
   }
   if (opt->verbosity >= 2) { /* lut.c:627-629 */
     printf("[   0] No LUTs found. Num gates: %d\n", st->num_gates - get_num_inputs(st));
   }
 done:
-  g_node_stage[stage == 0 ? 0 : (stage - 1) / 2]++;
+  g_node_stage[chained ? 4 : stage == 0 ? 0 : (stage - 1) / 2]++;
   g_seconds[2] += now() - t0;
   return out;
 }

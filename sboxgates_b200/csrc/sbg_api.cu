@@ -211,9 +211,9 @@ struct EnumBuffers {
 
 // What the enumeration kernels of one width read besides the problem block: the function order(s)
 // (widths 5 and 7) or the gate order (width 3), the kernel form (EnumForm), the 7-LUT ticket source
-// (Enum7Source; kSrcList at the other widths), the 7-LUT shape (Enum7Shape; the chain with kSrcWhole
-// only) and, for the filtered and grouped forms, the filter block (take_filter; its histogram
-// pointer is the lane's, set at launch).
+// (Enum7Source; kSrcList at the other widths), the 7-LUT shape (Enum7Shape; the chain over the list
+// in the plain form only) and, for the filtered and grouped forms, the filter block (take_filter;
+// its histogram pointer is the lane's, set at launch).
 struct EnumInputs {
   EnumOrders ord;
   EnumGateOrder gates;
@@ -1644,6 +1644,17 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
             E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, h->d_tab.p,
             flt);
       } else {
+        if (in.shape == kShapeChain && in.source == kSrcList) {
+          // sbg_search7_chain's first match: the plain count and range passes only
+          if constexpr (FORM == kFormPlain && (MODE == kEnumCount || MODE == kEnumRange)) {
+            return run(k_enum7_chain_list<NW, MODE>, decomp_smem<NW>(n), prob, E.d_ectl.p, in.ord,
+                L.d_sorted.p, h->list7.count, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out,
+                a, b, part, nparts, h->d_tab.p, flt);
+          } else {
+            return fail(h, SBG_ERR_STATE, "internal: the list-form chain has no form %d, pass %d",
+                FORM, MODE);
+          }
+        }
         if (in.shape == kShapeChain) {
           return run(k_enum7_chain<NW, MODE, FORM>, enum7_all_smem<NW>(n), prob, E.d_ectl.p,
               in.ord, E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts,
@@ -2966,6 +2977,57 @@ int sbg_enum7_chain(sbg_handle *h, int part, int nparts, const uint8_t *outer_or
   // as sbg_enum7_all: no list is built or touched
   return run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, part, nparts, max_matches, out, n_out,
       total, feasible);
+}
+
+// The first chain match over the list: run_enum's count-free first K with K = 1 (windows of list
+// entries that double until a match is known), then the record turned into an sbg_result.
+int sbg_search7_chain(sbg_handle *h, const uint8_t *outer_order, const uint8_t *middle_order,
+    sbg_result *res) {
+  if (h == nullptr || res == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
+  if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
+  if (cur(h).n < 7) return fail(h, SBG_ERR_ARG, "the 7-LUT chain needs n >= 7");
+  if (!valid_order(outer_order) || !valid_order(middle_order)) {
+    return fail(h, SBG_ERR_ARG, "function order is not a permutation");
+  }
+  EnumInputs in7;
+  memcpy(in7.ord.order[0], outer_order, 256);
+  memcpy(in7.ord.order[1], middle_order, 256);
+  in7.form = kFormPlain;   // the depth, function and grouping settings are not read
+  in7.source = kSrcList;
+  in7.shape = kShapeChain;
+  memset(&in7.filter, 0, sizeof(in7.filter));
+  sbg_match m;
+  uint64_t found = 0;
+  // the installed list, else phase 1 runs and installs it (as for sbg_enum7)
+  int rc = run_enum<7>(h, kBeginKeepCtl, CallInputs(), in7, 0, 1, 1, &m, &found, nullptr, nullptr);
+  if (rc != SBG_OK) return rc;
+  memset(res, 0, sizeof(*res));
+  res->key = SBG_KEY_NONE;
+  res->tuples_feasible = h->list7.count;
+  res->tuples_swept = h->list7.swept;
+  if (found == 0) return SBG_OK;
+  res->found = 1;
+  res->key = m.key;
+  res->index = m.key >> 24;
+  res->ordering = (int)((m.key >> 16) & 0xff);
+  res->pos_outer = (int)((m.key >> 8) & 0xff);
+  res->pos_middle = (int)(m.key & 0xff);
+  res->func_outer = m.func_outer;
+  res->func_middle = m.func_middle;
+  for (int i = 0; i < 7; i++) res->gates[i] = m.gates[i];
+  // L3's solved bits from the host's tables, as finish7_slot does for the tree
+  const sbg_handle::HostProblem &hp = cur(h);
+  uint64_t x1[4], x2[4];
+  sbg_lut_table(m.func_outer, hp.tables[m.gates[0]], hp.tables[m.gates[1]], hp.tables[m.gates[2]],
+      x1);
+  sbg_lut_table(m.func_middle, x1, hp.tables[m.gates[3]], hp.tables[m.gates[4]], x2);
+  if (!sbg_solve_inner(x2, hp.tables[m.gates[5]], hp.tables[m.gates[6]], hp.target, hp.mask,
+      &res->func_inner, &res->inner_seen) || res->func_inner != m.func_inner
+      || res->inner_seen != m.inner_seen) {
+    return fail(h, SBG_ERR_STATE, "internal: the first chain match does not decompose");
+  }
+  return SBG_OK;
 }
 
 int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,

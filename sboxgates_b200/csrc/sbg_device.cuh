@@ -3519,7 +3519,7 @@ __device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, 
 }
 
 // Where the 7-LUT enumeration takes its combinations from (template parameter SRC of enum7_body):
-//   kSrcList   the installed phase-1 list (sbg_enum7): ticket t of the part is list entry
+//   kSrcList   the installed phase-1 list (sbg_enum7, sbg_search7_chain): ticket t of the part is list entry
 //              idx = t * nparts + part, and the key's high field is idx;
 //   kSrcWhole  every 7-combination (sbg_enum7_all, n <= kEnum7AllMaxGates): a ticket is a 6-gate
 //              prefix a < ... < f <= n - 2 in lexicographic order, dealt to the parts in blocks of
@@ -3534,10 +3534,10 @@ __device__ __forceinline__ unsigned long long row_size7(const uint8_t *fo_list, 
 //              the depth filter a prefix, or a lane's g, that no ordering within the bound can
 //              use is dropped before the feasibility work, and `feasible` counts the feasible
 //              combinations with such an ordering.
-// The shape (template parameter SHAPE, kShapeChain with kSrcWhole only) picks the rows: the tree's
-// 70 ordering rows over its 25 outer triples, or the chain's 210 rows k = 6 j + q over all 35
-// (key rank << 24 | k << 16 | po << 8 | pm; a ticket holds at most (n - 6) * 210 * 65,536 < 2^32
-// matches).  Stage 1 (outer_ok7) is the same for both: an outer function must leave a conflict-free
+// The shape (template parameter SHAPE) picks the rows: the tree's 70 ordering rows over its 25
+// outer triples, or the chain's 210 rows k = 6 j + q over all 35 (key rank << 24 | k << 16 | po << 8
+// | pm, or idx << 24 over the list (sbg_search7_chain); a ticket holds at most (n - 6) * 210 * 65,536
+// < 2^32 matches, a list entry 210 * 65,536).  Stage 1 (outer_ok7) is the same for both: an outer function must leave a conflict-free
 // 5-input remainder over (x1, the other four gates) either way.  So is triples_with_colourings,
 // which decides exactly whether outer_ok7 leaves a survivor; the chain uses it for triples 0..24
 // and runs outer_ok7 on the other ten.  The depth pruning is the shape's: a tree needs every gate
@@ -3574,7 +3574,6 @@ __device__ __forceinline__ void enum7_body(const DevProblem *__restrict__ prob,
   constexpr bool EMIT = MODE != kEnumCount;
   constexpr bool CHAIN = SHAPE == kShapeChain;
   constexpr int NJ = triples7<SHAPE>();
-  static_assert(!CHAIN || SRC == kSrcWhole, "the chain is enumerated over the whole space only");
   extern __shared__ uint32_t smem[];
   __shared__ uint8_t s_ord[2][256];      // position -> outer / middle function
   __shared__ uint8_t s_fo[kWarpsPerCta][256];
@@ -3952,6 +3951,22 @@ __global__ void __launch_bounds__(kThreads) k_enum7_chain(const DevProblem *__re
     int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
   enum7_body<NW, MODE, FORM, kSrcWhole, kShapeChain>(prob, ectl, ord, nullptr, 0u, counts, offsets,
       out, max_out, t_begin, t_end, part, nparts, tab, flt);
+}
+
+// The chain over the installed list (sbg_search7_chain): k_enum7's tickets and launch shape with
+// the chain's rows, key idx << 24 | k << 16 | po << 8 | pm.  A list entry holds at most 210 * 65,536
+// matches, within the u32 per-ticket counts.  Only the plain form's count and range passes exist:
+// the first-match search is all that runs it.
+template <int NW, int MODE>
+__global__ void __launch_bounds__(kThreads) k_enum7_chain_list(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, const uint64_t *__restrict__ list,
+    unsigned int list_count, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumNoFilter flt) {
+  static_assert(MODE == kEnumCount || MODE == kEnumRange, "the list-form chain counts and emits");
+  enum7_body<NW, MODE, kFormPlain, kSrcList, kShapeChain>(prob, ectl, ord, list, list_count, counts,
+      offsets, out, max_out, t_begin, t_end, part, nparts, tab, flt);
 }
 
 

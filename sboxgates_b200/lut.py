@@ -259,6 +259,16 @@ class LutEngine:
                                          _order_ptr(middle_order), C.byref(res)))
         return res
 
+    def search7_chain(self, outer_order, middle_order):
+        """The first 7-LUT chain L3(L2(L1(a,b,c), d, e), f, g) over the 7-LUT list search7 tries
+        (sbg_search7_chain; the installed list of the current problem, else phase 1 runs and
+        installs it): an SbgResult with key idx << 24 | k << 16 | po << 8 | pm, ordering = the chain
+        row k, gates a..g in chain-row order and L3's solved bits (see chain_result_luts)."""
+        res = SbgResult()
+        self._check(self.lib.sbg_search7_chain(self._h, _order_ptr(outer_order),
+                                               _order_ptr(middle_order), C.byref(res)))
+        return res
+
     # -- one call per node / batches of nodes --------------------------------------------------
     @staticmethod
     def _job(slot, order5=None, outer=None, middle=None, gate_order=None):
@@ -935,15 +945,31 @@ def chain_luts(match, rng_or_fill):
     if int(match["width"]) != 7 or int(match["shape"]) != SBG_SHAPE_CHAIN:
         raise ValueError("not a chain match (width %d, shape %d)"
                          % (int(match["width"]), int(match["shape"])))
+    return _chain_luts(match["func_outer"], match["func_middle"], match["func_inner"],
+                       match["inner_seen"], match["gates"], rng_or_fill)
+
+
+def chain_result_luts(res, rng_or_fill):
+    """A found chain result (LutEngine.search7_chain, an SbgResult) -> its three LUTs, as
+    chain_luts gives them for a match: [(L1, (a, b, c)), (L2, (("new", 0), d, e)),
+    (L3, (("new", 1), f, g))], L3 filled from rng_or_fill (an int or an rng, as there)."""
+    if not res.found:
+        raise ValueError("the chain search found nothing")
+    return _chain_luts(res.func_outer, res.func_middle, res.func_inner, res.inner_seen,
+                       res.gates, rng_or_fill)
+
+
+def _chain_luts(func_outer, func_middle, func_inner, inner_seen, gates, rng_or_fill):
+    """The three LUTs of a chain L3(L2(L1(a,b,c), d, e), f, g), gates a..g, with L3 filled."""
     if isinstance(rng_or_fill, (int, np.integer)):
         f3 = int(rng_or_fill)
-        if not 0 <= f3 < 256 or not inner_completes(match["func_inner"], match["inner_seen"], f3):
+        if not 0 <= f3 < 256 or not inner_completes(func_inner, inner_seen, f3):
             raise ValueError("function %d does not complete the inner LUT" % f3)
     else:
-        f3 = _fill(match["func_inner"], match["inner_seen"], rng_or_fill)
-    g = [int(x) for x in match["gates"]]
-    return [(int(match["func_outer"]), (g[0], g[1], g[2])),
-            (int(match["func_middle"]), (("new", 0), g[3], g[4])),
+        f3 = _fill(func_inner, inner_seen, rng_or_fill)
+    g = [int(x) for x in gates]
+    return [(int(func_outer), (g[0], g[1], g[2])),
+            (int(func_middle), (("new", 0), g[3], g[4])),
             (f3, (("new", 1), g[5], g[6]))]
 
 
@@ -1055,22 +1081,31 @@ def enumerate_lut_search(engine, tables, target, mask, inbits, gate_order, rng, 
 class LutSearchResult:
     """What lut_search() would add to the graph (lut.c:489-631): `luts` = the add_lut calls in
     order, each (function, in1, in2, in3) with inputs either gate numbers or ("new", k) = the k-th
-    LUT added by this call; `stage` = 3, 5, 7 or 0 (NO_GATE)."""
+    LUT added by this call; `stage` = 3, 5, 7 or 0 (NO_GATE); `shape` = how a stage-7 result wires
+    its three LUTs: "tree" (search_7lut's) or "chain" (lut_search(..., chain=True))."""
     stage: int
     luts: List[tuple] = field(default_factory=list)
     node: object = None
+    shape: str = "tree"
 
 
-def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=True, allow7=True):
+def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=True, allow7=True,
+               chain=False):
     """lut.c:489-631 as ONE device call: the 3-LUT scan over the caller's shuffled gate order
     (lut.c:501-523), search_5lut (lut.c:553) and search_7lut (lut.c:593), each only if the earlier
     ones found nothing.  allow5 / allow7 = check_num_gates_possible(st, 2 / 3) (lut.c:525, 582).
 
+    chain=True adds a stage the reference does not have: when search_7lut ran and found nothing,
+    the first 7-LUT chain L3(L2(L1(a,b,c), d, e), f, g) over the same list and orders
+    (LutEngine.search7_chain), returned as stage 7 with shape "chain" and luts [(L1, a, b, c),
+    (L2, ("new", 0), d, e), (L3, ("new", 1), f, g)].  A node without a chain gets exactly the result
+    and RNG state of chain=False.
+
     RNG: the reference draws 256 values on entry to search_5lut and 512 before phase 2 of
-    search_7lut, plus one per solved LUT with unseen cells (lut.c:104-106).  Which of those happen
-    depends on the stages' outcomes, so the shuffles are computed from a COPY of the generator
-    (looking ahead) and the real one is advanced afterwards by exactly what the reference would
-    have consumed."""
+    search_7lut, plus one per solved LUT with unseen cells (lut.c:104-106; the chain's L3 likewise).
+    Which of those happen depends on the stages' outcomes, so the shuffles are computed from a COPY
+    of the generator (looking ahead) and the real one is advanced afterwards by exactly what the
+    reference would have consumed."""
     n = len(tables)
     ahead = rng.copy()
     order5 = shuffled_order(ahead) if (allow5 and n >= 5) else None
@@ -1102,4 +1137,10 @@ def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=Tru
         # evaluates them right to left, so the MIDDLE LUT is added first (lower gate number)
         return LutSearchResult(7, [(r[1], r[6], r[7], r[8]), (r[0], r[3], r[4], r[5]),
                                    (r[2], ("new", 1), ("new", 0), r[9])], node)
+    if chain:
+        # the engine still holds this node's list (search_node installed it)
+        res = engine.search7_chain(outer, middle)
+        if res.found:
+            luts = [(f,) + ins for f, ins in chain_result_luts(res, rng)]
+            return LutSearchResult(7, luts, node, shape="chain")
     return LutSearchResult(0, [], node)

@@ -98,6 +98,7 @@ SIGNATURES = {
     "sbg_use_problem": (C.c_int, [C.c_void_p, C.c_int]),
     "sbg_search5": (C.c_int, [C.c_void_p, u8p, C.POINTER(SbgResult)]),
     "sbg_search7": (C.c_int, [C.c_void_p, u8p, u8p, C.POINTER(SbgResult)]),
+    "sbg_search7_chain": (C.c_int, [C.c_void_p, u8p, u8p, C.POINTER(SbgResult)]),
     "sbg_search5_part": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u64p]),
     "sbg_finish5": (C.c_int, [C.c_void_p, C.c_uint64, u8p, C.POINTER(SbgResult)]),
     "sbg_filter7_part": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u64p, C.POINTER(C.c_int)]),
