@@ -60,7 +60,8 @@ typedef struct sbg_handle sbg_handle;
 typedef struct {
   int32_t found;
   int32_t ordering;        /* k: 0..9 (lut.c:189-229) or 0..69 (lut.c:396-415); sbg_search7_chain:
-                              the chain row, 0..209 (sbg_chain_row) */
+                              the chain row, 0..209 (sbg_chain_row); sbg_search4_shared: the
+                              shared-input row, 0..11 (sbg_shared_row) */
   int32_t pos_outer;       /* position of func_outer in the shuffled order */
   int32_t pos_middle;      /* 7-LUT only */
   uint8_t func_outer;
@@ -161,6 +162,19 @@ int sbg_search7(sbg_handle *h, const uint8_t *outer_order /*256*/, const uint8_t
    problem loaded. */
 int sbg_search7_chain(sbg_handle *h, const uint8_t *outer_order /*256*/,
     const uint8_t *middle_order /*256*/, sbg_result *res);
+/* The first shared-input two-LUT circuit L2(L1(a,b,c), u, v), {u, v} = {s, d} with s one of a, b, c
+   (the shape of sbg_enum4_shared, which search_5lut never tries: its five gates are distinct), over
+   every 4-combination of the current problem, any n >= 4.  The result is sbg_enum4_shared's first
+   match (smallest key rank << 12 | k << 8 | po).  res: found, key, ordering = the row k (0..11),
+   pos_outer = po, func_outer = L1, func_inner / inner_seen = L2's solved bits and seen cells (cells
+   x1<<2 | u<<1 | v), gates[0..4] = a, b, c, u, v (add_lut's argument order, as for a 5-LUT result),
+   index = rank, tuples_feasible = the feasible 4-combinations met, tuples_swept = the
+   4-combinations of the 3-gate prefixes swept, inbits rejections included (C(n,4) on a miss; the
+   sweep stops in windows of prefixes once a match is known); nothing matched: found = 0, key =
+   SBG_KEY_NONE.  The caller applies L2's random fill and adds L1, then L2 over (L1, u, v).  The
+   depth, function and grouping settings are not read; the installed 7-LUT list stays as it was.
+   SBG_ERR_ARG: n < 4 or an order that is not a permutation; SBG_ERR_STATE: no problem loaded. */
+int sbg_search4_shared(sbg_handle *h, const uint8_t *func_order /*256*/, sbg_result *res);
 
 /* ---- one call per node, batches of independent nodes ----------------------------------------- */
 /* A job is what lut_search() does for one node (lut.c:489-631): the 3-LUT scan over the caller's
@@ -264,13 +278,15 @@ typedef struct {
   uint8_t func_middle;     /* 23: 7-LUT: the function at position key & 0xff of the middle order */
   uint8_t func_inner;      /* 24: solved bits only; don't-care bits are 0 (3-LUT: the LUT) */
   uint8_t inner_seen;      /* 25: bit c set = inner cell c occurs under the mask */
-  uint8_t width;           /* 26: 3, 5 or 7 */
+  uint8_t width;           /* 26: 3, 5 or 7; 4 for a shared-input circuit (sbg_enum4_shared) */
   uint8_t shape;           /* 27: how a 7-LUT match wires its LUTs, SBG_SHAPE_TREE (every call but
-                              sbg_enum7_chain, and widths 3 and 5) or SBG_SHAPE_CHAIN */
+                              sbg_enum7_chain and sbg_enum4_shared, and widths 3 and 5),
+                              SBG_SHAPE_CHAIN or SBG_SHAPE_SHARED */
   uint8_t pad[4];          /* 28: 0 */
 } sbg_match;
 #define SBG_SHAPE_TREE 0    /* L3(L1(a,b,c), L2(d,e,f), g): search_7lut's wiring */
 #define SBG_SHAPE_CHAIN 1   /* L3(L2(L1(a,b,c), d, e), f, g) */
+#define SBG_SHAPE_SHARED 2  /* L2(L1(a,b,c), u, v) over four gates, {u, v} = {s, d}, s in {a, b, c} */
 #define SBG_ENUM_MAX_MATCHES (1u << 24)   /* largest max_matches of one call */
 
 /* Enumerates the matches of the current problem in this part's share of the work (part/nparts as
@@ -331,6 +347,31 @@ int sbg_enum7_all(sbg_handle *h, int part, int nparts, const uint8_t *outer_orde
 int sbg_enum7_chain(sbg_handle *h, int part, int nparts, const uint8_t *outer_order,
     const uint8_t *middle_order, uint64_t max_matches, sbg_match *out, uint64_t *n_out,
     uint64_t *total, uint64_t *feasible);
+/* The two-LUT realisations search_5lut never tries: L2 reads one of L1's inputs again,
+   L2(L1(a,b,c), s, d) with s in {a, b, c}.  For each value of s, L1 may then compute a different
+   function of the other two, so the shape covers more than any circuit over five distinct gates.
+   Combinations: every 4-combination r0 < r1 < r2 < r3 in lexicographic order with no gate excluded
+   by inbits that passes check_n_lut_possible(4) (no cell of 16 holds a masked 1 and a masked 0).
+   Row k = 3 j + q (sbg_shared_row): j = the position of d, the gate L1 does not read; q = the index
+   of s among L1's three positions, ascending.  L1's cells are a<<2 | b<<1 | c, L1's gates
+   ascending; L2's are x1<<2 | u<<1 | v with (u, v) = {s, d} ascending.  A match is (combination, k,
+   po) with L1 = func_order[po] (search_5lut's shuffled order) for which L2 is solvable without a
+   random fill.  Key rank << 12 | k << 8 | po, rank = the combination's lexicographic rank among
+   C(n,4) (below 2^32 at n <= 500, so it reads as a 5-LUT key).  Record: width 4, shape
+   SBG_SHAPE_SHARED, gates[0..2] = a, b, c and gates[3..4] = u, v (add_lut's argument order: the
+   record reads as a 5-LUT one with s repeated), gates[5..6] = 0, func_outer = L1, func_inner /
+   inner_seen = L2's solved bits and seen cells.  Depth (sbg_enum_set_depth) 1 + max(1 + max(Da,
+   Db, Dc), Du, Dv); function filter: outer = L1, inner = L2 (middle plays no part); groupings:
+   SBG_GROUP_SHAPE key >> 8, SBG_GROUP_TUPLE key >> 12.  *feasible = the share's feasible
+   4-combinations (under a depth filter, those with a row within the bound).  part/nparts,
+   max_matches, the count-free first K, the cursor and its calls (fetch, pick, group sizes, depth
+   counts, global ranks) behave as for sbg_enum5; a share's tickets are 3-gate prefixes dealt in
+   blocks of 16, and the count buffers take 12 bytes per prefix, C(n-1, 3) of them (248 MB at
+   n = 500).  The call builds no list and leaves an installed one alone.  SBG_ERR_ARG: n < 4, an
+   order that is not a permutation, or a depth filter of another n; SBG_ERR_STATE: no problem
+   loaded.  The call ends the cursor, whatever it returns. */
+int sbg_enum4_shared(sbg_handle *h, int part, int nparts, const uint8_t *func_order,
+    uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible);
 /* The matches of lut_search's 3-LUT scan (lut.c:501-523) over the caller's shuffled gate order
    (n entries): the position triples i < k < m whose gates gate_order[i], gate_order[k],
    gate_order[m] pass check_n_lut_possible(3, ...) under the mask (get_lut_function then cannot
@@ -350,7 +391,8 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
     uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible);
 
 /* ---- matches at any rank: the enumeration cursor ---------------------------------------------- */
-/* The cursor is the last sbg_enum3 / sbg_enum5 / sbg_enum7 / sbg_enum7_all / sbg_enum7_chain call
+/* The cursor is the last sbg_enum3 / sbg_enum4_shared / sbg_enum5 / sbg_enum7 / sbg_enum7_all /
+   sbg_enum7_chain call
    on the handle that counted
    (total != NULL; max_matches may be 0).  Ranks are positions in that call's share (part/nparts),
    in ascending key order: 0 .. total-1.  The device keeps what that count found (matches per
@@ -361,7 +403,7 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
    it was counted with; the caller's buffers of that call are not read again.  Cursor lifetime:
      - a counted sbg_enum* call replaces it; a count-free one ends it;
      - any call of sbg_load_problem, sbg_stage_problem, sbg_use_problem, sbg_search5, sbg_search7,
-       sbg_search7_chain, sbg_search_node, sbg_search_batch, sbg_search5_part, sbg_finish5, sbg_filter7_part,
+       sbg_search7_chain, sbg_search4_shared, sbg_search_node, sbg_search_batch, sbg_search5_part, sbg_finish5, sbg_filter7_part,
        sbg_set_list7, sbg_list7_device, sbg_set_list7_device, sbg_allgather_merge7 (every handle
        given), sbg_decomp7_part, sbg_finish7 or sbg_alu_peak ends it, whatever the call returns;
      - sbg_last_error, sbg_launch_count, sbg_transfer_stats, sbg_host_seconds, sbg_last_kernel_ms,
@@ -372,7 +414,8 @@ int sbg_enum3(sbg_handle *h, int part, int nparts, const uint16_t *gate_order,
      - sbg_enum_set_grouping ends it, whatever the call returns.
    Without a cursor both calls return SBG_ERR_STATE.
    A fetch or pick does the emit work of every ticket it touches up to the last wanted rank in it:
-   a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT), a list
+   a ticket is a position pair (3-LUT, up to n - 2 matches), a 3-gate prefix (5-LUT; shared-input:
+   up to n - 3 combinations of 12 * 256 matches), a list
    entry (7-LUT, up to 70 * 65,536 matches) or a 6-gate prefix (sbg_enum7_all, up to n - 7
    combinations of that many; sbg_enum7_chain, of 210 * 65,536), so one deep rank can cost a whole
    ticket's sweep. */
@@ -425,7 +468,8 @@ int sbg_enum_set_global(sbg_handle *h, const uint64_t *sums, uint64_t stride,
      3-LUT a,b,c:     1 + max(Da, Db, Dc);
      5-LUT a..e:      1 + max(1 + max(Da, Db, Dc), Dd, De)            (outer LUT over a,b,c);
      7-LUT a..g:      1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df), Dg);
-     7-LUT chain a..g: 1 + max(1 + max(1 + max(Da, Db, Dc), Dd, De), Df, Dg) (sbg_enum7_chain).
+     7-LUT chain a..g: 1 + max(1 + max(1 + max(Da, Db, Dc), Dd, De), Df, Dg) (sbg_enum7_chain);
+     shared-input a..c, u, v: 1 + max(1 + max(Da, Db, Dc), Du, Dv)    (sbg_enum4_shared).
    Under a filter the matches of sbg_enum3 / sbg_enum5 / sbg_enum7 are exactly the unfiltered
    matches of depth <= max_depth: keys, key order and records are unchanged, only the set shrinks,
    and ranks are ranks within it.  The 7-LUT list is still the phase-1 list (the first
@@ -485,6 +529,7 @@ int sbg_inner_table(const uint64_t *inner, uint8_t *out);
    sharing a key prefix,
      SBG_GROUP_SHAPE: the gates and the ordering row (the wiring): 5-LUT key >> 8, 7-LUT key >> 16;
      SBG_GROUP_TUPLE: the gate set: 5-LUT key >> 12, 7-LUT key >> 23 (chain: key >> 24).
+   A shared-input key (sbg_enum4_shared) groups as a 5-LUT key: >> 8 (shape), >> 12 (tuple).
    A 3-LUT key already is its gate set and wiring, so at width 3 every grouping is the identity.
    The total is the number of groups holding at least one match (after the depth and function
    filters); each group has one record, its first match (smallest key), byte-identical to the
@@ -542,6 +587,9 @@ int sbg_weighted_tickets(int n, uint32_t group_pairs, uint32_t *out);
 int sbg_ordering_row(int width, int k, int *row);
 /* Chain row k < 210 of sbg_enum7_chain: the seven positions in record order a..g. */
 int sbg_chain_row(int k, int *row);
+/* Shared-input row k < 12 of sbg_enum4_shared: the five positions (0..3 in the combination) in
+   record order a, b, c, u, v; one of u, v repeats one of a, b, c. */
+int sbg_shared_row(int k, int *row);
 /* Closed form of get_lut_function without the random fill (lut.c:79-103): returns 1 and the
    solved function / seen mask, or 0 on conflict. */
 int sbg_solve_inner(const uint64_t *in1, const uint64_t *in2, const uint64_t *in3,

@@ -34,7 +34,15 @@ _Static_assert(offsetof(sbg_options, randomize) == 2019 && offsetof(sbg_options,
    L3(L2(L1(a,b,c), d, e), f, g) over the same 7-combinations and function orders
    (sbg_search7_chain) is built from three add_lut calls, where the reference would go on to
    multiplexer recursion.  A node without a chain leaves the state and the random stream exactly as
-   without the variable; a node with one takes only L3's don't-care fill from the generator. */
+   without the variable; a node with one takes only L3's don't-care fill from the generator.
+   SBG_LUT_SHARED=1 (node variant; default off) adds another such stage, between search_5lut and
+   search_7lut: when search_5lut ran and found nothing, the first two-LUT circuit whose L2 reads one
+   of L1's inputs again, L2(L1(a,b,c), u, v) with {u, v} = {s, d} and s in {a, b, c}
+   (sbg_search4_shared, over every 4-combination, under search_5lut's function order), is built
+   from two add_lut calls.  search_7lut (and the chain stage) then run only if it finds nothing, so
+   with the variable set a node's device call stops after search_5lut.  A node without such a
+   circuit leaves the state and the random stream exactly as without the variable; a node with one
+   takes only L2's don't-care fill from the generator (search_7lut's 512 draws do not happen). */
 #define SBG_SHIM_MAX_GPUS 8
 static sbg_handle *g_handles[SBG_SHIM_MAX_GPUS];
 static int g_ngpus = 0;
@@ -44,11 +52,14 @@ static uint64_t g_sharded_calls = 0;
 #define g_handle (g_handles[0])
 static uint64_t g_calls[3] = {0, 0, 0};          /* search_5lut, search_7lut, lut_search */
 static double g_seconds[3] = {0.0, 0.0, 0.0};
-static uint64_t g_node_stage[5] = {0, 0, 0, 0, 0};  /* node calls that ended at: nothing, 3, 5, 7,
-                                                      the 7-LUT chain */
+static uint64_t g_node_stage[6] = {0, 0, 0, 0, 0, 0};  /* node calls that ended at: nothing, 3, 5,
+                                                         7, the 7-LUT chain, the shared-input pair */
 static int g_lut_chain = 0;                         /* SBG_LUT_CHAIN */
 static uint64_t g_chain_calls = 0;                  /* sbg_search7_chain calls and their seconds */
 static double g_chain_seconds = 0.0;
+static int g_lut_shared = 0;                        /* SBG_LUT_SHARED */
+static uint64_t g_shared_calls = 0;                 /* sbg_search4_shared calls and their seconds */
+static double g_shared_seconds = 0.0;
 static double g_kernel_ms[4] = {0.0, 0.0, 0.0, 0.0}; /* search5, filter7, ordering, decomp7 */
 static int g_stats = 0;
 
@@ -156,18 +167,24 @@ static void shim_exit(void) {
   if (g_stats) {
     uint64_t tr[5] = {0, 0, 0, 0, 0};
     sbg_transfer_stats(g_handle, tr);
-    char chain_col[64] = "";   /* only with SBG_LUT_CHAIN, so the default line stays as it was */
+    /* only with SBG_LUT_CHAIN / SBG_LUT_SHARED, so the default line stays as it was */
+    char chain_col[64] = "", shared_col[64] = "";
     if (g_lut_chain) {
       snprintf(chain_col, sizeof(chain_col), ", 7-LUT chain %llu",
           (unsigned long long)g_node_stage[4]);
     }
+    if (g_lut_shared) {
+      snprintf(shared_col, sizeof(shared_col), ", shared-input pair %llu",
+          (unsigned long long)g_node_stage[5]);
+    }
     fprintf(stderr, "[sbg] start-up (sbg_create) %.3f s, inside the first call; "
-        "lut_search: %llu calls %.3f s (ended at: 3-LUT %llu, 5-LUT %llu, 7-LUT %llu%s, nothing %llu); "
+        "lut_search: %llu calls %.3f s (ended at: 3-LUT %llu, 5-LUT %llu%s, 7-LUT %llu%s, nothing %llu); "
         "search_5lut: %llu calls %.3f s; search_7lut: %llu calls %.3f s; "
         "%llu kernel launches; state changes: %llu bulk copies, %llu as kernel arguments, %llu none; "
         "%llu B host->device, %llu B device->host\n", g_init_seconds,
         (unsigned long long)g_calls[2], g_seconds[2], (unsigned long long)g_node_stage[1],
-        (unsigned long long)g_node_stage[2], (unsigned long long)g_node_stage[3], chain_col,
+        (unsigned long long)g_node_stage[2], shared_col, (unsigned long long)g_node_stage[3],
+        chain_col,
         (unsigned long long)g_node_stage[0], (unsigned long long)g_calls[0], g_seconds[0],
         (unsigned long long)g_calls[1], g_seconds[1],
         (unsigned long long)sbg_launch_count(g_handle), (unsigned long long)tr[2],
@@ -182,6 +199,10 @@ static void shim_exit(void) {
     }
     fprintf(stderr, "[sbg] waiting by stage: 3-LUT scan %.3f s, search_5lut %.3f s, search_7lut "
         "%.3f s\n", hs[2], hs[3], hs[4]);
+    if (g_lut_shared) {
+      fprintf(stderr, "[sbg] shared-input stage: %llu calls %.3f s, %llu nodes took a pair\n",
+          (unsigned long long)g_shared_calls, g_shared_seconds, (unsigned long long)g_node_stage[5]);
+    }
     if (g_lut_chain) {
       fprintf(stderr, "[sbg] 7-LUT chain stage: %llu calls %.3f s, %llu nodes took a chain\n",
           (unsigned long long)g_chain_calls, g_chain_seconds, (unsigned long long)g_node_stage[4]);
@@ -216,6 +237,7 @@ static sbg_handle *handle(void) {
     }
     g_stats = getenv("SBG_SHIM_STATS") != NULL;
     g_lut_chain = getenv("SBG_LUT_CHAIN") != NULL && atoi(getenv("SBG_LUT_CHAIN")) != 0;
+    g_lut_shared = getenv("SBG_LUT_SHARED") != NULL && atoi(getenv("SBG_LUT_SHARED")) != 0;
     for (int i = 0; i < want; i++) {
       int rc = sbg_create(&g_handles[i], first + i);
       if (rc != SBG_OK) {
@@ -547,7 +569,9 @@ uint16_t lut_search(sbg_state *st, const sbg_ttable target, const sbg_ttable mas
   static int split = -1;
   if (split < 0) split = getenv("SBG_NODE_SPLIT") != NULL && atoi(getenv("SBG_NODE_SPLIT")) != 0;
   const bool chain5 = do5 && n >= 5 && !big5 && !split;
-  const bool chain7 = chain5 && do7 && n >= 7 && !big7;
+  /* with SBG_LUT_SHARED the shared-input stage sits between search_5lut and search_7lut, so the
+     device call stops after search_5lut */
+  const bool chain7 = chain5 && do7 && n >= 7 && !big7 && !g_lut_shared;
   if (chain5) {
     job.flags |= SBG_DO_SEARCH5;
     job.order5 = order5;
@@ -566,6 +590,7 @@ uint16_t lut_search(sbg_state *st, const sbg_ttable target, const sbg_ttable mas
   uint16_t out = SBG_SHIM_NO_GATE;
   int stage = 0;
   bool chained = false;   /* the node took the 7-LUT chain (SBG_LUT_CHAIN) */
+  bool shared = false;    /* the node took the shared-input pair (SBG_LUT_SHARED) */
   if (nr.found_stage == 3) { /* lut.c:501-523 */
     const uint16_t gi = nr.gates3[0], gk = nr.gates3[1], gm = nr.gates3[2];
     uint8_t func = nr.func3;
@@ -612,6 +637,35 @@ uint16_t lut_search(sbg_state *st, const sbg_ttable target, const sbg_ttable mas
       goto done;
     }
     trace_call(5, st, target, mask, false, NULL);
+    if (g_lut_shared) {
+      /* not in the reference: the first two-LUT circuit whose L2 reads one of L1's inputs again,
+         under search_5lut's function order, before search_7lut runs */
+      const double ts = now();
+      sbg_result rs;
+      rc = sbg_search4_shared(h, order5, &rs);
+      if (rc != SBG_OK) die("sbg_search4_shared", rc, h);
+      g_shared_calls++;
+      g_shared_seconds += now() - ts;
+      if (rs.found) {
+        const uint16_t *g = rs.gates;
+        const uint8_t l1 = rs.func_outer;
+        const uint8_t l2 = fill_dont_cares(rs.func_inner, rs.inner_seen);
+        if (opt->verbosity >= 1) {
+          printf("[   0]   Selected shared: %02x %02x    %3d %3d %3d %3d %3d\n", l1, l2, g[0], g[1],
+              g[2], g[3], g[4]);
+        }
+        const sbg_ttable t1 = generate_lut_ttable(l1, st->gates[g[0]].table,
+            st->gates[g[1]].table, st->gates[g[2]].table);
+        const sbg_ttable t2 = generate_lut_ttable(l2, t1, st->gates[g[3]].table,
+            st->gates[g[4]].table);
+        require(ttable_equals_mask(target, t2, mask), __LINE__);
+        const uint16_t g1 = add_lut(st, l1, t1, g[0], g[1], g[2]);
+        out = checked(add_lut(st, l2, t2, g1, g[3], g[4]), st, target, mask, __LINE__);
+        stage = 5;
+        shared = true;
+        goto done;
+      }
+    }
   }
   if (!do7) goto done; /* lut.c:582-586 */
 
@@ -697,7 +751,7 @@ uint16_t lut_search(sbg_state *st, const sbg_ttable target, const sbg_ttable mas
     printf("[   0] No LUTs found. Num gates: %d\n", st->num_gates - get_num_inputs(st));
   }
 done:
-  g_node_stage[chained ? 4 : stage == 0 ? 0 : (stage - 1) / 2]++;
+  g_node_stage[shared ? 5 : chained ? 4 : stage == 0 ? 0 : (stage - 1) / 2]++;
   g_seconds[2] += now() - t0;
   return out;
 }

@@ -26,6 +26,7 @@ namespace {
 uint64_t h_binom[501][8];
 int h_rows7[70][7];
 int h_rows7c[210][7];
+int h_rows4s[12][5];
 int h_rows5[10][5];
 bool g_tables_ready = false;
 
@@ -87,6 +88,22 @@ void build_host_tables() {
       for (int i = 0; i < 4; i++) {
         if (i != d && i != e) row[w++] = rest[i];
       }
+    }
+  }
+  // shared-input rows (sbg_shared_row): k = 3 j + q, j = the position of d (the gate L1 does not
+  // read), q = the index of the shared gate s among L1's three positions; record order: L1's
+  // positions ascending, then {s, d} ascending.
+  k = 0;
+  for (int j = 0; j < 4; j++) {
+    int l1[3], r = 0;
+    for (int i = 0; i < 4; i++) {
+      if (i != j) l1[r++] = i;
+    }
+    for (int q = 0; q < 3; q++) {
+      int *row = h_rows4s[k++];
+      row[0] = l1[0]; row[1] = l1[1]; row[2] = l1[2];
+      row[3] = std::min(l1[q], j);
+      row[4] = std::max(l1[q], j);
     }
   }
   g_tables_ready = true;
@@ -1608,13 +1625,14 @@ int copy_matches(sbg_handle *h, sbg_lane &L, sbg_match *out, uint64_t n) {
   return SBG_OK;
 }
 
-// One enumeration pass (MODE: count, range or pick emit, or sizes) of width 3, 5 or 7 over
-// tickets [a, b) of the lane's problem (pick and sizes: entries [a, b) of the ticket list in
-// EnumCtl::sel).
+// One enumeration pass (MODE: count, range or pick emit, or sizes) of width 3, 4 (the shared-input
+// two-LUT circuits of sbg_enum4_shared), 5 or 7 over tickets [a, b) of the lane's problem (pick and
+// sizes: entries [a, b) of the ticket list in EnumCtl::sel).
 template <int WIDTH, int MODE>
 int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int nparts,
     uint64_t max_out, uint64_t a, uint64_t b) {
-  static_assert(WIDTH == 3 || WIDTH == 5 || WIDTH == 7, "enumeration widths are 3, 5 and 7");
+  static_assert(WIDTH == 3 || WIDTH == 4 || WIDTH == 5 || WIDTH == 7,
+      "enumeration widths are 3, 4, 5 and 7");
   const sbg_handle::HostProblem &hp = h->slots[L.slot];
   const int n = hp.n;
   const DevProblem *prob = h->d_slots.p + L.slot;
@@ -1639,6 +1657,10 @@ int launch_enum(sbg_handle *h, sbg_lane &L, const EnumInputs &in, int part, int 
       if constexpr (WIDTH == 3) {
         return run(k_enum3<NW, MODE, FORM>, decomp_smem<NW>(n), prob, E.d_ectl.p, in.gates,
             E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, flt);
+      } else if constexpr (WIDTH == 4) {
+        return run(k_enum4s<NW, MODE, FORM>, sweep_smem<NW>(n), prob, E.d_ectl.p, in.ord,
+            E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, h->d_tab.p,
+            flt);
       } else if constexpr (WIDTH == 5) {
         return run(k_enum5<NW, MODE, FORM>, sweep_smem<NW>(n), prob, E.d_ectl.p, in.ord,
             E.d_ecount.p, E.d_eoffset.p, E.d_ematch.p, max_out, a, b, part, nparts, h->d_tab.p,
@@ -1687,20 +1709,22 @@ uint64_t deal_share(uint64_t blocks, int q, int nparts) {
 }
 
 // Tickets per deal block of an enumeration of `width` from `source` (Enum7Source): kDeal position
-// pairs, 3-gate prefixes or 6-gate prefixes, or one 7-LUT list entry.
+// pairs, 3-gate prefixes (widths 4 and 5) or 6-gate prefixes, or one 7-LUT list entry.
 unsigned int enum_block_size(int width, int source) {
   return width == 7 && source == kSrcList ? 1u : (unsigned)kDeal;
 }
 
-// sbg_enum3 / sbg_enum5 / sbg_enum7 / sbg_enum7_all / sbg_enum7_chain once their arguments are checked.  Lane 0
+// sbg_enum3 / sbg_enum4_shared / sbg_enum5 / sbg_enum7 / sbg_enum7_all / sbg_enum7_chain once their
+// arguments are checked.  Lane 0
 // takes the current problem slot, and k_begin (flags, begin_in) brings its problem block up to date;
 // a 7-LUT enumeration over the list without an installed one runs phase 1 instead, which does that
 // and installs the list.  Then the part's tickets are counted (in windows when only the first
 // max_matches are wanted), their offsets taken, and the first max_matches emitted and copied out.
+// *swept (may be NULL): the tickets the count went through, all of the part's when counting.
 template <int WIDTH>
 int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const EnumInputs &in,
     int part, int nparts, uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total,
-    uint64_t *feasible) {
+    uint64_t *feasible, uint64_t *swept = nullptr) {
   SBG_CUDA(h, cudaSetDevice(h->device));
   sbg_lane &L = h->lane[0];
   EnumBuffers &E = h->ebuf;
@@ -1719,8 +1743,8 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   // this part's tickets: its deal blocks (the last one may be cut short)
   const int n = h->slots[L.slot].n;
   const uint64_t B = enum_block_size(WIDTH, in.source);
-  const uint64_t items = WIDTH == 3 ? h_binom[n][2] : WIDTH == 5 ? h_binom[n - 2][3]
-      : whole ? h_binom[n - 1][6] : h->list7.count;
+  const uint64_t items = WIDTH == 3 ? h_binom[n][2] : WIDTH == 4 ? h_binom[n - 1][3]
+      : WIDTH == 5 ? h_binom[n - 2][3] : whole ? h_binom[n - 1][6] : h->list7.count;
   const uint64_t blocks = (items + B - 1) / B;
   const uint64_t tickets = deal_share(blocks, part, nparts) * B;
   if ((rc = E.d_ectl.grow(h, L.stream, 1)) != SBG_OK) return rc;
@@ -1735,7 +1759,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
   }
   const bool count_all = total != nullptr;
   uint64_t window = count_all ? tickets
-      : (WIDTH == 3 ? kEnumWindow3 : WIDTH == 5 ? kEnumWindow5
+      : (WIDTH == 3 ? kEnumWindow3 : WIDTH == 4 || WIDTH == 5 ? kEnumWindow5
          : whole ? kEnumWindow7All : kEnumWindow7);
   uint64_t done = 0;
   EnumCtl ec;
@@ -1763,6 +1787,7 @@ int run_enum(sbg_handle *h, uint32_t flags, const CallInputs &begin_in, const En
     if ((rc = copy_matches(h, L, out, emit)) != SBG_OK) return rc;
   }
   *n_out = emit;
+  if (swept != nullptr) *swept = done;
   if (count_all) {
     // every ticket counted: any rank of the share can be emitted again from counts and offsets
     EnumCursor &c = h->cursor;
@@ -1915,7 +1940,7 @@ int block_sums(sbg_handle *h, sbg_lane &L, uint64_t nblocks) {
 
 // A range or pick emit pass of the cursor's width over tickets [a, b) (pick: entries [a, b) of
 // sel.tickets) into d_ematch, or the sizes pass over entries [a, b) of sel.tickets into d_psizes
-// (grouped cursors of widths 5 and 7 only); sel and the sizes pointer travel in the EnumCtl block.
+// (grouped cursors of widths 4, 5 and 7 only); sel and the sizes pointer travel in the EnumCtl block.
 template <int MODE>
 int emit_sel(sbg_handle *h, sbg_lane &L, uint64_t max_out, uint64_t a, uint64_t b,
     const EnumSel &sel) {
@@ -1927,11 +1952,13 @@ int emit_sel(sbg_handle *h, sbg_lane &L, uint64_t max_out, uint64_t a, uint64_t 
     unsigned long long *sizes = h->ebuf.d_psizes.p;
     SBG_CUDA(h, cudaMemcpyAsync(ectl + offsetof(EnumCtl, sizes), &sizes, sizeof(sizes),
         cudaMemcpyHostToDevice, L.stream));
+    if (c.width == 4) return launch_enum<4, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
     if (c.width == 5) return launch_enum<5, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
     return launch_enum<7, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
   } else {
     switch (c.width) {
       case 3: return launch_enum<3, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
+      case 4: return launch_enum<4, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
       case 5: return launch_enum<5, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
       default: return launch_enum<7, MODE>(h, L, c.in, c.part, c.nparts, max_out, a, b);
     }
@@ -2116,6 +2143,13 @@ int sbg_chain_row(int k, int *row) {
   build_host_tables();
   if (row == nullptr || k < 0 || k >= 210) return SBG_ERR_ARG;
   for (int i = 0; i < 7; i++) row[i] = h_rows7c[k][i];
+  return SBG_OK;
+}
+
+int sbg_shared_row(int k, int *row) {
+  build_host_tables();
+  if (row == nullptr || k < 0 || k >= 12) return SBG_ERR_ARG;
+  for (int i = 0; i < 5; i++) row[i] = h_rows4s[k][i];
   return SBG_OK;
 }
 
@@ -2339,6 +2373,9 @@ int sbg_create(sbg_handle **out, int device) {
     uint8_t rows7c[210][7];
     for (int k = 0; k < 210; k++) for (int i = 0; i < 7; i++) rows7c[k][i] = (uint8_t)h_rows7c[k][i];
     SBG_CUDA(h, cudaMemcpyToSymbol(c_rows7c, rows7c, sizeof(rows7c)));
+    uint8_t rows4s[12][5];
+    for (int k = 0; k < 12; k++) for (int i = 0; i < 5; i++) rows4s[k][i] = (uint8_t)h_rows4s[k][i];
+    SBG_CUDA(h, cudaMemcpyToSymbol(c_rows4s, rows4s, sizeof(rows4s)));
   }
 
   if ((rc = h->d_slots.grow(h, h->lane[0].stream, kSlots)) != SBG_OK) return rc;
@@ -3026,6 +3063,84 @@ int sbg_search7_chain(sbg_handle *h, const uint8_t *outer_order, const uint8_t *
       &res->func_inner, &res->inner_seen) || res->func_inner != m.func_inner
       || res->inner_seen != m.inner_seen) {
     return fail(h, SBG_ERR_STATE, "internal: the first chain match does not decompose");
+  }
+  return SBG_OK;
+}
+
+// The shared-input two-LUT enumeration's inputs: the 5-LUT function order, no middle order.
+int shared_inputs(sbg_handle *h, const uint8_t *func_order, EnumInputs &in4) {
+  if (cur(h).n < 4) return fail(h, SBG_ERR_ARG, "the shared-input two-LUT circuits need n >= 4");
+  if (!valid_order(func_order)) return fail(h, SBG_ERR_ARG, "func_order is not a permutation");
+  memcpy(in4.ord.order[0], func_order, 256);
+  memset(in4.ord.order[1], 0, 256);
+  in4.source = kSrcList;
+  in4.shape = kShapeShared;
+  return SBG_OK;
+}
+
+int sbg_enum4_shared(sbg_handle *h, int part, int nparts, const uint8_t *func_order,
+    uint64_t max_matches, sbg_match *out, uint64_t *n_out, uint64_t *total, uint64_t *feasible) {
+  int rc;
+  if ((rc = check_enum_args(h, part, nparts, max_matches, out, n_out)) != SBG_OK) return rc;
+  EnumInputs in4;
+  if ((rc = shared_inputs(h, func_order, in4)) != SBG_OK) return rc;
+  if ((rc = take_filter(h, 4, in4)) != SBG_OK) return rc;
+  // only bring the problem block up to date: an installed 7-LUT list and its control words stay
+  return run_enum<4>(h, kBeginKeepCtl, CallInputs(), in4, part, nparts, max_matches, out, n_out,
+      total, feasible);
+}
+
+// The first shared-input match: run_enum's count-free first K with K = 1 (windows of 3-gate
+// prefixes that double until a match is known), then the record turned into an sbg_result.
+int sbg_search4_shared(sbg_handle *h, const uint8_t *func_order, sbg_result *res) {
+  if (h == nullptr || res == nullptr) return SBG_ERR_ARG;
+  h->api_seq++;   // ends the enumeration cursor
+  if (!h->problem_ready) return fail(h, SBG_ERR_STATE, "no problem loaded");
+  EnumInputs in4;
+  int rc;
+  if ((rc = shared_inputs(h, func_order, in4)) != SBG_OK) return rc;
+  in4.form = kFormPlain;   // the depth, function and grouping settings are not read
+  memset(&in4.filter, 0, sizeof(in4.filter));
+  sbg_match m;
+  uint64_t found = 0, feasible = 0, prefixes = 0;
+  rc = run_enum<4>(h, kBeginKeepCtl, CallInputs(), in4, 0, 1, 1, &m, &found, nullptr, &feasible,
+      &prefixes);
+  if (rc != SBG_OK) return rc;
+  const sbg_handle::HostProblem &hp = cur(h);
+  const int n = hp.n;
+  memset(res, 0, sizeof(*res));
+  res->key = SBG_KEY_NONE;
+  res->tuples_feasible = feasible;
+  // the 4-combinations of the prefixes swept: those ranked below the first one of prefix
+  // `prefixes` (the prefixes are the 3-combinations of 0..n-2 in lexicographic order)
+  res->tuples_swept = h_binom[n][4];
+  if (prefixes < h_binom[n - 1][3]) {
+    uint16_t pre[3];
+    unrank_combination(prefixes, n - 1, 3, pre);
+    uint64_t rank = 0;
+    int x = 0;
+    for (int pos = 0; pos < 3; pos++) {
+      for (; x < pre[pos]; x++) rank += h_binom[n - x - 1][3 - pos];
+      x++;
+    }
+    res->tuples_swept = rank;
+  }
+  if (found == 0) return SBG_OK;
+  res->found = 1;
+  res->key = m.key;
+  res->index = m.key >> 12;
+  res->ordering = (int)((m.key >> 8) & 0xf);
+  res->pos_outer = (int)(m.key & 0xff);
+  res->func_outer = m.func_outer;
+  for (int i = 0; i < 5; i++) res->gates[i] = m.gates[i];
+  // L2's solved bits from the host's tables, as finish5 does for search_5lut
+  uint64_t x1[4];
+  sbg_lut_table(m.func_outer, hp.tables[m.gates[0]], hp.tables[m.gates[1]], hp.tables[m.gates[2]],
+      x1);
+  if (!sbg_solve_inner(x1, hp.tables[m.gates[3]], hp.tables[m.gates[4]], hp.target, hp.mask,
+      &res->func_inner, &res->inner_seen) || res->func_inner != m.func_inner
+      || res->inner_seen != m.inner_seen) {
+    return fail(h, SBG_ERR_STATE, "internal: the first shared-input match does not decompose");
   }
   return SBG_OK;
 }

@@ -117,7 +117,9 @@ struct DevParams7 {
 
 // How a 7-LUT match wires its three LUTs (SBG_SHAPE_TREE, SBG_SHAPE_CHAIN): the tree
 // L3(L1(a,b,c), L2(d,e,f), g) of search_7lut, or the chain L3(L2(L1(a,b,c), d, e), f, g).
-enum Enum7Shape : int { kShapeTree = 0, kShapeChain = 1 };
+// kShapeShared (SBG_SHAPE_SHARED) is the two-LUT circuit L2(L1(a,b,c), u, v) over four gates whose
+// L2 reads one of L1's inputs again (sbg_enum4_shared).
+enum Enum7Shape : int { kShapeTree = 0, kShapeChain = 1, kShapeShared = 2 };
 
 // Lane-indexed lookup tables live in global memory (coalesced, L1-resident): a constant-memory load
 // whose address differs per lane is replayed once per distinct address.
@@ -2925,7 +2927,8 @@ __device__ __forceinline__ uint32_t lut_word(uint32_t func, uint32_t x, uint32_t
 }
 
 // A match's record of width 3, 5 or 7: the first WIDTH gates of G, zeros in the fields the width
-// does not use (func_outer at width 3, func_middle below width 7).
+// does not use (func_outer at width 3, func_middle below width 7).  A shared-input record is laid
+// out as a 5-LUT one (WIDTH 5, a repeated gate among a..e) with width 4, its number of gates.
 template <int WIDTH, int SHAPE = kShapeTree>
 __device__ __forceinline__ void store_match(DevMatch *__restrict__ dst, unsigned long long key,
     const int *G, uint32_t fo, uint32_t fm, uint32_t inner, uint32_t seen) {
@@ -2937,7 +2940,7 @@ __device__ __forceinline__ void store_match(DevMatch *__restrict__ dst, unsigned
   m.func_middle = WIDTH == 7 ? (uint8_t)fm : (uint8_t)0;
   m.func_inner = (uint8_t)inner;
   m.inner_seen = (uint8_t)seen;
-  m.width = (uint8_t)WIDTH;
+  m.width = (uint8_t)(SHAPE == kShapeShared ? 4 : WIDTH);
 #pragma unroll
   for (int i = 0; i < 5; i++) m.pad[i] = i == 0 ? (uint8_t)SHAPE : (uint8_t)0;
   *dst = m;
@@ -3419,6 +3422,253 @@ __global__ void __launch_bounds__(kThreads) k_enum5(const DevProblem *__restrict
     unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
     int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
   enum5_body<NW, MODE, FORM>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
+      part, nparts, tab, flt);
+}
+
+// ---- shared-input two-LUT circuits (sbg_enum4_shared) --------------------------------------------
+// L2(L1(a,b,c), u, v) over a 4-combination r0 < r1 < r2 < r3, where {u, v} = {s, d}: d is the gate
+// L1 does not read and s is one of L1's three.  Row k = 3 j + q (sbg_shared_row): d at position j,
+// s the q-th of L1's positions.  c_rows4s[k] holds the row's positions in record order a, b, c, u, v
+// (L1's ascending, then u < v).  For one row this is search_5lut's decomposition test on the
+// 5-tuple (a, b, c, u, v) with s repeated, at ordering row 0 (identity): summary5 leaves the cells
+// where the two copies of s disagree empty, and outer_ok5 then decides L1 exactly.
+__constant__ uint8_t c_rows4s[12][5];
+
+// The sweep of one part, tickets t_begin .. t_end-1: a ticket is a 3-gate prefix of the
+// 4-combinations, dealt in blocks of kDeal as k_enum5 deals its prefixes, and the lanes take the
+// last gate d.  A combination passes when no gate is excluded by inbits and no cell of its 16 holds
+// a masked 1 and a masked 0 (the mixed prefix cells split by d).  Per feasible combination the 12
+// rows run as enum5_body's orderings do, with the same filter, grouping and emit steps; key
+// rank << 12 | k << 8 | po.  A ticket holds at most (n - 3) * 12 * 256 < 2^32 matches.  Depth (the
+// filtered forms) 1 + max(1 + max(Da, Db, Dc), Du, Dv): a match needs every gate below the bound
+// and at most one at bound - 1 (then as d), and every combination with that has a row within the
+// bound, so the pruning is exact and `feasible` counts the combinations with such a row.
+template <int NW, int MODE, int FORM>
+__device__ __forceinline__ void enum4s_body(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders &ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> &flt) {
+  constexpr bool FILTER = FORM != kFormPlain, GR = FORM == kFormGrouped;
+  constexpr int P = 3, K = 4, NC = 1 << P;
+  extern __shared__ uint32_t smem[];
+  __shared__ uint8_t s_ord[256];
+  const int n = prob->n;
+  const int npad = (n + 3) & ~3;
+  uint32_t *s_tabs = smem;
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  uint32_t *cells = smem + NW * npad + warp * (NC * 2 * NW);  // per prefix cell: C1[NW], C0[NW]
+  stage_tables(s_tabs, prob, NW, npad);
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) s_ord[i] = ord.order[0][i];
+  const uint16_t *s_dep = nullptr;
+  const uint32_t *s_fn = nullptr;
+  int B = 0;
+  bool inner_all = true;
+  if constexpr (FILTER) {
+    stage_filter<MODE>(flt, n, s_dep, s_fn);
+    B = flt.max_depth;
+    inner_all = flt.inner_all != 0;
+  }
+  __syncthreads();
+  uint32_t T[NW], M[NW];
+#pragma unroll
+  for (int w = 0; w < NW; w++) {
+    T[w] = prob->T[w];
+    M[w] = prob->M[w];
+  }
+  const uint32_t inmask = prob->inmask;
+  const uint64_t total = c_binom[n - 1][P];
+
+  enum_tickets<MODE>(ectl, counts, offsets, max_out, t_begin, t_end,
+      [&](unsigned long long t, EnumTicket &tk, unsigned long long &feasible) {
+    const uint64_t dealt = dealt_item(t, part, nparts);
+    if (dealt < total) {
+      int pre[P];
+      uint64_t base_rank;
+      unrank_prefix_warp<P, K, true>(dealt, n, pre, base_rank, lane);
+      bool rejected = false;
+#pragma unroll
+      for (int i = 0; i < P; i++) rejected |= (pre[i] < 8) && ((inmask >> pre[i]) & 1u);
+      int pre_deep = 0;   // prefix gates of depth B - 1 (at most one gate of a match may have it)
+      if constexpr (FILTER) {
+#pragma unroll
+        for (int i = 0; i < P; i++) {
+          rejected |= s_dep[pre[i]] >= B;
+          pre_deep += s_dep[pre[i]] >= B - 1;
+        }
+        rejected |= pre_deep > 1;
+      }
+      const int last = pre[P - 1];
+      const uint32_t R = rejected ? 0u : (uint32_t)(n - last - 1);
+      uint32_t mixed = 0;
+      if (R != 0) {
+        // prefix cell `lane` (first prefix gate = most significant bit), kept if mixed
+        bool mx = false;
+        if (lane < NC) {
+          uint32_t ones = 0, zeros = 0;
+#pragma unroll
+          for (int w = 0; w < NW; w++) {
+            uint32_t tt = M[w];
+#pragma unroll
+            for (int i = 0; i < P; i++) {
+              const uint32_t tv = s_tabs[w * npad + pre[i]];
+              tt &= ((lane >> (P - 1 - i)) & 1) ? tv : ~tv;
+            }
+            cells[lane * 2 * NW + w] = tt & T[w];
+            cells[lane * 2 * NW + NW + w] = tt & ~T[w];
+            ones |= tt & T[w];
+            zeros |= tt & ~T[w];
+          }
+          mx = ones != 0 && zeros != 0;
+        }
+        mixed = __ballot_sync(kFull, mx);
+        __syncwarp();
+      }
+      bool done = false;
+      for (uint32_t q0 = 0; q0 < R && !done; q0 += 32) {
+        const uint32_t q = q0 + lane;
+        bool alive = q < R;
+        const int gd = last + 1 + (int)q;
+        if (gd < 8 && ((inmask >> gd) & 1u)) alive = false;
+        if constexpr (FILTER) {
+          if (alive) {
+            const int dd = s_dep[gd];
+            alive = dd < B && pre_deep + (dd >= B - 1) <= 1;
+          }
+        }
+        for (uint32_t mc = mixed; mc != 0 && alive; mc &= mc - 1) {
+          const int cj = __ffs(mc) - 1;
+          uint32_t a1 = 0, a0 = 0, b1 = 0, b0 = 0;
+#pragma unroll
+          for (int w = 0; w < NW; w++) {
+            const uint32_t td = s_tabs[w * npad + gd];
+            const uint32_t c1 = cells[cj * 2 * NW + w], c0 = cells[cj * 2 * NW + NW + w];
+            a1 |= c1 & td; b1 |= c0 & td;
+            a0 |= c1 & ~td; b0 |= c0 & ~td;
+          }
+          if ((a1 && b1) || (a0 && b0)) alive = false;
+        }
+        for (uint32_t fb = __ballot_sync(kFull, alive); fb != 0 && !done; fb &= fb - 1) {
+          const int src = __ffs(fb) - 1;
+          const int g4[4] = {pre[0], pre[1], pre[2], __shfl_sync(kFull, gd, src)};
+          feasible++;
+          [[maybe_unused]] SizeWalkOf<MODE> sw;
+          for (int k = 0; k < 12 && !done; k++) {
+            int g5[5];
+#pragma unroll
+            for (int i = 0; i < 5; i++) g5[i] = g4[c_rows4s[k][i]];
+            int kd = 0;
+            if constexpr (FILTER) {
+              int d5[5];
+#pragma unroll
+              for (int i = 0; i < 5; i++) d5[i] = s_dep[g5[i]];
+              kd = depth5(d5, 0);
+              if (kd > B) continue;
+            }
+            uint32_t H1, H0;
+            summary5<NW>(s_tabs, npad, g5, T, M, lane, H1, H0);
+            uint32_t ok[8], surv_mine = 0;
+            uint32_t rr[8];
+            if constexpr (FILTER) outer_ok5_rr(H1, H0, 0, lane, tab, ok, rr);
+            else outer_ok5(H1, H0, 0, lane, tab, ok);
+            uint32_t c = 0;
+#pragma unroll
+            for (int hi = 0; hi < 8; hi++) {
+              uint32_t surv = ok[hi] & __brev(ok[7 - hi]);
+              if constexpr (FILTER) {
+                surv &= s_fn[hi];
+                if (!inner_all) {
+                  const uint32_t rr0 = __shfl_sync(kFull, rr[7 - hi], 31 - lane);
+                  surv &= __ballot_sync(kFull, inner_ok5(s_fn, rr[hi], rr0));
+                }
+              }
+              if constexpr (GR && MODE != kEnumSizes) c |= surv;   // only whether the set is empty
+              else c += __popc(surv);
+              if (lane == hi) surv_mine = surv;
+            }
+            if constexpr (MODE == kEnumSizes) {
+              if (sw.sizing) {
+                sw.size += c;
+                continue;
+              }
+              if (c == 0) continue;
+              sw.size = c;
+              if (flt.grouping == kGroupTuple && size_wanted(tk)) {
+                sw.sizing = true;   // the combination's later rows add to it; its step follows them
+                continue;
+              }
+              done = emit_step<MODE>(lane == 0, tk, [&](unsigned long long s) {
+                ectl->sizes[s] = sw.size;
+              });
+              if (flt.grouping == kGroupTuple) break;
+              continue;
+            }
+            if constexpr (GR) {
+              if (MODE == kEnumCount) {
+                if (c == 0) continue;
+                tk.count++;
+                if (flt.hist_on && lane == 0) hist_add(kd, 1);
+                if (flt.grouping == kGroupTuple) break;
+                continue;
+              }
+            }
+            if (MODE == kEnumCount) {
+              tk.count += c;
+              if constexpr (FILTER) {
+                if (flt.hist_on && lane == 0 && c != 0) hist_add(kd, c);
+              }
+              continue;
+            }
+            if (c == 0) continue;
+            // positions in ascending order: lane takes position 32 * w + lane
+            const unsigned long long key_hi = ((base_rank + q0 + src) << 12) | ((uint64_t)k << 8);
+#pragma unroll 1
+            for (int w = 0; w < 8; w++) {
+              const uint32_t pos = 32u * w + lane;
+              const uint32_t fo = s_ord[pos];
+              bool hit = (__shfl_sync(kFull, surv_mine, fo >> 5) >> (fo & 31u)) & 1u;
+              if constexpr (GR) {
+                // the group's record: its lowest position with a hit
+                const uint32_t bal = __ballot_sync(kFull, hit);
+                if (bal == 0) continue;
+                hit = hit && (bal & lanemask_lt()) == 0;
+                done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
+                  write_match<NW, 5, kShapeShared>(out + i, key_hi | pos, g5, 0, fo, 0, s_tabs,
+                      npad, T, M);
+                });
+                break;
+              }
+              done = emit_step<MODE>(hit, tk, [&](unsigned long long i) {
+                write_match<NW, 5, kShapeShared>(out + i, key_hi | pos, g5, 0, fo, 0, s_tabs, npad,
+                    T, M);
+              });
+            }
+            if constexpr (GR) {
+              if (flt.grouping == kGroupTuple) break;
+            }
+          }
+          if constexpr (MODE == kEnumSizes) {
+            if (sw.sizing) {
+              done = emit_step<MODE>(lane == 0, tk, [&](unsigned long long s) {
+                ectl->sizes[s] = sw.size;
+              });
+            }
+          }
+        }
+      }
+    }
+  });
+  flush_hist<MODE, FORM>(flt);
+}
+
+template <int NW, int MODE, int FORM>
+__global__ void __launch_bounds__(kThreads) k_enum4s(const DevProblem *__restrict__ prob,
+    EnumCtl *__restrict__ ectl, const EnumOrders ord, uint32_t *__restrict__ counts,
+    const unsigned long long *__restrict__ offsets, DevMatch *__restrict__ out,
+    unsigned long long max_out, unsigned long long t_begin, unsigned long long t_end, int part,
+    int nparts, const DevTables *__restrict__ tab, const EnumFilterOf<FORM> flt) {
+  enum4s_body<NW, MODE, FORM>(prob, ectl, ord, counts, offsets, out, max_out, t_begin, t_end,
       part, nparts, tab, flt);
 }
 

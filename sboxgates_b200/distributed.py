@@ -265,6 +265,13 @@ class DistributedLutSearch:
                                                                  nparts),
             max_matches)
 
+    def enumerate4_shared(self, order, max_matches):
+        """The shared-input two-LUT realisations (LutEngine.enumerate4_shared), over every
+        4-combination: no list is installed, and `feasible` is summed over the ranks."""
+        return self._enumerate(
+            lambda k, part, nparts: self.engine.enumerate4_shared(order, k, True, part, nparts),
+            max_matches)
+
     def fetch_matches(self, first, count):
         """The whole's matches at ranks first .. min(first + count, total) - 1 (the last
         enumerate* call's), the same on every rank."""

@@ -16,7 +16,7 @@ from . import native
 from .native import (SbgResult, SbgJob, SbgNodeResult, NativeLibraryError, SBG_KEY_NONE,
                      SBG_LIST_CAP, SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7, MATCH_DTYPE,
                      SBG_ENUM_MAX_MATCHES, SBG_MAX_GATES, SBG_MAX_DEPTH, SBG_DEPTH_BINS,
-                     SBG_ENUM7_ALL_MAX_GATES, SBG_SHAPE_TREE, SBG_SHAPE_CHAIN)
+                     SBG_ENUM7_ALL_MAX_GATES, SBG_SHAPE_TREE, SBG_SHAPE_CHAIN, SBG_SHAPE_SHARED)
 
 NO_GATE = 0xFFFF  # state.h:30
 
@@ -108,6 +108,18 @@ def chain_row(k):
     row = (C.c_int * 7)()
     if lib.sbg_chain_row(int(k), row) != 0:
         raise ValueError("bad chain row %r" % (k,))
+    return [int(x) for x in row]
+
+
+def shared_row(k):
+    """Row k (0..11) of the shared-input two-LUT circuit L2(L1(a,b,c), u, v) (sbg_shared_row): the
+    4-combination's positions in record order a, b, c, u, v.  k = 3 j + q: j = the position of d,
+    the gate L1 does not read; q = the index of the shared gate s among L1's three positions;
+    (u, v) = {s, d} ascending."""
+    lib = native.load_library()
+    row = (C.c_int * 5)()
+    if lib.sbg_shared_row(int(k), row) != 0:
+        raise ValueError("bad shared-input row %r" % (k,))
     return [int(x) for x in row]
 
 
@@ -267,6 +279,15 @@ class LutEngine:
         res = SbgResult()
         self._check(self.lib.sbg_search7_chain(self._h, _order_ptr(outer_order),
                                                _order_ptr(middle_order), C.byref(res)))
+        return res
+
+    def search4_shared(self, func_order):
+        """The first shared-input two-LUT circuit L2(L1(a,b,c), u, v), {u, v} = {s, d} with s one
+        of a, b, c, over every 4-combination (sbg_search4_shared): an SbgResult laid out as a
+        search5 result (gates a, b, c, u, v; key rank << 12 | k << 8 | po, ordering = the
+        shared_row k), so result5_to_ret applies L2's fill to it."""
+        res = SbgResult()
+        self._check(self.lib.sbg_search4_shared(self._h, _order_ptr(func_order), C.byref(res)))
         return res
 
     # -- one call per node / batches of nodes --------------------------------------------------
@@ -439,6 +460,15 @@ class LutEngine:
         records of shape SBG_SHAPE_CHAIN (see chain_luts).  The installed list stays."""
         return self._enumerate(self.lib.sbg_enum7_chain, [outer_order, middle_order], max_matches,
                                count, part, nparts)
+
+    def enumerate4_shared(self, func_order, max_matches, count=True, part=0, nparts=1):
+        """The two-LUT realisations search_5lut never tries, L2(L1(a,b,c), u, v) with {u, v} =
+        {s, d} and s one of a, b, c (sbg_enum4_shared), over every 4-combination: keys rank << 12 |
+        k << 8 | po with k a shared_row and L1 = func_order[po], records of width 4 and shape
+        SBG_SHAPE_SHARED laid out as 5-LUT records (match_to_ret reads them).  The installed 7-LUT
+        list stays."""
+        return self._enumerate(self.lib.sbg_enum4_shared, [func_order], max_matches, count, part,
+                               nparts)
 
     def enumerate3(self, gate_order, max_matches, count=True, part=0, nparts=1):
         """Every match of lut_search's 3-LUT scan over `gate_order` (a permutation of the current
@@ -621,23 +651,28 @@ _GROUPINGS = {None: native.SBG_GROUP_NONE, "shape": native.SBG_GROUP_SHAPE,
               "tuple": native.SBG_GROUP_TUPLE}
 # the key bits below a group's id, per (grouping, width, wiring): positions (shape), then the row
 _GROUP_SHIFT = {("shape", 5, "tree"): 8, ("shape", 7, "tree"): 16, ("tuple", 5, "tree"): 12,
-                ("tuple", 7, "tree"): 23, ("shape", 7, "chain"): 16, ("tuple", 7, "chain"): 24}
+                ("tuple", 7, "tree"): 23, ("shape", 7, "chain"): 16, ("tuple", 7, "chain"): 24,
+                ("shape", 4, "shared"): 8, ("tuple", 4, "shared"): 12}
+# the wiring each width's records may have
+_SHAPES = {3: ("tree",), 4: ("shared",), 5: ("tree",), 7: ("tree", "chain")}
 
 
 def match_group(key, width, grouping, shape="tree"):
     """The id of the group an enumerated match's key belongs to under a grouping (see
     LutEngine.set_grouping): the key itself for None and for width 3, else key >> 8 / key >> 16
     (shape, 5- / 7-LUT) or key >> 12 / key >> 23 (tuple).  shape="chain" reads a key of
-    enumerate7_chain (width 7): key >> 16 (shape) or key >> 24 (tuple).  Matches of one group have
-    equal ids; groups come in ascending id order."""
+    enumerate7_chain (width 7): key >> 16 (shape) or key >> 24 (tuple); shape="shared" a key of
+    enumerate4_shared (width 4, the only width with that wiring): key >> 8 (shape) or key >> 12
+    (tuple), as a 5-LUT key.  Matches of one group have equal ids; groups come in ascending id
+    order."""
     if grouping not in _GROUPINGS:
         raise ValueError("grouping must be None, 'shape' or 'tuple', not %r" % (grouping,))
-    if width not in (3, 5, 7):
-        raise ValueError("width must be 3, 5 or 7")
-    if shape not in ("tree", "chain"):
-        raise ValueError("shape must be 'tree' or 'chain', not %r" % (shape,))
-    if shape == "chain" and width != 7:
-        raise ValueError("a chain is a 7-LUT wiring")
+    if width not in _SHAPES:
+        raise ValueError("width must be 3, 4, 5 or 7")
+    if shape not in ("tree", "chain", "shared"):
+        raise ValueError("shape must be 'tree', 'chain' or 'shared', not %r" % (shape,))
+    if shape not in _SHAPES[width]:
+        raise ValueError("width %d has no %r wiring" % (width, shape))
     key = int(key)
     if not 0 <= key < 2**64:
         raise ValueError("key must lie in 0..2**64-1")
@@ -667,17 +702,25 @@ def _trim(hist):
     return hist[:int(nz[-1]) + 1].copy() if nz.size else hist[:0].copy()
 
 
+def _is_shared(record):
+    """Whether a MATCH_DTYPE record is a shared-input pair (enumerate4_shared)."""
+    return int(record["width"]) == 4 and int(record["shape"]) == SBG_SHAPE_SHARED
+
+
 def match_depth(record, depth):
     """The depth of the gate an enumerated match (a MATCH_DTYPE record) would add, given the depth
     of every gate of the problem: 1 + max(Da, Db, Dc) for a 3-LUT; 1 + max(1 + max(Da, Db, Dc),
     Dd, De) for a 5-LUT (outer LUT over a, b, c); 1 + max(1 + max(Da, Db, Dc), 1 + max(Dd, De, Df),
     Dg) for a 7-LUT (outer over a, b, c, middle over d, e, f); 1 + max(1 + max(1 + max(Da, Db, Dc),
-    Dd, De), Df, Dg) for a 7-LUT chain (the record's shape).  Gates in the record's order."""
+    Dd, De), Df, Dg) for a 7-LUT chain (the record's shape); 1 + max(1 + max(Da, Db, Dc), Du, Dv)
+    for a shared-input pair (width 4; gates a, b, c, u, v, one repeated).  Gates in the record's
+    order."""
     width = int(record["width"])
-    d = [int(depth[int(g)]) for g in record["gates"][:width]]
+    shared = _is_shared(record)
+    d = [int(depth[int(g)]) for g in record["gates"][:5 if shared else width]]
     if width == 3:
         return 1 + max(d)
-    if width == 5:
+    if width == 5 or shared:
         return 1 + max(1 + max(d[:3]), d[3], d[4])
     if width == 7 and int(record["shape"]) == SBG_SHAPE_CHAIN:
         return 1 + max(1 + max(1 + max(d[:3]), d[3], d[4]), d[5], d[6])
@@ -698,17 +741,18 @@ def shallowest_matches(engine, width, orders, depth, max_matches, whole=False, s
     need not be its shallowest.  whole=True (width 7 only) searches every 7-combination
     (enumerate7_all) instead of the phase-1 list, so the result is the state's shallowest 7-LUT
     realisation, not the list's.  shape="chain" (width 7 only) takes the chain realisations of
-    enumerate7_chain, which always cover every 7-combination."""
-    if width not in (3, 5, 7):
-        raise ValueError("width must be 3, 5 or 7")
+    enumerate7_chain, which always cover every 7-combination; shape="shared" (width 4, orders
+    (func_order,)) the shared-input pairs of enumerate4_shared."""
+    if width not in _SHAPES:
+        raise ValueError("width must be 3, 4, 5 or 7")
     if whole and width != 7:
         raise ValueError("whole=True applies to width 7 only")
-    if shape not in ("tree", "chain"):
-        raise ValueError("shape must be 'tree' or 'chain', not %r" % (shape,))
-    if shape == "chain" and width != 7:
-        raise ValueError("shape='chain' applies to width 7 only")
-    name = ("enumerate7_chain" if shape == "chain" else "enumerate7_all" if whole
-            else "enumerate%d" % width)
+    if shape not in ("tree", "chain", "shared"):
+        raise ValueError("shape must be 'tree', 'chain' or 'shared', not %r" % (shape,))
+    if shape not in _SHAPES[width]:
+        raise ValueError("width %d has no %r wiring" % (width, shape))
+    name = ("enumerate7_chain" if shape == "chain" else "enumerate4_shared" if shape == "shared"
+            else "enumerate7_all" if whole else "enumerate%d" % width)
     run = getattr(engine, name)
     engine.set_depth_filter(depth, SBG_DEPTH_BINS - 1)
     run(*orders, 0)
@@ -799,9 +843,10 @@ def allowed_fill(func_inner, inner_seen, inner=None):
 def match_functions_allowed(record, outer=None, middle=None, inner=None):
     """The function filter's test on one enumerated match (a MATCH_DTYPE record), sets as for
     LutEngine.set_function_filter (None: all 256): func_outer in outer (5- and 7-LUT), func_middle
-    in middle (7-LUT), and allowed_fill finds an inner function."""
+    in middle (7-LUT), and allowed_fill finds an inner function.  A shared-input record (width 4)
+    is tested as a 5-LUT one: outer = L1, inner = L2."""
     width = int(record["width"])
-    if width not in (3, 5, 7):
+    if width not in (3, 5, 7) and not _is_shared(record):
         raise ValueError("not a match record (width %d)" % width)
     if width > 3 and outer is not None and int(record["func_outer"]) not in set(outer):
         return False
@@ -913,14 +958,17 @@ def search_7lut(engine, tables, target, mask, inbits, rng):
 def match_to_ret(match, rng):
     """One enumerated match (a record of Enumeration.matches) -> the reference's ret[10]
     (lut.c:202-211 / 453-462), the don't-care bits of the inner function filled from `rng` as
-    get_lut_function would fill them.  A 3-LUT match has no ret[10]: see match_to_lut3."""
+    get_lut_function would fill them.  A 3-LUT match has no ret[10]: see match_to_lut3.  A
+    shared-input match (enumerate4_shared, width 4) has search_5lut's layout [L1, L2, a, b, c, u,
+    v, 0, 0, 0], one of u, v repeating one of a, b, c: its LUTs are added as a 5-LUT result's are,
+    L1 over (a, b, c), then L2 over (L1, u, v)."""
     if int(match["width"]) == 3:
         raise ValueError("a 3-LUT match has no ret[10]; use match_to_lut3")
     if int(match["shape"]) == SBG_SHAPE_CHAIN:
         raise ValueError("a chain match has no ret[10] (search_7lut's wiring); use chain_luts")
     fi = _fill(match["func_inner"], match["inner_seen"], rng)
     gates = [int(g) for g in match["gates"]]
-    if int(match["width"]) == 5:
+    if int(match["width"]) == 5 or _is_shared(match):
         return [int(match["func_outer"]), fi] + gates[:5] + [0, 0, 0]
     return [int(match["func_outer"]), int(match["func_middle"]), fi] + gates
 
@@ -1041,6 +1089,18 @@ def enumerate_7lut_chain(engine, tables, target, mask, inbits, outer, middle, ma
     return engine.enumerate7_chain(outer, middle, max_matches, count, part, nparts)
 
 
+def enumerate_4lut_shared(engine, tables, target, mask, inbits, order, max_matches, count=True,
+                          part=0, nparts=1):
+    """The realisations by two LUTs whose L2 reads one of L1's inputs again, L2(L1(a,b,c), u, v)
+    with {u, v} = {s, d} and s one of a, b, c, which search_5lut never tries, over every feasible
+    4-combination under search_5lut's function order `order` (LutEngine.enumerate4_shared).
+    Consumes no RNG; match_to_ret applies the fill per match."""
+    if len(tables) < 4:
+        raise ValueError("the shared-input two-LUT circuits need at least 4 gates")
+    engine.load(tables, target, mask, inbits)
+    return engine.enumerate4_shared(order, max_matches, count, part, nparts)
+
+
 def enumerate_3lut(engine, tables, target, mask, inbits, gate_order, max_matches, count=True,
                    part=0, nparts=1):
     """Every realisation of the state by lut_search's 3-LUT scan over `gate_order` (an
@@ -1082,15 +1142,16 @@ class LutSearchResult:
     """What lut_search() would add to the graph (lut.c:489-631): `luts` = the add_lut calls in
     order, each (function, in1, in2, in3) with inputs either gate numbers or ("new", k) = the k-th
     LUT added by this call; `stage` = 3, 5, 7 or 0 (NO_GATE); `shape` = how a stage-7 result wires
-    its three LUTs: "tree" (search_7lut's) or "chain" (lut_search(..., chain=True))."""
+    its three LUTs: "tree" (search_7lut's) or "chain" (lut_search(..., chain=True)); a stage-5
+    result is "tree" (search_5lut's) or "shared" (lut_search(..., shared=True))."""
     stage: int
     luts: List[tuple] = field(default_factory=list)
     node: object = None
     shape: str = "tree"
 
 
-def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=True, allow7=True,
-               chain=False):
+def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=True, allow7=True, *,
+               shared=False, chain=False):
     """lut.c:489-631 as ONE device call: the 3-LUT scan over the caller's shuffled gate order
     (lut.c:501-523), search_5lut (lut.c:553) and search_7lut (lut.c:593), each only if the earlier
     ones found nothing.  allow5 / allow7 = check_num_gates_possible(st, 2 / 3) (lut.c:525, 582).
@@ -1100,6 +1161,15 @@ def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=Tru
     (LutEngine.search7_chain), returned as stage 7 with shape "chain" and luts [(L1, a, b, c),
     (L2, ("new", 0), d, e), (L3, ("new", 1), f, g)].  A node without a chain gets exactly the result
     and RNG state of chain=False.
+
+    shared=True adds a stage the reference does not have between search_5lut and search_7lut: when
+    search_5lut ran and found nothing, the first two-LUT circuit whose L2 reads one of L1's inputs
+    again (LutEngine.search4_shared, under search_5lut's order), returned as stage 5 with shape
+    "shared" and luts [(L1, a, b, c), (L2, ("new", 0), u, v)].  search_7lut then does not run, so its
+    512 draws do not happen; the device call of the node stops after search_5lut, and search_7lut
+    is a call of its own (LutEngine.search7) when the stage finds nothing.  A node without a match
+    gets exactly the result and RNG state of shared=False, with or without chain.  Both switches
+    are keyword-only, so that a call cannot set one where it meant the other.
 
     RNG: the reference draws 256 values on entry to search_5lut and 512 before phase 2 of
     search_7lut, plus one per solved LUT with unseen cells (lut.c:104-106; the chain's L3 likewise).
@@ -1113,7 +1183,9 @@ def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=Tru
     if allow5 and allow7 and n >= 7:
         outer, middle = shuffled_orders7(ahead)
     engine.load(tables, target, mask, inbits)
-    node = engine.search_node(0, order5, outer, middle, gate_order)
+    staged = shared and order5 is not None   # search_7lut waits for the shared-input stage
+    node = engine.search_node(0, order5, None if staged else outer, None if staged else middle,
+                              gate_order)
     if node.found_stage == 3:
         fi = node.func3
         if node.seen3 != 0xFF:
@@ -1127,18 +1199,25 @@ def lut_search(engine, tables, target, mask, inbits, gate_order, rng, allow5=Tru
     if node.found_stage == 5:
         r = result5_to_ret(node.r5, rng).ret
         return LutSearchResult(5, [(r[0], r[2], r[3], r[4]), (r[1], ("new", 0), r[5], r[6])], node)
+    if staged:
+        res = engine.search4_shared(order5)
+        if res.found:
+            r = result5_to_ret(res, rng).ret
+            return LutSearchResult(5, [(r[0], r[2], r[3], r[4]), (r[1], ("new", 0), r[5], r[6])],
+                                   node, shape="shared")
     if outer is None:
         return LutSearchResult(0, [], node)
     for _ in range(512):
         rng.next()
-    if node.found_stage == 7:
-        r = result7_to_ret(node.r7, rng).ret
+    r7 = engine.search7(outer, middle) if staged else node.r7
+    if r7.found:
+        r = result7_to_ret(r7, rng).ret
         # lut.c:622-624 nests the outer and middle add_lut calls as arguments of the third; gcc
         # evaluates them right to left, so the MIDDLE LUT is added first (lower gate number)
         return LutSearchResult(7, [(r[1], r[6], r[7], r[8]), (r[0], r[3], r[4], r[5]),
                                    (r[2], ("new", 1), ("new", 0), r[9])], node)
     if chain:
-        # the engine still holds this node's list (search_node installed it)
+        # the engine still holds this node's list (search_node or search7 installed it)
         res = engine.search7_chain(outer, middle)
         if res.found:
             luts = [(f,) + ins for f, ins in chain_result_luts(res, rng)]

@@ -62,7 +62,8 @@ SBG_GROUP_NONE = 0        # enumeration groupings (sbg_enum_set_grouping): every
 SBG_GROUP_SHAPE = 1       #   one per (gates, ordering row),
 SBG_GROUP_TUPLE = 2       #   one per gate set
 SBG_SHAPE_TREE = 0        # a 7-LUT record's wiring (sbg_match::shape): L3(L1(a,b,c), L2(d,e,f), g),
-SBG_SHAPE_CHAIN = 1       #   or L3(L2(L1(a,b,c), d, e), f, g) (sbg_enum7_chain)
+SBG_SHAPE_CHAIN = 1       #   or L3(L2(L1(a,b,c), d, e), f, g) (sbg_enum7_chain);
+SBG_SHAPE_SHARED = 2      # a width-4 record: L2(L1(a,b,c), u, v), u or v one of a, b, c (sbg_enum4_shared)
 
 SBG_DO_SCAN3, SBG_DO_SEARCH5, SBG_DO_SEARCH7 = 1, 2, 4
 SBG_LANES = 8
@@ -99,6 +100,7 @@ SIGNATURES = {
     "sbg_search5": (C.c_int, [C.c_void_p, u8p, C.POINTER(SbgResult)]),
     "sbg_search7": (C.c_int, [C.c_void_p, u8p, u8p, C.POINTER(SbgResult)]),
     "sbg_search7_chain": (C.c_int, [C.c_void_p, u8p, u8p, C.POINTER(SbgResult)]),
+    "sbg_search4_shared": (C.c_int, [C.c_void_p, u8p, C.POINTER(SbgResult)]),
     "sbg_search5_part": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u64p]),
     "sbg_finish5": (C.c_int, [C.c_void_p, C.c_uint64, u8p, C.POINTER(SbgResult)]),
     "sbg_filter7_part": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u64p, C.POINTER(C.c_int)]),
@@ -107,6 +109,7 @@ SIGNATURES = {
     "sbg_finish7": (C.c_int, [C.c_void_p, C.c_uint64, u8p, u8p, C.POINTER(SbgResult)]),
     "sbg_ordering_row": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "sbg_chain_row": (C.c_int, [C.c_int, C.POINTER(C.c_int)]),
+    "sbg_shared_row": (C.c_int, [C.c_int, C.POINTER(C.c_int)]),
     "sbg_solve_inner": (C.c_int, [u64p, u64p, u64p, u64p, u64p, u8p, u8p]),
     "sbg_lut_table": (None, [C.c_uint8, u64p, u64p, u64p, u64p]),
     "sbg_enum5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, C.c_uint64, C.c_void_p, u64p, u64p,
@@ -117,6 +120,8 @@ SIGNATURES = {
                                 u64p, u64p, u64p]),
     "sbg_enum7_chain": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, u8p, C.c_uint64, C.c_void_p,
                                   u64p, u64p, u64p]),
+    "sbg_enum4_shared": (C.c_int, [C.c_void_p, C.c_int, C.c_int, u8p, C.c_uint64, C.c_void_p, u64p,
+                                   u64p, u64p]),
     "sbg_enum3": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint16), C.c_uint64,
                             C.c_void_p, u64p, u64p, u64p]),
     "sbg_enum_fetch": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, u64p]),
